@@ -1,4 +1,4 @@
-"""acco_b200 - a Blackwell (B200, sm_100a) native implementation of ACCO
+"""acco_b200 - a Hopper (H100, sm_90a) native implementation of ACCO
 ("Accumulate while you Communicate"), DPU and sharded-optimizer DDP training.
 
 Public API (same shape as the reference repo's, `trainer_decoupled.py:170-186`)::

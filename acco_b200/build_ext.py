@@ -1,8 +1,8 @@
-"""In-tree build of the sm_100a extension ``acco_b200/_C.so``.
+"""In-tree build of the sm_90a (Hopper, H100) extension ``acco_b200/_C.so``.
 
-Explicit ``nvcc`` / ``g++`` invocations (no JIT cache under ``~/.cache``: the built ``.so`` must sit
-in the tree so it travels to the GPU box).  Every ``.cu`` is compiled with
-``-gencode arch=compute_100a,code=sm_100a -lineinfo`` - sm_100a only, no fallback architectures.
+Explicit ``nvcc`` / ``g++`` invocations (no JIT cache under ``~/.cache``: the built ``.so`` sits in the
+tree, next to the package that loads it).  Every ``.cu`` is compiled with
+``-gencode arch=compute_90a,code=sm_90a -lineinfo`` - sm_90a only, no fallback architectures.
 Objects are cached in ``acco_b200/_build`` and rebuilt when a source or header is newer.
 """
 from __future__ import annotations
@@ -20,7 +20,7 @@ SRC = os.path.join(PKG, "csrc")
 OBJ = os.path.join(PKG, "_build")
 OUT = os.path.join(PKG, "_C.so")
 
-NVCC_ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "--use_fast_math", "-Xcompiler", "-fPIC", "-Xptxas", "-v",
               "--expt-relaxed-constexpr"]
 
@@ -88,7 +88,7 @@ def build(verbose: bool = True, force: bool = False) -> str:
                          cpp_o[:-2] + ".log"))
     if jobs:
         if verbose:
-            print(f"[acco_b200.build] compiling {len(jobs)} translation unit(s) for sm_100a ...", flush=True)
+            print(f"[acco_b200.build] compiling {len(jobs)} translation unit(s) for sm_90a ...", flush=True)
         with cf.ThreadPoolExecutor(max_workers=min(len(jobs), os.cpu_count() or 4)) as ex:
             list(ex.map(lambda j: _run(*j), jobs))
     if jobs or force or not os.path.exists(OUT):

@@ -1,7 +1,7 @@
 """Checkpoint files: atomic writes, discovery of the latest complete checkpoint, elastic re-sharding of the optimizer state.
 
 The reference only ever *saves* ``model.state_dict()`` (`/root/reference/trainer_decoupled.py:559-574,593-598`; the optimizer
-save is commented out and nothing can be loaded back, SURVEY section 5 "Checkpoint / resume").  Layout kept from it::
+save is commented out and nothing can be loaded back).  Layout kept from it::
 
     checkpoints/{id_run}_model_{count_grad_tot}.pt      periodic (every >= save_interval_s), HF parameter names
     checkpoints/{id_run}_model.pt                       final      (``dpu_model`` / ``_ddp_model`` variants)

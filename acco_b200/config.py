@@ -3,7 +3,7 @@
 The reference composes ``config/config.yaml`` + one file from each of the groups
 ``data/ train/ model/`` with Hydra (`main.py:25`, `config/config.yaml:2-5`) and passes
 ``cfg.train`` whole as the trainer's ``args`` (`main.py:60`).  Hydra/omegaconf are not
-installed on the (offline) B200 image, so this module re-implements the subset that the
+installed on the (offline) GPU image, so this module re-implements the subset that the
 reference relies on, on top of PyYAML:
 
 * ``defaults:`` list of ``{group: option}`` entries -> ``<config_dir>/<group>/<option>.yaml``

@@ -1,4 +1,4 @@
-// Python bindings (torch extension) for the acco_b200 sm_100a kernels.  Kernels live in plain .cu
+// Python bindings (torch extension) for the acco_b200 sm_90a kernels.  Kernels live in plain .cu
 // files with C launchers (no torch headers there, so they compile in seconds); this file only
 // validates tensors, allocates outputs and forwards raw pointers on the current CUDA stream.
 #include <torch/extension.h>
@@ -295,10 +295,8 @@ void ce_bwd_inplace(torch::Tensor logits, torch::Tensor labels, torch::Tensor ls
 int default_grid(int mode, long long slice) {
     const long long vec = slice / 8;
     long long want = (vec + 255) / 256;
-    // comm round: ONE CTA per SM.  NVLS: 256 threads x 64 registers = 16 K registers, exactly what a 384 x 128-register tcgen05 GEMM
-    // CTA leaves free, so GEMMs keep launching beside the round (measured at 8 GPUs: with two round CTAs per SM every GEMM waited
-    // for the round to drain - Llama-1B batch 1: 16.1 ms/step instead of ~11.5); 148 x 256 threads x 2 vectors in flight is still
-    // ~20x the bandwidth-delay product of the NVLS path.
+    // comm round: ONE CTA per SM (256 threads x 64 registers).  A GEMM CTA fills its SM's register file, so round CTAs run on the SMs
+    // no GEMM CTA holds; more than one per SM would not add bandwidth on the NVLS path.
     long long cap = mode == 0 ? (long long)sm_count() * 4 : (long long)sm_count();
     if (want < 1) want = 1;
     return (int)std::min(want, cap);
@@ -381,7 +379,7 @@ void rs_adam_ag(std::vector<int64_t> acc_ptrs, std::vector<int64_t> theta_ptrs, 
     TORCH_CHECK(acco_rs_adam_ag(&P, grad_bf16, out_bf16, (int)mode, g, stream()) == 0, "rs_adam_ag launch failed");
 }
 
-// ---------------------------------------------------------------- tcgen05 GEMM (+ fused weight all-gather)
+// ---------------------------------------------------------------- wgmma GEMM (+ fused weight all-gather)
 // y[M,N] = x[M,K] @ w[N,K]^T.  With `peer_ptrs` (address of W on every rank), `tile_owner` (int32 [ceil(N/256)]: -1 local,
 // r = pull from rank r), `flags` (uint32 [ceil(N/256)*ceil(K/64)*2]) and `state` (int32[2]: epoch, done counter) the weight
 // tiles owned by other ranks are gathered over NVLink inside the GEMM and written through to `w`.
@@ -421,9 +419,9 @@ torch::Tensor gemm_tn(torch::Tensor x, torch::Tensor w, std::vector<int64_t> pee
     return y;
 }
 
-// General tcgen05 GEMM:  out[M,N] (+)= A * B^T (+ bias).
+// General wgmma GEMM:  out[M,N] (+)= A * B^T (+ bias).
 //   a: [M,K] (a_mn = false, K contiguous) or [K,M] (a_mn = true);   b: [N,K] (b_mn = false) or [K,N] (b_mn = true)
-//   rows may be strided (stride(0) % 8 == 0, stride(1) == 1).  accumulate: out += (TMA reduce-add epilogue, split-K allowed).
+//   rows may be strided (stride(0) % 8 == 0, stride(1) == 1).  accumulate: out += (adding epilogue, split-K allowed).
 torch::Tensor gemm(torch::Tensor a, torch::Tensor b, c10::optional<torch::Tensor> out, c10::optional<torch::Tensor> bias, bool a_mn, bool b_mn,
                    bool accumulate, int64_t bn, int64_t splits, int64_t pm, int64_t pn, int64_t msub, int64_t max_ctas) {
     auto ok2d = [](const torch::Tensor& t) {
@@ -458,7 +456,7 @@ torch::Tensor gemm(torch::Tensor a, torch::Tensor b, c10::optional<torch::Tensor
     return y;
 }
 
-// heuristic's pick for a shape: {bn, splits, pm, pn, msub}
+// heuristic's pick for a shape: {bn, splits, pm, pn, rows per CTA / 128}
 std::vector<int64_t> gemm_choose(int64_t M, int64_t N, int64_t K, bool a_mn, bool b_mn, bool accumulate) {
     int o[5] = {0, 0, 0, 0, 0};
     acco_gemm_choose((int)M, (int)N, (int)K, a_mn ? 1 : 0, b_mn ? 1 : 0, accumulate ? 1 : 0, sm_count(), o);
@@ -479,11 +477,11 @@ int64_t gemm_max_clusters(int64_t cl) { return acco_gemm_max_clusters((int)cl, s
 int64_t num_sms() { return sm_count(); }
 
 // Experimental (ACCO_CARVEOUT_ALL=1): make "large shared memory" the device-wide default L1 / shared split, so that kernels without an
-// explicit preference (elementwise, norms, CE, ATen, cuDNN) use the same carve-out as the tcgen05 GEMMs and the round kernel and can
+// explicit preference (elementwise, norms, CE, ATen, cuDNN) use the same carve-out as the wgmma GEMMs and the round kernel and can
 // share an SM with them (an SM is only re-partitioned when idle: tools/coresidency_check.py).  Returns the CUDA error code.
 int64_t prefer_shared_carveout() { return (int64_t)cudaDeviceSetCacheConfig(cudaFuncCachePreferShared); }
 
-// ---------------------------------------------------------------- tcgen05 flash attention (experimental, opt-in: ACCO_ATTN=tcgen05)
+// ---------------------------------------------------------------- flash attention (opt-in: ACCO_ATTN=own)
 bool attn_supported(int64_t B, int64_t S, int64_t Hq, int64_t Hk, int64_t D, double scale) {
     return acco_attn_supported((int)B, (int)S, (int)Hq, (int)Hk, (int)D, (float)scale) != 0;
 }

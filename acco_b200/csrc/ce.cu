@@ -1,7 +1,7 @@
 // Softmax cross-entropy over bf16 logits [T, Vp] with `V <= Vp` valid columns (the rest is LM-head
 // alignment padding), HF semantics: rows whose label == ignore_index contribute nothing, loss is
 // the mean over the remaining rows (loss_utils.py:45-67).  No fp32 copy of the logits is ever made
-// (the reference up-casts all 8x1024x50257 logits to fp32 = 1.5 GiB, SURVEY K19).
+// (the reference up-casts all 8x1024x50257 logits to fp32 = 1.5 GiB).
 //
 //   ce_fwd : one CTA per row, ONE streaming pass (online max/sum in fp32) -> lse[row], row_loss[row]
 //   ce_reduce : deterministic tree over rows -> loss (mean) and inv_n = 1 / #valid rows

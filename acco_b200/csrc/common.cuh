@@ -1,4 +1,4 @@
-// Shared device helpers for the acco_b200 sm_100a kernels.
+// Shared device helpers for the acco_b200 sm_90a kernels.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

@@ -193,7 +193,7 @@ extern "C" int acco_swiglu_bwd(const void* dout, const void* gu, void* dgu, long
 }
 
 // ---- debug: an SM "occupier" with the resource footprint of the NVLS round kernel (256 threads x 64 registers, no dynamic smem),
-// one CTA per SM, spinning for `ns` nanoseconds.  tools/coresidency_check.py launches it next to the tcgen05 GEMMs to see whether
+// one CTA per SM, spinning for `ns` nanoseconds.  tools/coresidency_check.py launches it next to the wgmma GEMMs to see whether
 // the two kinds of CTA share an SM (ACCO's overlap depends on it).
 namespace acco {
 __global__ void __launch_bounds__(256, 4) occupy_kernel(unsigned long long ns, float* sink) {

@@ -1,6 +1,6 @@
 // RMSNorm / fused residual-add + RMSNorm, forward and backward, bf16 I/O with fp32 statistics.
 //
-// Replaces HF Llama's ~7 eager kernels per norm (modeling_llama.py:53-70; SURVEY K18).
+// Replaces HF Llama's ~7 eager kernels per norm (modeling_llama.py:53-70).
 // Layout: x [T, H] row-major bf16.  A row is owned by `tpr` consecutive threads (a multiple of
 // 32), each holding VPT 16-byte vectors of the row in registers as packed bf16, so every element
 // is read from HBM exactly once per pass; a CTA of 256..512 threads processes several rows at a

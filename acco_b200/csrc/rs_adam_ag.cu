@@ -9,7 +9,7 @@
 //
 // It replaces, per round, the reference's: all_reduce(count) + reduce_scatter_tensor + cast +
 // mul_(1/count) + ~17 foreach AdamW kernels + cast + all_gather_into_tensor + up to 7 clone/restore
-// copies (trainer_decoupled.py:67-126; SURVEY K1-K11) - with NO NCCL call on the path.
+// copies (trainer_decoupled.py:67-126K11) - with NO NCCL call on the path.
 //
 // Transport (chosen at launch):
 //   * NVLS multicast : `multimem.ld_reduce.add.acc::f32.v4.bf16x2` pulls the switch-reduced sum of all
@@ -72,7 +72,7 @@ ACCO_DEVINL uint32_t ld_acquire_sys(const uint32_t* p) {
     return v;
 }
 // Spin until *p >= epoch (wrap-safe).  Failure detection: a peer that never arrives (crashed / hung rank) would hang
-// this kernel - and with it the whole job - forever (the reference has the same property through NCCL, SURVEY section 5);
+// this kernel - and with it the whole job - forever (the reference has the same property through NCCL);
 // after `watchdog_s` seconds the kernel traps instead, which surfaces as a CUDA error on the host.
 ACCO_DEVINL void wait_flag(const uint32_t* p, uint32_t epoch, int watchdog_s) {
     unsigned long long t0 = 0;
@@ -243,12 +243,12 @@ __global__ void __launch_bounds__(32) round_gate_kernel(const __grid_constant__ 
     }
 }
 
-// NVLS rounds run as 256-thread x 64-register CTAs (16 K registers): one such CTA fits beside a 384 x 128-register tcgen05 GEMM CTA
-// on the same SM, so the round really overlaps the compute it hides behind instead of waiting for SMs to drain.
+// NVLS rounds run as 256-thread x 64-register CTAs (16 K registers), one per SM.  The wgmma GEMM CTA (384 threads x 168 registers)
+// takes the whole register file of its SM, so a round CTA and a GEMM CTA never share an SM: the round overlaps the compute only on
+// SMs that no GEMM CTA holds (between GEMMs, or when a GEMM's grid is smaller than the GPU).  How much overlap that leaves on 8 GPUs
+// is not measured.
 // kSmall (experimental, ACCO_ROUND_LOCAL_SMALL=1, local mode only): give the single-GPU round the NVLS variant's footprint (256
-// threads x <= 64 registers, one CTA per SM, max shared-memory carve-out) so that it can co-reside with the GEMM CTAs of the next
-// phase instead of taking turns with them (~0.6 ms of a 10.1 ms step at N = 1, ROADMAP item 1).  Not measured yet; the default
-// instantiations compile to the same SASS as before this parameter existed.
+// threads x <= 64 registers, one CTA per SM, max shared-memory carve-out).  Not measured; the default instantiations do not use it.
 template <int MODE, bool kSmall = false> constexpr int round_threads() { return (MODE == 2 || kSmall) ? 256 : kAdamThreads; }
 
 template <typename G, typename O, int MODE, bool kSmall = false>
@@ -399,9 +399,9 @@ __global__ void __launch_bounds__(round_threads<MODE, kSmall>(), (MODE == 2 || k
     }
 }
 
-// The round shares SMs with the tcgen05 GEMMs, which run with the maximum shared-memory carve-out (225.5 KiB per CTA).  An SM is only
+// The round shares SMs with the wgmma GEMMs, which run with the maximum shared-memory carve-out.  An SM is only
 // re-partitioned between L1 and shared memory when it is idle, so a kernel that prefers another carve-out can never be co-resident with
-// them - it waits for the SM to drain (measured with tools/coresidency_check.py: GEMMs and a default-carve-out CTA take turns).
+// them - it waits for the SM to drain (tools/coresidency_check.py checks this).
 // Ask for the same configuration.
 template <typename G, typename O, int MODE>
 static void prefer_max_smem_carveout() {

@@ -5,7 +5,7 @@
 * :class:`PadCollator` - ragged SFT batches: right-pad to the longest row, emit ``attention_mask``
   and ``labels`` with pad positions set to -100.  With ``pad == eos`` (the reference sets
   ``tokenizer.pad_token_id = eos_token_id``, `main.py:46`) HF's
-  ``DataCollatorForLanguageModeling(mlm=False)`` masks *every* EOS label (SURVEY Q11); that is
+  ``DataCollatorForLanguageModeling(mlm=False)`` masks *every* EOS label ; that is
   reproduced with ``mask_all_pad_tokens=True`` (default) and can be switched off.
 """
 from __future__ import annotations

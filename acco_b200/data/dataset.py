@@ -2,7 +2,7 @@
 reference relies on (`trainer_base.py:100-124,193-200`, `main.py:49-50`): ``column_names``,
 ``shard(num_shards, index)``, ``map(fn, batched=True, remove_columns=..., num_proc=...)``,
 ``train_test_split(test_size, seed)``, ``save_to_disk`` / ``load_from_disk``.  Real HF datasets
-are accepted everywhere too; this class exists because the B200 box is offline."""
+are accepted everywhere too; this class exists because the GPU machines are offline."""
 from __future__ import annotations
 
 import os

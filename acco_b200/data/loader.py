@@ -1,7 +1,7 @@
 """Batch loading: random sampling with ``drop_last`` (`trainer_base.py:203-218`), an *endless*
 iterator that restarts epochs (`trainer_decoupled.py:386-397`), pinned staging buffers and an
 asynchronous host->device copy on a side stream (the reference does a synchronous ``.to()`` per
-micro-batch, SURVEY K21).
+micro-batch).
 
 The producer is a background thread (collation of in-memory token rows is cheap and releases the
 GIL inside numpy/torch); it keeps ``prefetch`` batches ahead, each already resident in pinned

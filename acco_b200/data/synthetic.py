@@ -1,10 +1,10 @@
-"""Synthetic corpora shaped like the reference's two datasets (the B200 box is offline, so
+"""Synthetic corpora shaped like the reference's two datasets (the GPU machines are offline, so
 ``datasets.load_dataset`` of `config/data/*.yaml` cannot run):
 
 * **openwebtext-shaped** pre-training documents: ragged token sequences with a heavy-tailed
   length distribution (mean ~900 tokens), meant for const-len packing;
 * **alpaca-shaped** SFT samples: short ragged prompt+response rows (mean ~180 tokens) that are
-  padded per batch (labels -100 on pad/EOS, SURVEY Q11).
+  padded per batch (labels -100 on pad/EOS).
 
 Token ids follow a Zipf-like marginal with a first-order Markov dependency so the LM loss can
 actually decrease (tests assert it does).  Documents are already token ids (``input_ids``

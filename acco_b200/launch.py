@@ -6,11 +6,11 @@ Here three launchers are recognised, in this order:
 1. **torchrun / torch.distributed.run** – ``RANK, LOCAL_RANK, WORLD_SIZE, MASTER_ADDR, MASTER_PORT``
 2. **Slurm ``srun``** – ``SLURM_PROCID, SLURM_LOCALID, SLURM_NTASKS, SLURM_JOB_NODELIST, SLURM_STEP_GPUS``
    (same derivation as the reference: master = first expanded host, port = 12346 + min GPU id,
-   but the min is numeric – the reference takes a *string* min, SURVEY Q12)
+   but the min is numeric – the reference takes a *string* min)
 3. **single process** – world of 1 (no env needed).
 
 One process drives one GPU.  The backend is ``nccl`` on CUDA and ``gloo`` on CPU (plumbing
-tests, BASELINE config 1).
+tests).
 """
 from __future__ import annotations
 

@@ -6,11 +6,11 @@ The reference's default pre-training model is ``GPTNeoForCausalLM`` built from
 (window 256) attention, **no 1/sqrt(d) scaling of QK^T** and fp32 eager attention
 (`transformers/models/gpt_neo/modeling_gpt_neo.py:105-130`), q/k/v projections without bias,
 tied LM head.  ``arch='gptneo'`` reproduces exactly that; ``arch='gpt2'`` is the same block
-with scaled, all-global attention (BASELINE config 1's "GPT-2 small").
+with scaled, all-global attention (benchmark configuration 1's "GPT-2 small").
 
-B200 layout (same recipe as the native Llama): activations are ``[T = B*S, H]`` row-major bf16; q/k/v are ONE fused
-``[3H, H]`` weight and one tcgen05 GEMM; biases are added in the GEMM epilogue; residual-add + LayerNorm, GELU-new and the
-softmax-CE are single sm_100a kernels (``ops.layernorm`` / ``ops.cross_entropy``); the vocabulary is padded to a multiple of
+GPU layout (same recipe as the native Llama): activations are ``[T = B*S, H]`` row-major bf16; q/k/v are ONE fused
+``[3H, H]`` weight and one wgmma GEMM; biases are added in the GEMM epilogue; residual-add + LayerNorm, GELU-new and the
+softmax-CE are single sm_90a kernels (``ops.layernorm`` / ``ops.cross_entropy``); the vocabulary is padded to a multiple of
 128 rows (50257 -> 50304; padded logits are masked inside the CE kernel and get zero gradient); wgrad GEMMs and the
 LayerNorm dw/db reductions accumulate straight into the flat gradient arena.  ``state_dict()`` / ``load_state_dict()`` speak
 HF GPT-Neo key names (``transformer.h.N.attn.attention.q_proj.weight`` ...) and un-padded shapes, so checkpoints interchange.

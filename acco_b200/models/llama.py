@@ -4,14 +4,14 @@ Role in the reference: the model is "whatever HF returns" (`main.py:33-41`; Llam
 finetuning configs, `README.md:76-82`), called as ``model(**inputs, labels=input_ids)`` with
 ``outputs[0]`` the loss (`trainer_decoupled.py:28-34`).  This implementation keeps that calling
 convention and the HF **checkpoint key names** (``model.layers.N.self_attn.q_proj.weight`` ...),
-but is laid out for the B200 path:
+but is laid out for the GPU kernel path:
 
 * activations are ``[T = B*S, H]`` row-major bf16 throughout; QKV and gate|up are single fused
   GEMMs (one weight each in the flat arena; split back to HF names only in ``state_dict()``);
 * the LM head / embedding is padded to a multiple of 128 rows so the logits GEMM has aligned
   leading dimensions (50257 -> 50304); padded columns are masked inside the fused CE kernel;
 * residual add + RMSNorm, RoPE (in place on the QKV buffer), SwiGLU and the softmax-CE are
-  single hand-written sm_100a kernels (``acco_b200/ops``); wgrad GEMMs accumulate directly into
+  single hand-written sm_90a kernels (``acco_b200/ops``); wgrad GEMMs accumulate directly into
   the flat gradient arena.
 """
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""Device-side timing and overlap accounting (the reference only has ``time.time()``, SURVEY 5).
+"""Device-side timing and overlap accounting (the reference only has ``time.time()``).
 
 :class:`CudaTimer` brackets a region with CUDA events on a stream and resolves lazily (no
 host sync at record time).  :class:`OverlapMeter` accumulates, per round, how long the compute

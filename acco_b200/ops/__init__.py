@@ -1,7 +1,7 @@
 """Hot ops.  Every op has two implementations with identical semantics:
 
-* a hand-written **sm_100a CUDA kernel** (``acco_b200/csrc/*.cu``, built in-tree into
-  ``acco_b200/_C.so`` by ``__graft_entry__.build()``) - the path that runs on a B200;
+* a hand-written **sm_90a CUDA kernel** (``acco_b200/csrc/*.cu``, built in-tree into
+  ``acco_b200/_C.so`` by ``__graft_entry__.build()``) - the path that runs on an H100;
 * a plain **PyTorch fp32 reference** (``*_ref`` functions) - the CPU path and the numerics oracle
   used by ``tests/``.
 
@@ -82,7 +82,7 @@ def have_ext() -> bool:
 
 
 def use_kernels(*tensors: torch.Tensor, bf16_only: bool = True) -> bool:
-    """True -> dispatch to the sm_100a kernels.  CUDA tensors without the extension are an
+    """True -> dispatch to the sm_90a kernels.  CUDA tensors without the extension are an
     error unless ``ACCO_ALLOW_FALLBACK=1``.  The activation kernels are bf16-only: fp32 CUDA
     tensors (``use_mixed_precision=False`` / fp32 DDP weights, not a hot configuration) take the
     PyTorch path."""
@@ -97,7 +97,7 @@ def use_kernels(*tensors: torch.Tensor, bf16_only: bool = True) -> bool:
     if os.environ.get("ACCO_ALLOW_FALLBACK") == "1":
         return False
     raise RuntimeError(
-        "acco_b200: CUDA tensors given but the sm_100a extension is not built/loaded "
+        "acco_b200: CUDA tensors given but the sm_90a extension is not built/loaded "
         f"({_EXT_ERR}). Build it with __graft_entry__.build() or set ACCO_ALLOW_FALLBACK=1.")
 
 

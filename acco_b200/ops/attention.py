@@ -5,11 +5,10 @@ The reference uses the HF attention dispatch (`modeling_llama.py:272`) or eager 
 (`modeling_gpt_neo.py:105-130`, including its missing 1/sqrt(d) scale and the 256-token local window on odd layers - both
 reproduced through ``scale`` / ``window``).
 
-``ACCO_ATTN=tcgen05`` switches the fused-QKV attention block to the repo's own tcgen05 flash-attention kernels
-(``csrc/attention_tcgen05.cu``: forward + backward, head_dim 64, S a multiple of 128).  EXPERIMENTAL: those kernels were written
-without GPU access and have not been executed yet - ``tools/attn_check.py`` is the bring-up harness, and
-:func:`attention_blockwise_ref` / :func:`attention_blockwise_bwd_ref` below are the executable specification of their schedule
-(CPU-tested against the fp32 reference)."""
+``ACCO_ATTN=own`` switches the fused-QKV attention block to the repo's own flash-attention kernels
+(``csrc/attention_wgmma.cu``: forward + backward on the tensor cores, head_dim 64, S a multiple of 128).  ``tools/attn_check.py``
+compares them with the fp32 reference, and :func:`attention_blockwise_ref` / :func:`attention_blockwise_bwd_ref` below give the
+reference semantics of their masking and bf16 rounding points (CPU-tested against the fp32 reference)."""
 from __future__ import annotations
 
 import math
@@ -83,12 +82,12 @@ def causal_attention(q, k, v, scale: Optional[float] = None, window: Optional[in
 
 
 def own_attention_enabled() -> bool:
-    """``ACCO_ATTN=tcgen05``: route the fused-QKV attention block through ``csrc/attention_tcgen05.cu`` (experimental)."""
-    return os.environ.get("ACCO_ATTN", "").lower() == "tcgen05"
+    """``ACCO_ATTN=own``: route the fused-QKV attention block through ``csrc/attention_wgmma.cu``."""
+    return os.environ.get("ACCO_ATTN", "").lower() == "own"
 
 
 # ----------------------------------------------------------------------------------------------
-# Executable specification of csrc/attention_tcgen05.cu: the same tiling (128 queries x 128 keys), the same order of operations
+# Executable specification of a blockwise flash attention: 128 queries x 128 keys per tile, the order of operations
 # (row max of the raw scores -> accumulate the PREVIOUS block's P V -> rescale -> exponentials of this block), the same masking
 # rule, the same places where values are rounded to bf16 (P, dS, outputs).  fp32 everywhere else.
 # ----------------------------------------------------------------------------------------------

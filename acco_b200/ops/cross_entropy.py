@@ -1,7 +1,7 @@
 """Softmax cross-entropy over (possibly vocab-padded) bf16 logits.
 
 HF up-casts the whole ``[B*S, V]`` logits tensor to fp32, shifts and runs log_softmax + nll
-(`transformers/loss/loss_utils.py:45-67`, SURVEY K19: 1.5 GiB of fp32 at 8x1024x50257).  Here
+(`transformers/loss/loss_utils.py:45-67`: 1.5 GiB of fp32 at 8x1024x50257).  Here
 forward is one streaming pass that keeps only ``lse[T]`` (online max/sum in fp32) and backward
 overwrites the logits buffer in place with ``(softmax - onehot) * scale`` (``csrc/ce.cu``).
 Columns ``>= valid_vocab`` (alignment padding of the LM head) are excluded from the softmax and

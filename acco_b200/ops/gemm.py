@@ -1,10 +1,10 @@
-"""Hand-written tcgen05 / TMEM / TMA GEMM (``csrc/gemm_tcgen05.cu``) - every contraction of the training step
+"""Hand-written wgmma / TMA GEMM (``csrc/gemm_wgmma.cu``) - every contraction of the training step
 (`trainer_decoupled.py:18-39`: the ``nn.Linear`` forward / dgrad / wgrad inside ``gradient_step``) - optionally fused
 with the all-gather of its weight operand (KERNEL B of the north star).
 
 ``gemm(a, b, ...)``            : ``out[M,N] (+)= A @ B^T (+ bias)`` with either operand K-major (``[rows, K]``) or
                                  MN-major (``[K, rows]``, i.e. a transposed view without a copy), ``accumulate=True``
-                                 = TMA reduce-add epilogue into ``out`` (beta = 1; split-K for small outputs).
+                                 = adding epilogue into ``out`` (beta = 1; split-K for small outputs).
 ``gemm_tn / gemm_nn / gemm_tt_acc`` : the forward / dgrad / wgrad specialisations used by ``ops.linear``.
 ``GatheredWeight`` + ``gemm_tn_gather(x, gw)`` : the forward GEMM where the row-blocks of ``w`` that live on
 other ranks (they own those slices of the flat arena and have just updated them) are pulled over NVLink
@@ -33,7 +33,7 @@ def _rowmajor(t: torch.Tensor) -> torch.Tensor:
 
 
 def gemm_supported(*mats: torch.Tensor) -> bool:
-    """Shapes the tcgen05 kernel takes: bf16 CUDA matrices whose row length is a multiple of 8 (16-byte TMA strides)."""
+    """Shapes the wgmma kernel takes: bf16 CUDA matrices whose row length is a multiple of 8 (16-byte TMA strides)."""
     return all(m.is_cuda and m.dtype == torch.bfloat16 and m.dim() == 2 and m.shape[1] % 8 == 0 and m.shape[0] > 0 for m in mats)
 
 
@@ -61,7 +61,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor = None, bias: torch
         return gemm_ref(a, b, out, bias, a_mn, b_mn, accumulate)
     y = load_ext(required=True).gemm(_rowmajor(a), _rowmajor(b), out, bias, bool(a_mn), bool(b_mn), bool(accumulate), int(bn), int(splits),
                                      int(pm), int(pn), int(msub), int(max_ctas))
-    count_launch("gemm_tcgen05")
+    count_launch("gemm")
     return y
 
 
@@ -120,5 +120,5 @@ class GatheredWeight:
 
 def gemm_tn_gather(x: torch.Tensor, w_local: torch.Tensor, gw: GatheredWeight, max_ctas: int = 0) -> torch.Tensor:
     out = load_ext(required=True).gemm_tn(x.contiguous(), w_local, gw.peer_ptrs, gw.tile_owner, gw.flags, gw.state, int(max_ctas))
-    count_launch("gemm_tcgen05_gather")
+    count_launch("gemm_gather")
     return out

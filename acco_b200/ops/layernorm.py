@@ -1,6 +1,6 @@
 """LayerNorm (weight + bias) and fused residual-add + LayerNorm, and GELU-new: the normalisation / activation of the
 GPT-2 / GPT-Neo family - the reference's default pre-training model (`/root/reference/main.py:39-41`,
-``config/model/gpt-neo-125M.json``; HF runs them as eager ATen ops, `modeling_gpt_neo.py`).  One sm_100a pass each
+``config/model/gpt-neo-125M.json``; HF runs them as eager ATen ops, `modeling_gpt_neo.py`).  One sm_90a pass each
 (``csrc/layernorm.cu``); dw / db are reduced deterministically and accumulated straight into the gradient arena."""
 from __future__ import annotations
 

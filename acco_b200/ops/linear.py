@@ -1,12 +1,12 @@
 """Linear layer with *fused gradient accumulation*.
 
 Autograd would materialise ``dW`` and then run a separate ``grad += dW`` pass over every weight
-(SURVEY K20).  When the weight's ``.grad`` already exists (it is a view of the flat gradient
+.  When the weight's ``.grad`` already exists (it is a view of the flat gradient
 arena) the wgrad GEMM accumulates straight into it (``beta = 1`` epilogue), and autograd sees
 ``None`` for the weight gradient.
 
-On CUDA bf16 all three contractions run on the hand-written tcgen05 kernel (``ops/gemm.py`` ->
-``csrc/gemm_tcgen05.cu``): forward TN (+ bias in the epilogue), dgrad with the weight as an MN-major B
+On CUDA bf16 all three contractions run on the hand-written wgmma kernel (``ops/gemm.py`` ->
+``csrc/gemm_wgmma.cu``): forward TN (+ bias in the epilogue), dgrad with the weight as an MN-major B
 operand, wgrad with both operands MN-major, split-K and a TMA reduce-add epilogue that adds straight
 into the arena view.  ``ACCO_GEMM=cublas`` switches back to the library GEMMs (A/B comparisons);
 shapes a TMA tensor map cannot describe (row length not a multiple of 8) and non-bf16 dtypes use the
@@ -22,10 +22,10 @@ import torch.nn.functional as F
 
 
 def _tc(*mats) -> bool:
-    """Route to the hand-written tcgen05 GEMM?"""
+    """Route to the hand-written wgmma GEMM?"""
     from . import use_kernels
     from .gemm import gemm_supported
-    if os.environ.get("ACCO_GEMM", "tcgen05") == "cublas":
+    if os.environ.get("ACCO_GEMM", "") == "cublas":
         return False
     return use_kernels(*mats) and gemm_supported(*mats)
 
@@ -104,7 +104,7 @@ def _linear_backward(ctx, dy):
         if ctx.accumulate and w.grad is not None:
             if acc_tc:
                 from .gemm import gemm_tt_acc
-                gemm_tt_acc(dy2, x2, w.grad)             # split-K + TMA reduce-add straight into the arena view
+                gemm_tt_acc(dy2, x2, w.grad)             # split-K adds straight into the arena view
             elif w.grad.dtype == dy2.dtype:
                 w.grad.addmm_(dy2.t(), x2)               # accumulate in the (library) GEMM epilogue
             else:
@@ -124,7 +124,7 @@ def _linear_backward(ctx, dy):
 
 
 class GatherLinearFn(torch.autograd.Function):
-    """Forward = KERNEL B (tcgen05 GEMM that all-gathers the remote row-blocks of ``weight`` over NVLink and
+    """Forward = KERNEL B (wgmma GEMM that all-gathers the remote row-blocks of ``weight`` over NVLink and
     writes them through to the local copy); backward = the usual dgrad (on the now complete local copy) and
     wgrad accumulation into the gradient arena."""
 

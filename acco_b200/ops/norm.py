@@ -1,7 +1,7 @@
 """RMSNorm and fused residual-add + RMSNorm (fp32 statistics, bf16 I/O).
 
 HF Llama computes the norm as ~7 eager kernels with an fp32 round trip
-(`transformers/models/llama/modeling_llama.py:53-70`, SURVEY K18); here forward is one pass
+(`transformers/models/llama/modeling_llama.py:53-70`); here forward is one pass
 (``csrc/norm.cu``) that also emits ``rstd`` for the backward, and the residual add of the
 surrounding block is folded in (``h = a + r; y = norm(h) * w``)."""
 from __future__ import annotations

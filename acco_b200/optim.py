@@ -2,7 +2,7 @@
 
 Reference: `trainer_decoupled.py:296-315` keeps ``params_opt`` (fp32 master copy of the rank's
 slice), its fp32 ``.grad`` and a ``torch.optim.AdamW(capturable=True)`` whose foreach step costs
-~17 kernel launches and ~10 passes over the shard (SURVEY K7), plus 1+3 shard-sized clones and
+~17 kernel launches and ~10 passes over the shard , plus 1+3 shard-sized clones and
 restores on every tentative round (K1, K2, K11).
 
 Here the state is four flat fp32 tensors of ``size_slice`` elements (``master, exp_avg, exp_avg_sq,
@@ -16,7 +16,7 @@ stash``) and an update is *one* pass described by :class:`AdamHyper`:
 
 which is exactly ``torch.optim.AdamW`` (decoupled weight decay, bias-corrected) - verified in
 ``tests/test_optim.py``.  :func:`adamw_shard_update_` below is the plain-PyTorch implementation
-(CPU / gloo path and numerics oracle for the sm_100a kernel in ``csrc/rs_adam_ag.cu``).
+(CPU / gloo path and numerics oracle for the sm_90a kernel in ``csrc/rs_adam_ag.cu``).
 """
 from __future__ import annotations
 

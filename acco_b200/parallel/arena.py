@@ -4,9 +4,9 @@ What the reference does (`trainer_base.py:284-331`, `trainer_decoupled.py:244-31
 one flat bf16 vector holds all parameters (every ``nn.Parameter.data`` is a view), one flat
 vector holds all gradients, a third ``com_buffer`` of ``ceil(N/W)*W`` elements carries grads out /
 weights in, and each rank owns an fp32 master copy of slice ``rank``.  Each round flip costs
-three full-model memory passes (``params<-com``, ``com<-grad``, ``grad<-0``; SURVEY K12-K15).
+three full-model memory passes (``params<-com``, ``com<-grad``, ``grad<-0``K15).
 
-B200-first redesign (no copies on the flip):
+GPU-first redesign (no copies on the flip):
 
 * ``theta[0], theta[1]`` - two full parameter buffers.  The model computes on ``theta[live]``
   while the communication round writes the *other* one; a flip re-points the parameter views.

@@ -1,7 +1,7 @@
 """Communication backends: one interface, three implementations.
 
 ==========  ===========================================================================
-``symm``    the product: ONE sm_100a kernel per round doing reduce-scatter (NVLS
+``symm``    the product: ONE sm_90a kernel per round doing reduce-scatter (NVLS
             ``multimem.ld_reduce`` / P2P loads straight out of the peers' gradient
             accumulators) + count exchange + scale + sharded AdamW (+ stash, commit flags) +
             all-gather push (``multimem.st`` / P2P stores into every peer's shadow parameter
@@ -11,7 +11,7 @@
             local AdamW kernel (or PyTorch ops), ``all_gather_into_tensor`` - the same call
             sequence as the reference's ``communication_step`` (`trainer_decoupled.py:67-126`),
             minus the clone/restore passes.
-``gloo``    same code as ``nccl`` on CPU tensors (plumbing tests, BASELINE config 1).
+``gloo``    same code as ``nccl`` on CPU tensors (plumbing tests).
 ==========  ===========================================================================
 
 A backend enqueues a whole *round* on the current stream (:meth:`launch_round`) and later
@@ -55,7 +55,7 @@ class CommBackend:
     # collectives -----------------------------------------------------------------------
     def init_sync(self, flat: torch.Tensor, mode: str = "broadcast") -> None:
         """Make every rank start from the same weights.  ``avg`` is the reference's behaviour
-        (`trainer_base.py:180`, SURVEY Q6); ``broadcast`` keeps rank 0's initialisation."""
+        (`trainer_base.py:180`); ``broadcast`` keeps rank 0's initialisation."""
         if self.world == 1:
             return
         if mode == "avg":

@@ -1,9 +1,8 @@
 """CUDA-graph capture of one micro-batch (forward + backward + loss read-out).
 
 The reference launches ~1.8 k eager kernels per micro-batch from Python and left
-``#@torch.compile`` / "static memory" stubs behind (`trainer_decoupled.py:17,199-200,386-397`;
-SURVEY section 0).  On B200 a 125M-parameter micro-batch is ~10 ms of GPU work, so launch
-overhead is first-order; here the whole micro-batch is captured once per
+``#@torch.compile`` / "static memory" stubs behind (`trainer_decoupled.py:17,199-200,386-397`).  A 125M-parameter micro-batch is a few tens of ms of GPU work
+split over ~1.5 k kernels, so launch overhead is first-order; here the whole micro-batch is captured once per
 ``(parameter buffer, gradient accumulator)`` pair - two graphs cover the ACCO double-buffer
 schedule - and replayed with a single ``cudaGraphLaunch``.  Gradients accumulate *inside* the
 graph into the flat arena (pointer-stable), inputs arrive in static device buffers filled by an

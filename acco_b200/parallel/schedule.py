@@ -1,7 +1,7 @@
 """Round state machine and LR schedules - the *semantics* of ACCO / DPU / DDP, with no
 tensors, streams or collectives in sight (so it is unit-testable and shared by every backend).
 
-Reference behaviour being reproduced (`trainer_decoupled.py:43-63, 67-126, 431-598`; SURVEY 3.2):
+Reference behaviour being reproduced (`trainer_decoupled.py:43-63, 67-126, 431-598`):
 rounds are numbered by ``count_after_init = 0, 1, 2, ...``.
 
 * **ACCO** - even rounds are *tentative*: the optimizer consumes the half-batch ``g~_t`` (grads
@@ -9,9 +9,7 @@ rounds are numbered by ``count_after_init = 0, 1, 2, ...``.
   (`:79-84, 113-121`).  Odd rounds are *real*: the optimizer consumes ``g~_t + g_t``, divides by
   the global micro-batch count, commits ``theta_{t+1}``, steps the LR scheduler (`:102-104`) and
   the global gradient counter advances (`:501-502`).
-* **DPU**  - every round commits, using gradients that are one round stale (SURVEY Q5: the
-  reference's implementation is sequential and re-uses some grads; this is the intended rule
-  ``theta_{t+1} = Opt(theta_t, g(theta_{t-1}))``, overlapped).
+* **DPU**  - every round commits, using gradients that are one round stale)``, overlapped).
 * **DDP**  - every round commits, synchronously, on fresh gradients (the reference pairs torch DDP
   with ZeroRedundancyOptimizer, `:226-241, 732-833`).
 
@@ -101,7 +99,7 @@ class RoundScheduler:
             if c % 2 == 0:
                 commit = COMMIT_NONE
                 if self.reference_quirks and c == 0:
-                    commit = COMMIT_STATE   # SURVEY Q1: round-0 state reset is a no-op in the reference
+                    commit = COMMIT_STATE   # round-0 state reset is a no-op in the reference
                 plan = RoundPlan(c, "tentative", read_acc, write_theta, commit, False, True, False, False, False)
             else:
                 plan = RoundPlan(c, "real", read_acc, write_theta, COMMIT_ALL, True, False, True, True, False)
@@ -197,8 +195,7 @@ def get_lr_lambda(name: str, num_warmup_steps: int, num_training_steps: int) -> 
 class LRSchedule:
     """``lr(k) = base_lr * lambda(k)`` where ``k`` counts scheduler steps.
 
-    ``unit='optimizer_step'`` reproduces the reference (SURVEY Q3: the LR moves once per *real*
-    optimizer step although the horizon ``nb_steps_tot`` is counted in micro-grads);
+    ``unit='optimizer_step'`` reproduces the reference;
     ``unit='grads'`` advances by the number of committed gradients (the authors' intent)."""
 
     base_lr: float

@@ -1,12 +1,12 @@
 """``DecoupledTrainer`` - ACCO / DPU / DDP training with a sharded optimizer.
 
-Public surface kept from the reference (`trainer_decoupled.py:170-186`, SURVEY 2.9): the
+Public surface kept from the reference (`trainer_decoupled.py:170-186`): the
 constructor keywords, ``.train()`` dispatching on ``args.method_name``, ``train_acco / train_dpu /
 train_ddp``, ``eval_loop``, ``warmup_steps``, ``get_weights / set_weights / get_grads / set_grads``,
 ``get_train_dataloader / get_eval_dataloader`` and the artefact layout (``tensorboard/``,
 ``checkpoints/{id_run}_model*.pt`` with HF key names, ``results.csv``).
 
-What is different underneath (see SURVEY 2.6/2.10 for what is being replaced):
+What is different underneath:
 
 * no Python communication thread, no ``mp.Barrier``: the main thread enqueues a whole round on a
   high-priority *communication stream* the moment the previous one has finished, and polls a CUDA
@@ -236,7 +236,7 @@ class DecoupledTrainer:
 
     # ---- read-only views under the reference's attribute names (`trainer_decoupled.py:170-315`), for code that inspects a trainer.
     # The thread machinery (`com_event`, `update_event`, `com_finished`) and `com_buffer` have no counterpart: there is no
-    # communication thread and no staging buffer (DESIGN section 2).
+    # communication thread and no staging buffer.
     @property
     def scheduler(self):
         """LR schedule object (`trainer_decoupled.py:310-315` builds an HF scheduler); ``get_last_lr()`` like torch schedulers."""
@@ -310,7 +310,7 @@ class DecoupledTrainer:
         mult = self.args.pad_to_multiple_of
         if mult is None:
             mult = 64 if self.is_cuda else 1        # few distinct padded lengths -> one CUDA graph per length
-            if self.is_cuda and os.environ.get("ACCO_ATTN", "").lower() == "tcgen05":
+            if self.is_cuda and os.environ.get("ACCO_ATTN", "").lower() == "own":
                 mult = 128                          # the own attention kernels tile the sequence in blocks of 128
         return PadCollator(pad_token_id=pad, max_length=int(self.args.max_length), pad_to_multiple_of=int(mult))
 
@@ -367,7 +367,7 @@ class DecoupledTrainer:
     # ------------------------------------------------------------------ fused all-gather + first-use GEMM (KERNEL B)
     def _setup_fused_ag(self) -> None:
         """``fused_ag_gemm``: the round kernel stops pushing the row-blocks of the model's GEMM weights; the first
-        forward GEMM after every flip pulls them from their owners over NVLink inside the tcgen05 kernel."""
+        forward GEMM after every flip pulls them from their owners over NVLink inside the wgmma GEMM kernel."""
         self._ag_on = False
         self._ag_stale = [False, False]     # theta[i] was rewritten by a round and its remote row-blocks are not pulled yet
         from .parallel.symm import SymmBackend
@@ -548,7 +548,7 @@ class DecoupledTrainer:
     # ================================================================== round machinery
     def _launch_round(self) -> None:
         plan = self.sched.next_plan()
-        # host-side protocol assertions (SURVEY section 5 "race detection"): the round must never consume the accumulator backward is
+        # host-side protocol assertions : the round must never consume the accumulator backward is
         # writing, nor overwrite the parameter buffer the model is bound to
         assert self._inflight is None, "a round is still in flight: complete it before launching the next one"
         if self._debug_poison:
@@ -579,7 +579,7 @@ class DecoupledTrainer:
         """Debug mode: NaN-fill the shadow parameter buffer right before the round that rewrites ALL of it is enqueued (same stream,
         so the round's writes land after the poison).  Correct schedules never read that buffer while the round is in flight - if
         compute does (a wrong flip, a missing event wait), the NaNs reach the loss immediately instead of silently training on torn
-        weights.  The reference's equivalent hazard is its unsynchronised `params <- com_buffer` copy (SURVEY Q8)."""
+        weights.  The reference's equivalent hazard is its unsynchronised `params <- com_buffer` copy ."""
         buf = self.arena.theta[plan.write_theta]
         if getattr(self, "_ag_on", False) or buf.data_ptr() == self.arena.theta[self.arena.live].data_ptr():
             return                      # fused-AG leaves pulled tiles to the next forward; single-buffer arenas have no shadow
@@ -885,7 +885,7 @@ class DecoupledTrainer:
                     prune_checkpoints(os.path.join(os.getcwd(), "checkpoints"), f"{self.id_run}{tag}", int(a.save_total_limit), self.rank)
 
     def _maybe_inject_fault(self, spec: str) -> None:
-        """Failure drill (the reference has no failure handling at all, SURVEY section 5): ``fault_inject="rank@count"`` makes
+        """Failure drill (the reference has no failure handling at all): ``fault_inject="rank@count"`` makes
         that rank die abruptly - no exception, no cleanup, like a lost GPU or an OOM-killed process - the first time the global
         gradient count reaches ``count``.  Its peers then fail in their next collective (NCCL / gloo error, or the signal-pad
         watchdog trap of the fused round kernel), the launcher restarts the group (``torchrun --max-restarts``) and
@@ -977,7 +977,7 @@ class DecoupledTrainer:
     # ================================================================== profiling
     def profile(self, steps: int = 4, outdir: Optional[str] = None, warmup: int = 1):
         """Run ``steps`` scheduling iterations under ``torch.profiler`` (CPU + CUDA activities) and export a Chrome trace
-        plus a per-op table to ``outdir`` (default ``./profiler/{id_run}``).  The reference has no tracing at all (SURVEY 5);
+        plus a per-op table to ``outdir`` (default ``./profiler/{id_run}``).  The reference has no tracing at all ;
         NVTX ranges are emitted as well when ``ACCO_NVTX=1``.  Returns the path of the trace."""
         from torch.profiler import ProfilerActivity, profile
         outdir = outdir or os.path.join(os.getcwd(), "profiler", str(self.id_run))

@@ -1,5 +1,5 @@
 """Small utilities: seeding (the reference seeds CUDA only with a hard-coded 42 and never seeds the
-CPU generator that actually initialises the model, `main.py:28`, SURVEY Q6), parameter counting,
+CPU generator that actually initialises the model, `main.py:28`), parameter counting,
 and the label-smoothed loss the reference instantiates (`trainer_base.py:63-68`,
 `utils/trainer_utils.py:862-902`) but never applies."""
 from __future__ import annotations

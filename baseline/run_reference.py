@@ -6,7 +6,7 @@ HF ``LlamaForCausalLM`` (cuBLAS / SDPA) under ``torch.autocast(bf16)`` - on the 
 batch shape and synthetic data as our arm.  None of this repo's models, kernels or engine is on
 that path.
 
-Environment shims (none of them touches reference code; SURVEY section 6):
+Environment shims (none of them touches reference code):
 * ``SLURM_*`` variables are synthesised from torchrun's ``RANK/LOCAL_RANK/WORLD_SIZE`` - the
   reference reads Slurm env directly (`trainer_base.py:137-146`);
 * ``omegaconf`` is not installed on this image: a 3-line stand-in provides
@@ -15,7 +15,7 @@ Environment shims (none of them touches reference code; SURVEY section 6):
   during the *timed* call so a 250 MB checkpoint write is not billed to the reference (our arm
   writes no checkpoint in its timed region either);
 * a watchdog aborts the process if the reference hangs (its barrier/reset protocol has a latent
-  race, SURVEY Q8).
+  race).
 
 Warm-up / timed split: ``train()`` is called twice on the same trainer - first with
 ``nb_grad_tot = warmup rounds``, then (timed) with ``nb_grad_tot = K rounds`` - the only way to
@@ -46,7 +46,7 @@ class _Args(dict):
 
 def reference_available() -> str:
     if not os.path.isfile(os.path.join(REF_DIR, "trainer_decoupled.py")):
-        return f"reference not installed under {REF_DIR} (see DESIGN.md, 'Reference arm')"
+        return f"reference not installed under {REF_DIR}"
     try:
         import datasets  # noqa: F401
         import transformers  # noqa: F401
@@ -92,7 +92,7 @@ def run_reference(steps: int, warmup: int, model_kw: Dict[str, Any], batch_size:
 
     def _abort():
         if rank == 0:
-            print('{"impl": "reference", "unavailable": "reference trainer hung (watchdog %.0fs); see SURVEY Q8"}' % watchdog_s, flush=True)
+            print('{"impl": "reference", "unavailable": "reference trainer hung (watchdog %.0fs): its unsynchronised params <- com_buffer copy can race"}' % watchdog_s, flush=True)
         os._exit(0)
     wd = threading.Timer(watchdog_s, _abort)
     wd.daemon = True

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Headline benchmark (BASELINE.json): training throughput in tokens/s, Llama-125M ACCO, bf16,
+"""Headline benchmark: training throughput in tokens/s, Llama-125M ACCO, bf16,
 sharded AdamW, synthetic openwebtext-shaped const-len batches of 8 x 1024 tokens per GPU
-(`config/train/acco.yaml` of the reference), weak scaling over 1/2/4/8 B200.
+(`config/train/acco.yaml` of the reference), weak scaling over 1/2/4/8 H100.
 
     python bench.py --gpus 1 --steps 20 --warmup 5
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port P \
@@ -108,7 +108,7 @@ class ClockSampler:
                 "reasons": sorted(reasons), "scope": getattr(self, "scope", "timed region")}
 
 
-# BASELINE.json configurations beyond the headline one (config 2 = the default flags).  The reference arm honours them too.
+# Named configurations beyond the headline one (config 2 = the default flags).  The reference arm honours them too.
 PRESETS_BENCH = {
     "llama125m": dict(model="llama125m", batch=8, seq=1024, n_acc=1, method="acco"),              # config 2 (headline)
     "llama125m-b1": dict(model="llama125m", batch=1, seq=1024, n_acc=1, method="acco"),            # comm/compute ~ 1: overlap matters
@@ -232,6 +232,8 @@ def run_ours(a) -> dict:
         loss = float(trainer.loss_host.item())
         n_params = trainer.len_params
         trainer._drain()
+        if a.dump_outputs and rank == 0:
+            dump_outputs(a.dump_outputs, trainer)
     finally:
         os.chdir(cwd)
     tok = a.batch * a.seq
@@ -244,7 +246,7 @@ def run_ours(a) -> dict:
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    mfu = value / world * flops_tok / (peaks.get("bf16_tflops_sustained", 1400.0) * 1e12)
+    mfu = value / world * flops_tok / (peaks.get("bf16_tflops_sustained", 989.0) * 1e12)   # default: H100 SXM data sheet, dense BF16
     return {
         "metric": METRIC, "value": value, "unit": "tokens/s", "n_gpus": world, "steps": a.steps, "warmup": max(a.warmup, 3),
         "ms_per_step": r_dev["ms"] / a.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -253,7 +255,7 @@ def run_ours(a) -> dict:
                    "micro_batch_per_gpu": a.batch, "seq_len": a.seq, "n_grad_accumulation": a.n_acc, "method": a.method,
                    "parallelism": f"dp{world}+zero1", "comm_backend": backend, "cuda_graphs": not a.no_graphs, "fused_ag_gemm": bool(a.fused_ag), "slow_rank_ms": a.slow_ms,
                    "step": "one trainer.step(): n_acc micro-batches/rank + one overlapped RS+AdamW+AG round",
-                   "l2": "per-step working set (250 MB weights x2 + >1 GB activations) exceeds the 126 MB L2; no explicit flush",
+                   "l2": "per-step working set (250 MB weights x2 + >1 GB activations) exceeds the 50 MB L2; no explicit flush",
                    "micro_batches_timed": r_dev["micro"]},
         "clocks": clocks,
         "e2e": {"value": e2e, "unit": "tokens/s", "ms_per_step": r_e2e["ms"] / a.steps, "wall_ms_per_step": r_e2e["wall_ms"] / a.steps,
@@ -265,6 +267,24 @@ def run_ours(a) -> dict:
         "comm_ms_per_round": overlap["comm_ms_mean"], "exposed_comm_ms_per_round": overlap["exposed_ms_mean"],
         "final_loss": loss,
     }
+
+
+DUMP_SAMPLE = 1 << 22          # parameters written by --dump-outputs: a fixed, seeded sample (16 MiB as float32)
+
+
+def dump_outputs(out_dir: str, trainer) -> None:
+    """What the timed path hands its caller after the last timed step: the loss of that step (``DecoupledTrainer.loss_host``) and
+    the model parameters once the round launched by that step has landed (a fixed, seeded sample of the flat parameter vector)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), trainer.loss_host.detach().cpu().double().numpy().reshape(1))
+    flat = trainer.arena.params_flat.detach().reshape(-1)
+    n = flat.numel()
+    if n > DUMP_SAMPLE:
+        idx = np.sort(np.random.default_rng(0).choice(n, DUMP_SAMPLE, replace=False))
+        flat = flat[torch.from_numpy(idx).to(flat.device)]
+    np.save(os.path.join(out_dir, "params_sample.npy"), flat.float().cpu().numpy())
 
 
 def run_reference_arm(a) -> dict:
@@ -319,9 +339,15 @@ def main():
     p.add_argument("--by-count", dest="by_count", action="store_true", help="time until the global gradient counter advanced by steps*world*n_acc")
     p.add_argument("--slow-rank", dest="slow_rank", type=int, default=1, help="rank slowed down when --slow-ms > 0 (heterogeneity experiment)")
     p.add_argument("--slow-ms", dest="slow_ms", type=float, default=0.0, help="extra GPU milliseconds per micro-batch on the slow rank")
+    p.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                   help="after the timed passes, write DIR/<name>.npy: the loss of the last step of the end-to-end pass and a seeded sample "
+                        "of the parameters once its round has landed.  Split-K weight gradients are summed with atomic adds, so two runs of "
+                        "the same build differ in the last bits; compare builds with a bf16 tolerance")
     p.add_argument("--preset", default=None, choices=sorted(PRESETS_BENCH),
-                   help="named BASELINE.json configurations (override --model/--batch/--seq/--n-acc/--method)")
+                   help="named configurations (override --model/--batch/--seq/--n-acc/--method)")
     a = p.parse_args()
+    if a.dump_outputs:
+        a.dump_outputs = os.path.abspath(a.dump_outputs)     # the timed run works in a temporary directory
     if a.preset:
         for k, v in PRESETS_BENCH[a.preset].items():
             setattr(a, k, v)

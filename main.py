@@ -3,7 +3,7 @@
 
     python main.py train=acco data=openwebtext model=llama125m            # 1 GPU (or CPU)
     torchrun --nproc-per-node 8 main.py train=acco model=llama125m       # 8 GPUs of one box
-    srun python -u main.py train=acco-ft data=alpaca model=llama3-8b     # Slurm, one task per GPU
+    srun python -u main.py train=acco-ft data=alpaca model=llama3-1b     # Slurm, one task per GPU
 
 Config groups ``train= data= model=`` and ``key=value`` overrides are composed by
 :mod:`acco_b200.config` (Hydra is not required).  The model is built from ``config/model/*.yaml``

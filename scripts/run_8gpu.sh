@@ -1,5 +1,5 @@
 #!/bin/bash
-# Single 8xB200 box without Slurm.
+# Single 8xH100 box without Slurm.
 #   scripts/run_8gpu.sh                                   # train=acco data=openwebtext model=llama125m
 #   NGPU=4 scripts/run_8gpu.sh train=dpu model=llama3-1b
 set -euo pipefail

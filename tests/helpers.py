@@ -25,7 +25,7 @@ def base_args(**kw):
 
 
 class ToyQuadratic(nn.Module):
-    """Loss whose k-th evaluation has gradient 0.1*(k+1)*p  (the toy of SURVEY 3.2's golden trace)."""
+    """Loss whose k-th evaluation has gradient 0.1*(k+1)*p  (the toy of the golden-trace test)."""
 
     def __init__(self, p0):
         super().__init__()

@@ -1,15 +1,14 @@
-"""Exhaustive interleaving check of the mbarrier protocols of the (not yet executed) tcgen05 attention kernels
-(csrc/attention_tcgen05.cu).  mbarrier phase / parity mistakes are the classic way such a kernel hangs or reads a stale tile, and
-they are a property of the SYNCHRONISATION SKELETON, which can be executed on a CPU: every warp role is transcribed as a straight
-program of `wait(barrier, parity)` / `arrive` / asynchronous TMA loads / tensor-core work + `tcgen05.commit`, with the parity
-expressions copied from the kernel, and a small explicit-state explorer runs every interleaving (including arbitrary delays of the
-TMA engine and of the in-order tensor pipe).  Checked: no deadlock, every role finishes, and every read sees the version of the
-tile it expects (K/V stage, S, P, O in the forward; Q/dO stage, S/dP, P/dS, dQ in the backward) while no tile is overwritten
-before its last reader is done.
+"""Exhaustive interleaving check of the mbarrier protocol of the own attention forward kernel (csrc/attention_wgmma.cu,
+`attn_fwd_kernel`).  mbarrier phase / parity mistakes are the classic way such a kernel hangs or reads a stale tile, and they are a
+property of the SYNCHRONISATION SKELETON, which can be executed on a CPU: every role (the TMA-issuing thread and the two consumer
+warpgroups) is transcribed as a straight program of `wait(barrier, parity)` / `arrive` / asynchronous TMA loads / tensor-core work,
+with the parity expressions copied from the kernel, and a small explicit-state explorer runs every interleaving (including
+arbitrary delays of the TMA engine).  The CTA barrier that ends a key block is modelled as a barrier every role arrives on and then
+waits for.  Checked: no deadlock, every role finishes, every read sees the K / V block it expects, and no stage is overwritten by a
+TMA load before its last reader is done.
 
 mbarrier semantics used: a barrier counts arrivals of the current phase; when the count is reached the phase number advances.
-`try_wait.parity p` succeeds iff the phase with parity p has completed, i.e. iff the parity of the CURRENT phase differs from p
-(a fresh barrier is in phase 0: waiting for parity 1 returns at once - the producers' "stage is free" idiom)."""
+`try_wait.parity p` succeeds iff the phase with parity p has completed, i.e. iff the parity of the CURRENT phase differs from p."""
 import pytest
 
 
@@ -100,87 +99,55 @@ def named(name, fn):
 
 # ================================================================================================ forward
 def forward_model(nblk, break_parity=False):
-    data = {"S": -1, "S_free": True, "P": -1, "P_free": True, "O": -1, "O_free": True, "Q": False}
+    """attn_fwd_kernel: thread 0 issues Q and the first two K/V blocks, then block i + 2 into stage i & 1 after the CTA barrier that
+    ends block i; both warpgroups wait full[i & 1] with parity (i >> 1) & 1, read the stage, and join the CTA barrier."""
+    data = {"Q": False}
     for s in range(2):
-        data[f"K{s}"], data[f"V{s}"], data[f"K{s}_free"], data[f"V{s}_free"] = -1, -1, True, True
+        data[f"KV{s}"], data[f"KV{s}_readers"] = -1, 0
 
-    def tma_tile(kind, s, i):
+    def tma_kv(s, i):
         def fn(d, what):
             if what == "issue":
-                assert d[f"{kind}{s}_free"], f"TMA overwrites {kind} stage {s} (holds block {d[f'{kind}{s}']}) with block {i}"
-                d[f"{kind}{s}_free"] = False
-                d[f"{kind}{s}"] = -1
+                assert d[f"KV{s}_readers"] == 0, f"TMA overwrites stage {s} (block {d[f'KV{s}']}) while it is read, with block {i}"
+                d[f"KV{s}"] = -1
             else:
-                d[f"{kind}{s}"] = i
-        return named(f"tma_{kind}{s}_{i}", fn)
+                d[f"KV{s}"] = i
+        return named(f"tma_kv{s}_{i}", fn)
 
     def tma_q(d, what):
         if what == "land":
             d["Q"] = True
 
-    def mma_s(i):
+    def read_begin(w, i):
         def fn(d):
-            assert d["Q"] and d[f"K{i & 1}"] == i, f"S_{i} reads K stage holding {d[f'K{i & 1}']}"
-            assert d["S_free"], f"S_{i} overwrites S_{d['S']} before the softmax has read it"
-            d["S"], d["S_free"] = i, False
-        return named(f"mma_S{i}", fn)
+            s = i & 1
+            assert d["Q"], f"warpgroup {w} reads Q before it landed"
+            assert d[f"KV{s}"] == i, f"warpgroup {w} block {i} reads stage {s} holding block {d[f'KV{s}']}"
+            d[f"KV{s}_readers"] += 1
+        return named(f"read_begin{w}_{i}", fn)
 
-    def mma_pv(i):
+    def read_end(w, i):
         def fn(d):
-            assert d["P"] == i and d[f"V{i & 1}"] == i, f"PV_{i} reads P_{d['P']} / V stage holding {d[f'V{i & 1}']}"
-            assert d["O_free"], f"PV_{i} overwrites O_{d['O']} before the softmax has accumulated it"
-            d["O"], d["O_free"] = i, False
-            d["P_free"] = True
-            d[f"K{i & 1}_free"] = d[f"V{i & 1}_free"] = True          # released by the commit that follows, in pipe order
-        return named(f"mma_PV{i}", fn)
+            d[f"KV{i & 1}_readers"] -= 1
+        return named(f"read_end{w}_{i}", fn)
 
-    def sm_read_s(i):
-        def fn(d):
-            assert d["S"] == i, f"softmax {i} reads S_{d['S']}"
-        return named(f"read_S{i}", fn)
-
-    def sm_read_o(i):
-        def fn(d):
-            assert d["O"] == i and not d["O_free"], f"softmax reads O_{d['O']} instead of O_{i}"
-            d["O_free"] = True
-        return named(f"read_O{i}", fn)
-
-    def sm_write_p(i):
-        def fn(d):
-            assert d["S"] == i, f"softmax {i} pass 2 reads S_{d['S']}"
-            assert d["P_free"], f"softmax {i} overwrites P_{d['P']} before its PV MMA has read it"
-            d["P"], d["P_free"] = i, False
-            d["S_free"] = True
-        return named(f"write_P{i}", fn)
-
-    producer = [("tma", "q_full", named("tma_q", tma_q))]
+    producer = [("tma", "q_full", named("tma_q", tma_q)), ("tma", "full0", tma_kv(0, 0))]
+    if nblk > 1:
+        producer += [("tma", "full1", tma_kv(1, 1))]
     for i in range(nblk):
-        s, ph = i & 1, (i >> 1) & 1
-        producer += [("wait", f"kv_empty{s}", ph ^ 1), ("tma", f"k_full{s}", tma_tile("K", s, i)), ("tma", f"v_full{s}", tma_tile("V", s, i))]
-
-    def issue_s(i):
-        return [("wait", f"k_full{i & 1}", (i >> 1) & 1), ("mma", mma_s(i)), ("commit", "s_full")]
-
-    mma = [("wait", "q_full", 0)] + issue_s(0)
-    for i in range(nblk):
-        s = i & 1
-        mma += [("wait", "p_full", (i & 1) if not break_parity else 0)]
-        if i + 1 < nblk:
-            mma += issue_s(i + 1)
-        mma += [("wait", f"v_full{s}", (i >> 1) & 1), ("mma", mma_pv(i)), ("commit", f"kv_empty{s}"), ("commit", "o_full")]
-
-    softmax = []
-    for i in range(nblk):
-        softmax += [("wait", "s_full", i & 1), ("do", sm_read_s(i))]
-        if i > 0:
-            softmax += [("wait", "o_full", (i - 1) & 1), ("do", sm_read_o(i - 1))]
-        softmax += [("do", sm_write_p(i)), ("arrive", "p_full")]
-    softmax += [("wait", "o_full", (nblk - 1) & 1), ("do", sm_read_o(nblk - 1))]
-
-    bars = {"q_full": 1, "s_full": 1, "p_full": 1, "o_full": 1}      # p_full: 128 arrivals in the kernel, one per softmax thread
-    for s in range(2):
-        bars.update({f"k_full{s}": 1, f"v_full{s}": 1, f"kv_empty{s}": 1})
-    return Model({"producer": producer, "mma": mma, "softmax": softmax}, bars, data)
+        producer += [("arrive", "cta"), ("wait", "cta", i & 1)]
+        if i + 2 < nblk:
+            producer += [("tma", f"full{i & 1}", tma_kv(i & 1, i + 2))]
+    roles = {"producer": producer}
+    for w in range(2):
+        prog = [("wait", "q_full", 0)]
+        for i in range(nblk):
+            parity = ((i >> 1) & 1) if not break_parity else 0
+            prog += [("wait", f"full{i & 1}", parity), ("do", read_begin(w, i)), ("do", read_end(w, i)), ("arrive", "cta"),
+                     ("wait", "cta", i & 1)]
+        roles[f"warpgroup{w}"] = prog
+    bars = {"q_full": 1, "full0": 1, "full1": 1, "cta": 3}           # the CTA barrier: thread 0's warpgroup and the two consumers
+    return Model(roles, bars, data)
 
 
 @pytest.mark.parametrize("nblk", [1, 2, 3, 4, 5, 6])
@@ -191,108 +158,3 @@ def test_forward_protocol(nblk):
 def test_forward_checker_catches_a_parity_bug():
     with pytest.raises(AssertionError):
         forward_model(3, break_parity=True).explore()
-
-
-# ================================================================================================ backward
-def backward_model(T, skip_dq_wait=False):
-    data = {"KV": False, "SdP": -1, "SdP_free": True, "PdS": -1, "PdS_free": True, "dQ": -1, "dQ_free": True, "dKV": 0}
-    for s in range(2):
-        data[f"QdO{s}"], data[f"QdO{s}_free"] = -1, True
-
-    def tma_kv(d, what):
-        if what == "land":
-            d["KV"] = True
-
-    def tma_qdo(s, it):
-        def fn(d, what):
-            if what == "issue":
-                assert d[f"QdO{s}_free"], f"TMA overwrites (Q, dO) stage {s} (iteration {d[f'QdO{s}']}) with iteration {it}"
-                d[f"QdO{s}_free"], d[f"QdO{s}"] = False, -1
-            else:
-                d[f"QdO{s}"] = it
-        return named(f"tma_QdO{s}_{it}", fn)
-
-    def mma_sdp(it):
-        def fn(d):
-            assert d["KV"] and d[f"QdO{it & 1}"] == it, f"S/dP {it} reads stage holding {d[f'QdO{it & 1}']}"
-            assert d["SdP_free"], f"S/dP {it} overwrites S/dP {d['SdP']} before the softmax has read it"
-            d["SdP"], d["SdP_free"] = it, False
-        return named(f"mma_SdP{it}", fn)
-
-    def mma_grads(it):
-        def fn(d):
-            assert d["PdS"] == it and d[f"QdO{it & 1}"] == it, f"gradient MMAs {it} read P/dS {d['PdS']} / stage {d[f'QdO{it & 1}']}"
-            assert d["dQ_free"], f"dQ {it} overwrites dQ {d['dQ']} before it was drained"
-            d["dQ"], d["dQ_free"] = it, False
-            d["PdS_free"] = True
-            d[f"QdO{it & 1}_free"] = True
-            d["dKV"] += 1
-        return named(f"mma_grads{it}", fn)
-
-    def sm_read(it):
-        def fn(d):
-            assert d["SdP"] == it, f"softmax {it} reads S/dP {d['SdP']}"
-        return named(f"read_SdP{it}", fn)
-
-    def sm_write(it):
-        def fn(d):
-            assert d["SdP"] == it
-            assert d["PdS_free"], f"softmax {it} overwrites P/dS {d['PdS']} before the gradient MMAs have read it"
-            d["PdS"], d["PdS_free"] = it, False
-            d["SdP_free"] = True
-        return named(f"write_PdS{it}", fn)
-
-    def dq_read(it):
-        def fn(d):
-            assert d["dQ"] == it and not d["dQ_free"], f"dQ drain {it} reads dQ {d['dQ']}"
-            d["dQ_free"] = True
-        return named(f"read_dQ{it}", fn)
-
-    def epilogue(d):
-        assert d["dKV"] == T, f"dK / dV epilogue after {d['dKV']} of {T} iterations"
-
-    producer = [("tma", "kv_full", named("tma_kv", tma_kv))]
-    for it in range(T):
-        s = it & 1
-        producer += [("wait", f"qdo_empty{s}", ((it >> 1) & 1) ^ 1), ("tma", f"qdo_full{s}", tma_qdo(s, it))]
-
-    def issue_sdp(it):
-        return [("wait", f"qdo_full{it & 1}", (it >> 1) & 1), ("mma", mma_sdp(it)), ("commit", "sdp_full")]
-
-    mma = [("wait", "kv_full", 0)] + issue_sdp(0)
-    for it in range(T):
-        mma += [("wait", "pds_full", it & 1)]
-        if it + 1 < T:
-            mma += issue_sdp(it + 1)
-        if it > 0 and not skip_dq_wait:
-            mma += [("wait", "dq_empty", (it - 1) & 1)]
-        mma += [("mma", mma_grads(it)), ("commit", "pds_empty"), ("commit", f"qdo_empty{it & 1}"), ("commit", "dq_full")]
-        if it == T - 1:
-            mma += [("commit", "dkv_full")]
-
-    wg0 = []
-    for it in range(T):
-        wg0 += [("wait", "sdp_full", it & 1), ("do", sm_read(it))]
-        if it > 0:
-            wg0 += [("wait", "pds_empty", (it - 1) & 1)]
-        wg0 += [("do", sm_write(it)), ("arrive", "pds_full")]
-    wg0 += [("wait", "dkv_full", 0), ("do", named("epilogue_dV", epilogue))]
-
-    wg1 = []
-    for it in range(T):
-        wg1 += [("wait", "dq_full", it & 1), ("do", dq_read(it)), ("arrive", "dq_empty")]
-    wg1 += [("wait", "dkv_full", 0), ("do", named("epilogue_dK", epilogue))]
-
-    bars = {"kv_full": 1, "sdp_full": 1, "pds_full": 1, "pds_empty": 1, "dq_full": 1, "dq_empty": 1, "dkv_full": 1,
-            "qdo_full0": 1, "qdo_full1": 1, "qdo_empty0": 1, "qdo_empty1": 1}
-    return Model({"producer": producer, "mma": mma, "wg0_softmax": wg0, "wg1_dq": wg1}, bars, data)
-
-
-@pytest.mark.parametrize("T", [1, 2, 3, 4, 5])
-def test_backward_protocol(T):
-    assert backward_model(T).explore() > T * 10
-
-
-def test_backward_checker_catches_a_missing_wait():
-    with pytest.raises(AssertionError):
-        backward_model(3, skip_dq_wait=True).explore()

@@ -1,9 +1,10 @@
-"""CPU checks for the tcgen05 attention kernels (csrc/attention_tcgen05.cu) - what can be verified without a GPU:
+"""CPU checks of the flash-attention specification and the glue of the own kernels (csrc/attention_wgmma.cu) - what can be verified
+without a GPU:
 
 * the blockwise schedule the kernels implement (``attention_blockwise_ref`` / ``attention_blockwise_bwd_ref``: delayed P V
   accumulation, running-max rescale, bf16 rounding points, dS scaling, GQA accumulation) against the fp32 reference + autograd;
 * the block ranges of the forward / backward loops against a brute-force visibility test (causal and sliding window);
-* the shared-memory images: what ``st_swz`` / a SWIZZLE_128B TMA box write versus what the tcgen05 shared-memory descriptors
+* the shared-memory images: what ``st_swz`` / a SWIZZLE_128B TMA box write versus what the wgmma shared-memory descriptors
   (K-major and MN-major views, the LBO / SBO / K-step constants of the kernel) address.  The address model is first checked on the
   two operand configurations that are proven on hardware by the GEMM tests (K-major boxes; MN-major {64, 64} boxes 8 KiB apart)."""
 import numpy as np
@@ -127,7 +128,7 @@ def test_dq_staging_image_matches_an_fp32_box():
 # ---------------------------------------------------------------------------------------------- autograd glue of the opt-in path
 class _FakeExt:
     """Stand-in for acco_b200._C on the CPU: the attention entry points backed by the blockwise specification, the RoPE kernels by
-    their reference math.  Exercises `_RopeAttentionFn`'s own-kernel branch (ACCO_ATTN=tcgen05) end to end - argument order,
+    their reference math.  Exercises `_RopeAttentionFn`'s own-kernel branch (ACCO_ATTN=own) end to end - argument order,
     saved tensors, packed d(qkv) layout, inverse rotation - everything except the CUDA kernels themselves."""
 
     @staticmethod
@@ -165,7 +166,7 @@ def test_own_attention_autograd_glue(monkeypatch, rope, window, scale):
     from acco_b200 import ops
     from acco_b200.ops import attention as A
     from acco_b200.ops.rope import rope_qkv_ref, rope_tables
-    monkeypatch.setenv("ACCO_ATTN", "tcgen05")
+    monkeypatch.setenv("ACCO_ATTN", "own")
     monkeypatch.setattr(ops, "load_ext", lambda required=False: _FakeExt)
     B, S, Hq, Hk, D = 2, 256, 4, 2, 64
     torch.manual_seed(1)

@@ -92,10 +92,11 @@ def test_shim_step_primitives_drive_a_round(workdir):
 
 
 @pytest.mark.parametrize("train,data", [("dpu", "synthetic"), ("ddp", "synthetic"), ("dpu-ft", "alpaca"), ("ddp-ft", "alpaca")])
-def test_every_shipped_train_config_runs(workdir, train, data):
+def test_every_shipped_train_config_runs(workdir, monkeypatch, train, data):
     """`config/train/{dpu,ddp,dpu-ft,ddp-ft}.yaml` through `main.py` (acco / acco-ft are covered above): warm-up rounds, eval
-    cadence, pad-collated SFT batches, synchronous DDP."""
+    cadence, pad-collated SFT batches, synchronous DDP - on the CPU / gloo path, also on a machine with a GPU."""
     import main as cli
+    monkeypatch.setattr(torch.cuda, "is_available", lambda: False)
     stats = cli.main([f"train={train}", "model=tiny", f"data={data}", "data.synthetic=true", "train.nb_steps_tot=16", "train.batch_size=2",
                       "train.max_length=32", "train.use_mixed_precision=False", "data.synthetic_docs=120", "data.synthetic_mean_len=20",
                       "train.warmup=0", "train.n_warmup_steps=2", "train.tensorboard=False", "train.save=False", "train.eval_step=4"])

@@ -101,7 +101,7 @@ def test_run_id_is_unique_outside_slurm_and_overridable(monkeypatch):
 def test_launcher_topology_discovery():
     """Rank / node topology from the launcher's environment: Slurm (`trainer_base.py:137-151`: SLURM_{PROCID,LOCALID,NODEID,NTASKS,
     JOB_NODELIST,STEP_GPUS}, master = first host of the node list, port 12346 + lowest GPU id - numeric, not the reference's string
-    min, SURVEY Q12) and torchrun (RANK / LOCAL_RANK / LOCAL_WORLD_SIZE / GROUP_RANK)."""
+    min) and torchrun (RANK / LOCAL_RANK / LOCAL_WORLD_SIZE / GROUP_RANK)."""
     from acco_b200.launch import discover_env
     slurm = {"SLURM_PROCID": "11", "SLURM_LOCALID": "3", "SLURM_NODEID": "1", "SLURM_NTASKS": "16", "SLURM_JOBID": "777",
              "SLURM_JOB_NODELIST": "gpu[07-08]", "SLURM_STEP_GPUS": "10,9,2,3"}

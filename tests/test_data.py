@@ -48,7 +48,7 @@ def test_collators():
     out = col([{"input_ids": [1, 2, eos, 3]}, {"input_ids": [4, 5]}])
     assert out["input_ids"].tolist() == [[1, 2, eos, 3], [4, 5, eos, eos]]
     assert out["attention_mask"].tolist() == [[1, 1, 1, 1], [1, 1, 0, 0]]
-    # pad == eos  =>  every EOS label is masked, also the real one (SURVEY Q11)
+    # pad == eos  =>  every EOS label is masked, also the real one
     assert out["labels"].tolist() == [[1, 2, -100, 3], [4, 5, -100, -100]]
     out2 = PadCollator(eos, mask_all_pad_tokens=False)([{"input_ids": [1, 2, eos, 3]}, {"input_ids": [4, 5]}])
     assert out2["labels"].tolist() == [[1, 2, eos, 3], [4, 5, -100, -100]]

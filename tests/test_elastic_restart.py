@@ -1,6 +1,6 @@
 """Failure drill, end to end on CPU (gloo): a rank dies mid-run -> its peer fails in the next collective -> torchrun restarts the
 worker group -> `resume_from=auto` picks up the newest complete checkpoint -> the job finishes.  (The reference hangs forever when a
-rank dies: no timeout, no restart, no resume - SURVEY section 5.)"""
+rank dies: no timeout, no restart, no resume)."""
 import os
 import subprocess
 import sys
@@ -13,7 +13,7 @@ def clean_env(**extra):
     and that port is held by this very process)."""
     drop = ("MASTER_ADDR", "MASTER_PORT", "RANK", "WORLD_SIZE", "LOCAL_RANK", "LOCAL_WORLD_SIZE", "GROUP_RANK")
     env = {k: v for k, v in os.environ.items() if k not in drop and not k.startswith(("SLURM_", "TORCHELASTIC_"))}
-    env.update(OMP_NUM_THREADS="2", PYTHONPATH=ROOT, **extra)
+    env.update(OMP_NUM_THREADS="2", PYTHONPATH=ROOT, CUDA_VISIBLE_DEVICES="", **extra)     # CPU ranks over gloo, also on a GPU machine
     return env
 
 

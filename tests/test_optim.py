@@ -82,7 +82,7 @@ def test_lr_units():
 
 
 def test_gemm_reference_layouts_match_torch():
-    """CPU path of ops.gemm (the numerics oracle of the tcgen05 kernel): K-major / MN-major operands, bias, accumulate."""
+    """CPU path of ops.gemm (the numerics oracle of the wgmma kernel): K-major / MN-major operands, bias, accumulate."""
     import torch
     from acco_b200.ops.gemm import gemm, gemm_nn, gemm_tn, gemm_tt_acc
     torch.manual_seed(0)

@@ -95,57 +95,57 @@ def test_tentative_plus_real_equals_one_large_batch_step(seed, n1, n2):
 
 
 # ----------------------------------------------------------------------------------------------
-# tcgen05 GEMM work decomposition (mirrors `decode_unit` / the unit loops of csrc/gemm_tcgen05.cu)
+# GEMM work decomposition (mirrors `decode_unit` / the unit loops of csrc/gemm_wgmma.cu)
 # ----------------------------------------------------------------------------------------------
-def _gemm_units(M, N, K, msub, bn, splits, pm, pn, slots):
-    """Python twin of the device-side tile scheduler: yields (cluster, pair, mu, n_blk, kb0, kb1) for every unit every pair runs."""
-    BM, BK, ctas = 128, 64, 2
-    rows_cta = BM * msub
+def _gemm_units(M, N, K, bn, splits, pm, pn, slots):
+    """Python twin of the device-side tile scheduler: yields (cluster, cta, mb, n_blk, kb0, kb1) for every unit every CTA runs.
+    A CTA computes 128-row tiles; a cluster is pm x pn CTAs (cluster rank = pi * pn + pj) owning a super-tile of pm x pn tiles."""
+    BM, BK = 128, 64
     num_n, num_k = -(-N // bn), -(-K // BK)
-    num_mu = -(-M // (ctas * rows_cta))
+    num_mb = -(-M // BM)
     num_sn = -(-num_n // pn)
-    tiles = -(-num_mu // pm) * num_sn
+    tiles = -(-num_mb // pm) * num_sn
     splits = max(1, min(splits, num_k))
     kbs = -(-num_k // splits)
     splits = -(-num_k // kbs)
     num_units = tiles * splits
     grid_clusters = min(num_units, slots)
     for cl in range(grid_clusters):
-        for pair in range(pm * pn):
-            pi, pj = divmod(pair, pn)
+        for cta in range(pm * pn):
+            pi, pj = divmod(cta, pn)
             t = cl
             while t < num_units:
                 s, tile = divmod(t, tiles)
-                smu, sn = divmod(tile, num_sn)
-                yield cl, pair, smu * pm + pi, sn * pn + pj, s * kbs, min(num_k, s * kbs + kbs)
+                smb, sn = divmod(tile, num_sn)
+                yield cl, cta, smb * pm + pi, sn * pn + pj, s * kbs, min(num_k, s * kbs + kbs)
                 t += grid_clusters
     return
 
 
 @settings(max_examples=150, deadline=None)
-@given(M=st.integers(1, 3000), N=st.integers(8, 1500), K=st.integers(8, 4000), msub=st.sampled_from([1, 2]), bn=st.sampled_from([64, 128, 192, 256]),
-       splits=st.integers(1, 9), pm=st.sampled_from([1, 2]), pn=st.sampled_from([1, 2]), slots=st.integers(1, 74))
-def test_gemm_tile_scheduler_covers_every_output_k_block_exactly_once(M, N, K, msub, bn, splits, pm, pn, slots):
-    """Every real (m-unit, n-block, k-block) triple is computed by exactly one pair; phantom tiles (odd counts under pair clusters) lie
-    entirely outside the matrix (TMA zero-fills their loads and clips their stores); all pairs of a cluster run the same number of
-    k-iterations (they share pipeline stages through multicast), and no split is empty."""
-    rows_pair = 256 * msub
-    num_mu, num_n, num_k = -(-M // rows_pair), -(-N // bn), -(-K // 64)
+@given(M=st.integers(1, 3000), N=st.integers(8, 1500), K=st.integers(8, 4000), bn=st.sampled_from([64, 128, 256]),
+       splits=st.integers(1, 9), pm=st.sampled_from([1, 2]), pn=st.sampled_from([1, 2]), slots=st.integers(1, 132))
+def test_gemm_tile_scheduler_covers_every_output_k_block_exactly_once(M, N, K, bn, splits, pm, pn, slots):
+    """Every real (m-block, n-block, k-block) triple is computed by exactly one CTA; phantom tiles (odd counts under clusters) lie
+    entirely outside the matrix (TMA zero-fills their loads, the epilogue stores nothing); all CTAs of a cluster run the same number
+    of k-iterations (they share pipeline stages through multicast), and no split is empty."""
+    BM = 128
+    num_mb, num_n, num_k = -(-M // BM), -(-N // bn), -(-K // 64)
     seen = {}
-    per_pair_iters = {}
-    for cl, pair, mu, n_blk, kb0, kb1 in _gemm_units(M, N, K, msub, bn, splits, pm, pn, slots):
+    per_cta_iters = {}
+    for cl, cta, mb, n_blk, kb0, kb1 in _gemm_units(M, N, K, bn, splits, pm, pn, slots):
         assert kb1 > kb0                                             # no empty split
-        per_pair_iters[(cl, pair)] = per_pair_iters.get((cl, pair), 0) + (kb1 - kb0)
-        real = mu < num_mu and n_blk < num_n
+        per_cta_iters[(cl, cta)] = per_cta_iters.get((cl, cta), 0) + (kb1 - kb0)
+        real = mb < num_mb and n_blk < num_n
         if not real:
-            assert mu * rows_pair >= M or n_blk * bn >= N            # phantom tile: fully out of range
+            assert mb * BM >= M or n_blk * bn >= N                   # phantom tile: fully out of range
             continue
         for kb in range(kb0, kb1):
-            key = (mu, n_blk, kb)
+            key = (mb, n_blk, kb)
             assert key not in seen, key
             seen[key] = True
-    assert len(seen) == num_mu * num_n * num_k
+    assert len(seen) == num_mb * num_n * num_k
     by_cluster = {}
-    for (cl, pair), it in per_pair_iters.items():
+    for (cl, cta), it in per_cta_iters.items():
         by_cluster.setdefault(cl, set()).add(it)
     assert all(len(v) == 1 for v in by_cluster.values())           # lock-step inside a cluster

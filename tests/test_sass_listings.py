@@ -18,11 +18,14 @@ def test_docs_sass_matches_built_extension():
     assert p.returncode == 0, p.stdout[-3000:]
 
 
-def test_blackwell_native_mnemonics_present():
-    """tcgen05 / TMEM / TMA / multimem instructions are in the shipped kernels (B200_PROFILING.md 'What proves a Blackwell-native kernel')."""
+def test_hopper_native_mnemonics_present():
+    """wgmma / TMA / setmaxnreg / multimem instructions are in the shipped kernels (docs/sass/mnemonics.json, tools/dump_sass.py)."""
     import json
     m = json.load(open(os.path.join(ROOT, "docs", "sass", "mnemonics.json")))
-    g = m["gemm_tcgen05_2sm.sass"]
-    assert g["UTCHMMA.2CTA"] > 0 and g["LDTM"] > 0 and g["UTMALDG.2D.2CTA"] > 0 and g["UTMASTG"] > 0 and g["UTMAREDG"] > 0
-    assert g["HMMA"] == 0                                   # no legacy mma.sync path
+    for name in ("gemm_wgmma_bn256_tn.sass", "gemm_wgmma_bn256_nn.sass", "gemm_wgmma_bn128_tt.sass"):
+        g = m[name]
+        assert g["HGMMA"] > 0 and g["UTMALDG"] > 0 and g["UTMALDG.2D.MULTICAST"] > 0 and g["UTMASTG"] > 0 and g["USETMAXREG"] > 0, name
+        assert g["HMMA"] == 0, name                          # no legacy mma.sync path
     assert m["rs_adam_ag_multimem_bf16.sass"]["LDGMC"] > 0   # multimem.ld_reduce
+    a = m["attn_fwd_wgmma.sass"]                             # own attention forward: wgmma fed by a TMA ring
+    assert a["HGMMA"] > 0 and a["UTMALDG"] > 0 and a["SYNCS"] > 0

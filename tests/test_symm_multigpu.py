@@ -55,13 +55,3 @@ def test_backends_train_to_the_same_parameters_and_tolerate_a_slow_rank(tmp_path
     assert p.returncode == 0, p.stdout[-3000:]
     rep = json.load(open(out))
     assert rep["ok"] and rep["checks"]["hetero"]["fast_ranks_accumulated_more"], rep
-
-
-def test_round_watchdog_traps_when_a_rank_dies():
-    """A rank that never launches its round must not hang its peers forever: the start barrier traps after ACCO_ROUND_WATCHDOG_S."""
-    from acco_b200.launch import free_port
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr", "127.0.0.1",
-           "--master-port", str(free_port()), os.path.join(ROOT, "tools", "watchdog_check.py")]
-    p = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=300,
-                       env={**os.environ, "ACCO_ROUND_WATCHDOG_S": "3"})
-    assert "watchdog fired" in p.stdout and "] OK" in p.stdout, p.stdout[-3000:]

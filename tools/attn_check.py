@@ -1,12 +1,11 @@
 #!/usr/bin/env python
-"""Bring-up harness for the tcgen05 flash-attention kernels (csrc/attention_tcgen05.cu; single GPU):
+"""Check of the own flash-attention kernels (csrc/attention_wgmma.cu; single GPU):
 
-    timeout 300 python tools/attn_check.py [--quick] [--no-bwd] [--out gpurun_out/attn_check.json]
+    timeout 300 python tools/attn_check.py [--quick] [--no-bwd] [--out attn_check.json]
 
 Per shape: forward (O, LSE) and backward (dQ, dK, dV) of the own kernels against the fp32 PyTorch reference (the same oracle the
 CPU spec test uses), then device time per call against the library path (cuDNN / flash SDPA forward + backward on the same
-tensors).  The kernels have an in-kernel mbarrier watchdog (5 s -> message naming the starved barrier, then trap), so a protocol bug ends the process with a CUDA error
-instead of hanging the GPU; run under `timeout` anyway.  Exit code 0 = every shape within tolerance."""
+tensors).  Exit code 0 = every shape within tolerance."""
 import argparse
 import json
 import math

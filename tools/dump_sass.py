@@ -1,12 +1,13 @@
 #!/usr/bin/env python
-"""Regenerate `docs/sass/*.sass` and `docs/sass/mnemonics.json` from the BUILT extension (`acco_b200/_C.so`).
+"""Summarise the SASS of the BUILT extension (`acco_b200/_C.so`, sm_90a) in `docs/sass/mnemonics.json`.
 
-    python tools/dump_sass.py            # rewrite the listings + summary
-    python tools/dump_sass.py --check    # exit 1 if the committed summary does not describe the built binary
+    python tools/dump_sass.py              # rewrite the summary
+    python tools/dump_sass.py --listings   # also write the full listings to docs/sass/*.sass (large; not kept in git)
+    python tools/dump_sass.py --check      # exit 1 if the committed summary does not describe the built binary
 
-The summary counts, per listed kernel, the SASS mnemonics that prove the Blackwell-native path (B200_PROFILING.md: `UTC*MMA` = tcgen05.mma,
-`LDTM` = tcgen05.ld, `UTMALDG` / `UTMASTG` / `UTMAREDG` = TMA load / store / reduce, `LDGMC` = multimem.ld_reduce ...).
-`tests/test_sass_listings.py` runs the --check so a stale listing cannot be committed again (round-1 finding)."""
+The summary counts, per listed kernel, the SASS mnemonics that show the Hopper-native path: `HGMMA` = wgmma.mma_async,
+`UTMALDG` / `UTMASTG` = TMA load / store, `SYNCS` = mbarrier operations, `USETMAXREG` = setmaxnreg, `REDG` = the split-K atomic
+adds, `LDGMC` = multimem.ld_reduce ...  `tests/test_sass_listings.py` runs the --check so a stale summary cannot be committed."""
 import json
 import os
 import re
@@ -18,16 +19,16 @@ SO = os.path.join(ROOT, "acco_b200", "_C.so")
 OUT = os.path.join(ROOT, "docs", "sass")
 
 KERNELS = {
-    "gemm_tcgen05_2sm.sass": "_ZN9acco_gemm11gemm_kernelILi2ELi1EEEvNS_6ParamsE",
-    "gemm_tcgen05_1sm.sass": "_ZN9acco_gemm11gemm_kernelILi1ELi1EEEvNS_6ParamsE",
+    "gemm_wgmma_bn256_tn.sass": "_ZN9acco_gemm11gemm_kernelILi256ELi0ELi0EEEvNS_6ParamsE",
+    "gemm_wgmma_bn256_nn.sass": "_ZN9acco_gemm11gemm_kernelILi256ELi0ELi1EEEvNS_6ParamsE",
+    "gemm_wgmma_bn128_tt.sass": "_ZN9acco_gemm11gemm_kernelILi128ELi1ELi1EEEvNS_6ParamsE",
     "rs_adam_ag_multimem_bf16.sass": "_ZN4acco17rs_adam_ag_kernelI13__nv_bfloat16S1_Li2ELb0EEEvNS_11RoundParamsE",
     "rs_adam_ag_p2p_bf16.sass": "_ZN4acco17rs_adam_ag_kernelI13__nv_bfloat16S1_Li1ELb0EEEvNS_11RoundParamsE",
     "round_gate.sass": "_ZN4acco17round_gate_kernelENS_11RoundParamsE",
-    "attn_fwd_tcgen05.sass": "_ZN9acco_attn15attn_fwd_kernelENS_9FwdParamsE",       # experimental (opt-in, not executed yet)
-    "attn_bwd_tcgen05.sass": "_ZN9acco_attn15attn_bwd_kernelENS_9BwdParamsE",
+    "attn_fwd_wgmma.sass": "_ZN9acco_attn15attn_fwd_kernelENS_9FwdParamsE",
 }
-MNEMONICS = ["UTCHMMA", "UTCHMMA.2CTA", "UTMALDG", "UTMALDG.2D.2CTA", "UTMALDG.2D.MULTICAST.2CTA", "UTMASTG", "UTMAREDG", "LDTM", "UTCBAR", "UCGABAR_ARV",
-             "SYNCS", "LDGMC", "HMMA", "MUFU.SQRT", "MUFU.EX2", "ACQBULK", "CCTL"]
+MNEMONICS = ["HGMMA", "UTMALDG", "UTMALDG.2D.MULTICAST", "UTMASTG", "UTMACMDFLUSH", "SYNCS", "USETMAXREG", "REDG", "LDGMC", "HMMA", "MUFU.SQRT",
+             "MUFU.EX2", "CCTL"]
 
 
 def listing(func: str) -> str:
@@ -57,7 +58,7 @@ def main():
     for fname, func in KERNELS.items():
         txt = listing(func)
         summary[fname] = {"function": func, **count(txt)}
-        if not check:
+        if not check and "--listings" in sys.argv:
             with open(os.path.join(OUT, fname), "w") as f:
                 f.write(txt)
     path = os.path.join(OUT, "mnemonics.json")

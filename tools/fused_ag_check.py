@@ -76,18 +76,18 @@ def main():
         dl = max(abs(a - b) for a, b in zip(base["losses"], fused["losses"]))
         dp = float((p0.float() - p1.float()).abs().max())
         good = (dl < 5e-2 and fused["rank_divergence"] == 0 and base["rank_divergence"] == 0 and dp < 2e-2
-                and fused["launches"].get("gemm_tcgen05_gather", 0) > 0 and fused["losses"][-1] < fused["losses"][0])
+                and fused["launches"].get("gemm_gather", 0) > 0 and fused["losses"][-1] < fused["losses"][0])
         ok = ok and good
         report["graphs" if graphs else "eager"] = {"max_loss_diff": dl, "max_param_diff": dp, "ok": good, "losses_base": base["losses"][-3:],
                                                    "losses_fused": fused["losses"][-3:], "fused": fused["fused"], "backend": fused["backend"],
-                                                   "gather_gemm_launches": fused["launches"].get("gemm_tcgen05_gather", 0),
+                                                   "gather_gemm_launches": fused["launches"].get("gemm_gather", 0),
                                                    "rank_divergence": fused["rank_divergence"], "base_rank_divergence": base["rank_divergence"], "bad": fused["bad"]}
     flag = torch.tensor([1 if ok else 0], device="cuda")
     dist.all_reduce(flag, op=dist.ReduceOp.MIN)
     report["ok"] = bool(flag.item())
     if env.rank == 0:
         print(json.dumps(report, indent=1))
-        out = os.path.join(ROOT, "gpurun_out", "fused_ag_check.json")
+        out = os.path.join(ROOT, "results", "fused_ag_check.json")
         os.makedirs(os.path.dirname(out), exist_ok=True)
         json.dump(report, open(out, "w"), indent=1)
     dist.barrier()

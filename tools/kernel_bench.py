@@ -2,7 +2,7 @@
 """Isolated timing of every hand-written kernel at the Llama-125M shapes (T = 8x1024 tokens), with achieved
 HBM bandwidth / tensor throughput against MEASURED_PEAKS.json.  L2 is flushed between timed launches.
 
-    python tools/kernel_bench.py [--only rmsnorm,ce,...] [--iters 20] [--out profiles/kernel_bench.json]
+    python tools/kernel_bench.py [--only rmsnorm,ce,...] [--iters 20] [--out kernel_bench.json]
 Also the target of `ncu --set full -k regex:<kernel>` captures (use --iters 1 --no-flush)."""
 import argparse
 import json
@@ -103,7 +103,7 @@ def main():
     rec("adamw_shard_tentative", lambda: ops.fused_adamw_shard(g, opt.master, opt.exp_avg, opt.exp_avg_sq, opt.stash, out, hp2), bytes_=N * (2 + 12 + 4 + 2))
     for (M, Nn, K) in ((T, 3 * H, H), (T, 2 * I, H), (T, H, I), (T, Vp, H), (8192, 8192, 8192)):
         xa, wb = bf(M, K), bf(Nn, K)
-        rec(f"gemm_tcgen05_{M}x{Nn}x{K}", lambda: gemm_tn(xa, wb), flops=2.0 * M * Nn * K)
+        rec(f"gemm_{M}x{Nn}x{K}", lambda: gemm_tn(xa, wb), flops=2.0 * M * Nn * K)
         rec(f"gemm_cublas_{M}x{Nn}x{K}", lambda: torch.nn.functional.linear(xa, wb), flops=2.0 * M * Nn * K)
     if a.out:
         os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)

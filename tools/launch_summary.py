@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Summarise an `ncu --metrics gpu__time_duration.sum --csv` launch log: time per kernel name.
 
-    python tools/launch_summary.py gpurun_out/launches.csv [--last N] [--top K]
+    python tools/launch_summary.py results/launches.csv [--last N] [--top K]
 """
 import csv
 import io

@@ -1,10 +1,11 @@
 #!/usr/bin/env python
 """Per-GPU memory plan of a training configuration (no GPU needed):
 
-    python tools/memory_plan.py --model llama3-8b --gpus 8 --batch 4 --seq 512 [--n-acc 2]
+    python tools/memory_plan.py --model llama3-1b --gpus 8 --batch 4 --seq 512
 
-Persistent buffers are exact (they follow the arena / optimizer layout: SURVEY 2.7, DESIGN section 2); activations are an estimate
-of what the native Llama keeps for backward (bf16 tensors saved by the fused ops + the padded logits).  B200: 180 GB of HBM3e."""
+Persistent buffers are exact (they follow the arena / optimizer layout: two bf16 parameter sets, two bf16 gradient accumulators and
+the fp32 optimizer shard); activations are an estimate of what the native Llama keeps for backward (bf16 tensors saved by the
+fused ops + the padded logits).  Budget: an 80 GB H100, of which 92 % is planned."""
 import argparse
 import json
 import os
@@ -45,12 +46,12 @@ def plan(cfg: LlamaConfig, world: int, batch: int, seq: int, method: str = "acco
     buffers["activations kept for backward (estimate, one micro-batch)"] = acts
     total = sum(buffers.values())
     return {"parameters": n, "size_slice": lay.size_slice, "buffers_gb": {k: v / GB for k, v in buffers.items()}, "total_gb": total / GB,
-            "fits_180gb": total < 0.92 * 180e9}
+            "fits_80gb": total < 0.92 * 80e9}
 
 
 def main(argv=None):
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", default="llama3-8b", choices=[k for k, (a, _) in PRESETS.items() if a == "llama"])
+    ap.add_argument("--model", default="llama3-1b", choices=[k for k, (a, _) in PRESETS.items() if a == "llama"])
     ap.add_argument("--gpus", type=int, default=8)
     ap.add_argument("--batch", type=int, default=4)
     ap.add_argument("--seq", type=int, default=512)

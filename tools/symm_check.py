@@ -8,8 +8,7 @@ tentative / real ...) on rank-specific random gradients with rank-specific micro
 BOTH backends, and after every round checks: identical global counts; fp32 master / Adam state /
 stash agree with the NCCL+fused-local-AdamW path within bf16-reduction tolerance; the gathered
 parameters are bit-identical on all ranks; the consumed accumulator is zero.  Then it times the
-round (CUDA events, max over ranks) and reports achieved NVLink bytes/s against the 770 GB/s/dir
-measured peer-copy figure (B200_PROFILING.md) and the HBM floor.
+round (CUDA events, max over ranks) and reports achieved NVLink bytes/s and the HBM floor.
 """
 import argparse
 import json
@@ -227,8 +226,8 @@ def main():
         hbm_bytes = S * (2 * W + 12 + 12 + 2 * W) + ar.layout.padded * 2   # reads+writes incl. accumulator zeroing
         report.setdefault("timing", {})[key] = {
             "backend": be.name, "ms_median": ms, "ms_min": min(times), "numel": n, "slice": S,
-            "nvlink_GBps_per_dir": link_bytes / (ms * 1e-3) / 1e9, "nvlink_frac_of_770": link_bytes / (ms * 1e-3) / 770e9,
-            "roofline_ms": max(link_bytes / 770e9, hbm_bytes / 6.46e12) * 1e3,
+            "nvlink_GBps_per_dir": link_bytes / (ms * 1e-3) / 1e9, "nvlink_frac_of_450": link_bytes / (ms * 1e-3) / 450e9,
+            "roofline_ms": max(link_bytes / 450e9, hbm_bytes / 3.35e12) * 1e3,
         }
         del be, ar, opt
         torch.cuda.empty_cache()
