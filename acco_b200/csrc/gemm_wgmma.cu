@@ -24,14 +24,19 @@
 //                                  with a cluster of pm x pn CTAs the CTAs of a row share their A tile and the CTAs of a column
 //                                  their B tile: each loads its share and TMA-multicasts it
 //   warpgroups 1-2 : consumers   - wgmma.mma_async m64nBNk16 on 64 rows each, accumulators in registers, one wgmma group in flight;
-//                                  release a stage to every CTA that wrote into it, then the epilogue (+bias, bf16, global store /
-//                                  exact fp32 read-modify-write for beta = 1 / bf16x2 atomic add for split-K partial sums)
+//                                  release a stage to every CTA that wrote into it, then the epilogue: +bias, bf16, staged through
+//                                  shared memory in 64 x 64 sub-tiles and written by TMA (store / bulk bf16 add for split-K partial
+//                                  sums); for beta = 1 with one K split the C sub-tile is TMA-loaded into the staging buffer while
+//                                  the mainloop runs and added in fp32 (one rounding).  The warpgroup does not wait for the stores:
+//                                  it goes on to its next tile and only reuses a staging buffer once its store has read it.
 //
 // Operand layouts in shared memory (wgmma canonical layouts, 128-byte swizzle):
 //   K-major  : rows of 64 k (128 B), 8-row swizzle atoms 1024 B apart (SBO); one TMA box {64 k, rows}
 //   MN-major : one TMA box {64 mn, 64 k} gives 64 rows (k) of 128 B = 8 KiB per 64-mn chunk;
 //              SBO = 1024 B between 8-k groups, LBO = 8192 B between 64-mn chunks; advancing K by 16 = +2048 B
 // In both layouts the 64-row half of the A tile that consumer warpgroup w multiplies starts 8 KiB * w into the stage.
+// Output staging: each consumer warpgroup owns two 8 KiB buffers of 64 rows x 64 columns (128 B per row, 128-byte swizzle: the
+// 16-byte chunk c of row r sits at chunk c ^ (r % 8)), the box of the output tensor map.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -51,7 +56,9 @@ constexpr int BM = 128, BN_MAX = 256, BK = 64;
 constexpr int A_BYTES = BM * BK * 2;               // 16 KiB per stage
 constexpr int RING_BYTES = 192 * 1024;             // 4 x 48 KiB (BN 256), 6 x 32 KiB (BN 128), 8 x 24 KiB (BN 64)
 constexpr int MAX_STAGES = 8;
-constexpr int SMEM_BYTES = RING_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+constexpr int EPI_BUF_BYTES = 64 * 64 * 2;         // one 64 x 64 bf16 output sub-tile
+constexpr int EPI_BYTES = 2 * 2 * EPI_BUF_BYTES;   // 2 consumer warpgroups x 2 buffers
+constexpr int SMEM_BYTES = RING_BYTES + EPI_BYTES + 1024 /*align*/ + 256 /*barriers*/;   // 230,656 B of the 232,448 B opt-in
 constexpr int THREADS = 384;
 constexpr int MAX_PEERS = 8;
 constexpr int MN_CHUNK_BYTES = 64 * BK * 2;        // one {64 mn, 64 k} box of an MN-major operand
@@ -60,6 +67,7 @@ struct Params {
     CUtensorMap map_a;                 // K-major: box {64 k, 128 / pn rows} of A [M, K]; MN-major: box {64 m, 64 k} of A^T [K, M]
     CUtensorMap map_b;                 // K-major: box {64 k, BN / pm rows} of B [N, K]; MN-major: box {64 n, 64 k} of B^T [K, N]
     CUtensorMap map_b_peer[MAX_PEERS]; // gather mode: B on each rank (peer-mapped), box {64 k, BN rows}
+    CUtensorMap map_d;                 // D [M, N] with row stride ldd, box {64 n, 64 m}: its extents clip ragged tiles
     const __nv_bfloat16* bias;         // optional [N]
     const int* tile_owner;             // [num_n] : -1 -> local copy is valid, r -> gather from rank r
     uint32_t* flags;                   // [num_n * num_k * 2] ready epochs
@@ -74,7 +82,8 @@ struct Params {
     int gather;                        // 0: plain GEMM (tile_owner ignored)
     int stages, stage_bytes;           // smem ring geometry: stages x (16 KiB of A + BN * 128 B of B)
     int pm, pn;                        // cluster = pm x pn CTAs: the pn CTAs of a row share A, the pm CTAs of a column share B
-    unsigned long long* dbg;           // optional: CTA 0 writes %globaltimer stamps of its phases (tools/gemm_timeline.py)
+    int band;                          // tile order: bands of `band` super-tile columns (decode_unit)
+    unsigned long long* dbg;          // optional: CTA 0 writes %globaltimer stamps of its phases (tools/gemm_timeline.py)
 };
 
 __device__ __forceinline__ void wait_flag_gpu(const uint32_t* f, uint32_t epoch) {
@@ -104,15 +113,24 @@ __device__ __forceinline__ void stamp(const Params& P, int slot) {
 // super-tile of pm x pn adjacent tiles; CTA (pi, pj) computes tile (smb * pm + pi, sn * pn + pj).  Tiles beyond the matrix (odd
 // counts) are phantom: their loads are zero-filled by TMA and nothing is stored, but the CTA still contributes its share of the
 // multicast operand loads.
+// Tile order inside a split: bands of `band` super-tile columns; inside a band the columns go fastest, then the rows, then the next
+// band.  band = num_sn is plain row-major order.  A narrower band keeps the B blocks of one band L2-resident while every row of A
+// passes by (the host picks it only when all of A stays in L2), so B is read from HBM about once instead of once per wave.
+// Gather mode uses band = num_sn: every waiter unit (m-block > 0) of a column comes after that column's gatherer unit (m-block 0)
+// in every CTA's sequence of units, which its flag protocol needs.
 struct Unit {
     int mb, n_blk, kb0, kb1;
 };
-__device__ __forceinline__ Unit decode_unit(int t, int tiles, int num_sn, int num_k, int kb_per_split, int pm, int pn, int pi, int pj) {
+__device__ __forceinline__ Unit decode_unit(int t, int tiles, int num_smb, int num_sn, int band, int num_k, int kb_per_split, int pm, int pn,
+                                            int pi, int pj) {
     Unit u;
     const int s = t / tiles, tile = t - s * tiles;
-    const int smb = tile / num_sn;
+    const int bi = tile / (band * num_smb), sn0 = bi * band;
+    const int width = min(band, num_sn - sn0);
+    const int r = tile - sn0 * num_smb;
+    const int smb = r / width;
     u.mb = smb * pm + pi;
-    u.n_blk = (tile - smb * num_sn) * pn + pj;
+    u.n_blk = (sn0 + r - smb * width) * pn + pj;
     u.kb0 = s * kb_per_split;
     u.kb1 = min(num_k, u.kb0 + kb_per_split);
     return u;
@@ -130,8 +148,10 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_kernel(const __grid_constant_
     extern __shared__ uint8_t smem_raw[];
     if (threadIdx.x == 0) stamp(P, 0);
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);   // SWIZZLE_128B needs 1024 B alignment
-    uint64_t* full_bar = (uint64_t*)(smem + RING_BYTES);      // [MAX_STAGES]  TMA bytes landed
+    uint8_t* epi_smem = smem + RING_BYTES;                    // [2 x 2] output staging buffers (1024 B aligned)
+    uint64_t* full_bar = (uint64_t*)(epi_smem + EPI_BYTES);   // [MAX_STAGES]  TMA bytes landed
     uint64_t* empty_bar = full_bar + MAX_STAGES;              // [MAX_STAGES]  stage reusable (every consumer that reads it released it)
+    uint64_t* c_bar = empty_bar + MAX_STAGES;                 // [2 x 2]       C sub-tile landed in a staging buffer (beta = 1)
 
     constexpr int B_BYTES = BN * BK * 2;
     const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
@@ -141,8 +161,9 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_kernel(const __grid_constant_
     const int pi = (int)cl_rank / pn, pj = (int)cl_rank - pi * pn;
     const int unit0 = blockIdx.x / cl_size, unit_stride = gridDim.x / cl_size;
     const int num_n = (P.N + BN - 1) / BN, num_k = (P.K + BK - 1) / BK, num_mb = (P.M + BM - 1) / BM;
-    const int num_sn = (num_n + pn - 1) / pn;
-    const int tiles = ((num_mb + pm - 1) / pm) * num_sn;
+    const int num_sn = (num_n + pn - 1) / pn, num_smb = (num_mb + pm - 1) / pm;
+    const int band = P.band;
+    const int tiles = num_smb * num_sn;
     const int num_units = tiles * P.splits;
     const int kbs = P.kb_per_split;
     // multicast masks (cluster ranks): the CTAs of my row share my A tile, the CTAs of my column my B tile.  The same set (row and
@@ -155,10 +176,12 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_kernel(const __grid_constant_
     if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&P.map_a) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&P.map_b) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&P.map_d) : "memory");
         for (int s = 0; s < n_stages; ++s) {
             mbar_init(&full_bar[s], 1);
             mbar_init(&empty_bar[s], 2u * (uint32_t)(pm + pn - 1));   // both consumer warpgroups of every CTA that reads what I (multi)cast
         }
+        for (int b = 0; b < 4; ++b) mbar_init(&c_bar[b], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -185,7 +208,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_kernel(const __grid_constant_
             const int nbch = (BN / 64) / pm, b_ch0 = pi * nbch;               // MN-major B: 64-n chunks [b_ch0, b_ch0 + nbch)
             const bool mc_a = pn > 1, mc_b = pm > 1;
             for (int t = unit0; t < num_units; t += unit_stride) {
-                const Unit u = decode_unit(t, tiles, num_sn, num_k, kbs, pm, pn, pi, pj);
+                const Unit u = decode_unit(t, tiles, num_smb, num_sn, band, num_k, kbs, pm, pn, pi, pj);
                 const int n_blk = u.n_blk;
                 const int m0 = u.mb * BM, n0 = n_blk * BN;
                 const int owner = P.gather ? P.tile_owner[n_blk] : -1;
@@ -261,13 +284,31 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_kernel(const __grid_constant_
             if (cl_size > 1) mbar_arrive_cluster_addr(map_to_cta(&empty_bar[s], (uint32_t)tid));
             else mbar_arrive(&empty_bar[s]);
         };
+        // epilogue: BN / 64 sub-tiles of 64 x 64 through this warpgroup's two staging buffers (sub-tile s uses buffer s % 2); thread 0
+        // of the warpgroup issues the TMA traffic.  Before a buffer is rewritten, the store that last read it must be done reading:
+        // the bulk group two commits back (one back with a single sub-tile per tile).
+        constexpr int NSUB = BN / 64;
+        constexpr int NPRE = NSUB < 2 ? NSUB : 2;          // C sub-tiles prefetched during the mainloop (beta = 1, one split)
+        uint8_t* epi = epi_smem + cw * 2 * EPI_BUF_BYTES;
+        uint64_t* cbar = c_bar + cw * 2;
+        const bool load_c = P.reduce && !P.atomic;
+        const int bar_id = 1 + cw;                         // named barrier of this warpgroup (0 is __syncthreads)
+        uint32_t c_phase = 0;                              // bit b: parity of cbar[b]
+        auto wait_buffer_free = [&]() {
+            if (NSUB == 1) bulk_wait_read<0>();
+            else bulk_wait_read<1>();
+        };
+        auto load_c_sub = [&](const Unit& u, int s) {
+            mbar_expect_tx(&cbar[s & 1], (uint32_t)EPI_BUF_BYTES);
+            tma_load_2d(&P.map_d, &cbar[s & 1], epi + (s & 1) * EPI_BUF_BYTES, u.n_blk * BN + s * 64, u.mb * BM + cw * 64);
+        };
         float acc[BN / 2];
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
         int stage = 0;
         uint32_t phase = 0;
         for (int t = unit0; t < num_units; t += unit_stride) {
-            const Unit u = decode_unit(t, tiles, num_sn, num_k, kbs, pm, pn, pi, pj);
+            const Unit u = decode_unit(t, tiles, num_smb, num_sn, band, num_k, kbs, pm, pn, pi, pj);
             int prev = -1;
             for (int kb = u.kb0; kb < u.kb1; ++kb) {
                 mbar_wait(&full_bar[stage], phase);
@@ -282,6 +323,11 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_kernel(const __grid_constant_
                     mma_k16<BN, A_MN, B_MN>(acc, da, db, (uint32_t)((kb > u.kb0) | (k != 0)));
                 }
                 wgmma_commit();
+                if (load_c && kb == u.kb0 && tid == 0) {
+                    // beta = 1: fetch the first C sub-tiles now, their latency hides behind this tile's mainloop
+                    bulk_wait_read<0>();
+                    for (int s = 0; s < NPRE; ++s) load_c_sub(u, s);
+                }
                 if (prev >= 0) {
                     wgmma_wait<1>();                   // the previous stage's wgmmas have retired: hand it back
                     release(prev);
@@ -292,39 +338,61 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_kernel(const __grid_constant_
             wgmma_wait<0>();
             reg_fence(acc);
             release(prev);
-            // ---------------- epilogue: fragment (row 16 warp + lane/4 (+8), columns 8 j + 2 (lane % 4) (+1)) -> global
-            const int row0 = u.mb * BM + cw * 64 + warp * 16 + (lane >> 2);
+            // ---------------- epilogue: fragment (row 16 warp + lane/4 (+8), columns 8 j + 2 (lane % 4) (+1)) -> staging -> TMA
+            const int m0 = u.mb * BM + cw * 64;
+            // my rows r = 16 warp + lane / 4 (+8) of the 64-row half; r % 8 = lane / 4 sets the swizzle of both
+            const uint32_t row_addr = smem_u32(epi) + (uint32_t)((warp * 16 + (lane >> 2)) * 128 + 4 * (lane & 3));
             const int colb = u.n_blk * BN + 2 * (lane & 3);
             const bool bias_on = P.bias != nullptr && u.kb0 == 0;
 #pragma unroll
-            for (int j = 0; j < BN / 8; ++j) {
-                const int col = colb + 8 * j;
-                if (col >= P.N) continue;                              // N % 8 == 0: col < N implies col + 1 < N
-                float b0 = 0.f, b1 = 0.f;
-                if (bias_on) {
-                    const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(P.bias + col));
-                    b0 = f.x; b1 = f.y;
+            for (int s = 0; s < NSUB; ++s) {
+                uint8_t* buf = epi + (s & 1) * EPI_BUF_BYTES;
+                const uint32_t buf_addr = row_addr + (uint32_t)((s & 1) * EPI_BUF_BYTES);
+                if (load_c) {
+                    if (s >= NPRE && tid == 0) {
+                        wait_buffer_free();
+                        load_c_sub(u, s);
+                    }
+                    mbar_wait(&cbar[s & 1], (c_phase >> (s & 1)) & 1u);
+                    c_phase ^= 1u << (s & 1);
+                } else {
+                    if (tid == 0) wait_buffer_free();
+                    named_barrier(bar_id, 128);
                 }
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int row = row0 + 8 * h;
-                    if (row >= P.M) continue;
-                    float v0 = acc[4 * j + 2 * h] + b0, v1 = acc[4 * j + 2 * h + 1] + b1;
-                    __nv_bfloat16* dst = P.out + (size_t)row * (size_t)P.ldd + col;
-                    if (P.atomic) {
-                        __nv_bfloat162 hv = __floats2bfloat162_rn(v0, v1);
-                        asm volatile("red.global.add.noftz.bf16x2 [%0], %1;" ::"l"(dst), "r"(*reinterpret_cast<uint32_t*>(&hv)) : "memory");
-                        continue;
+                for (int jj = 0; jj < 8; ++jj) {
+                    const int j = s * 8 + jj;
+                    const int col = colb + 8 * j;
+                    float b0 = 0.f, b1 = 0.f;
+                    if (bias_on && col < P.N) {                    // N % 8 == 0: col < N implies col + 1 < N
+                        const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(P.bias + col));
+                        b0 = f.x; b1 = f.y;
                     }
-                    if (P.reduce) {
-                        // beta = 1 with a single K split: exact fp32 accumulate (one rounding), nobody else touches this tile
-                        const float2 c = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(dst));
-                        v0 += c.x; v1 += c.y;
+                    const uint32_t chunk_addr = buf_addr + (uint32_t)((jj ^ (lane >> 2)) << 4);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const uint32_t dst = chunk_addr + h * 8 * 128;
+                        float v0 = acc[4 * j + 2 * h] + b0, v1 = acc[4 * j + 2 * h + 1] + b1;
+                        if (load_c) {
+                            // beta = 1 with a single K split: exact fp32 accumulate (one rounding), nobody else touches this tile
+                            const uint32_t cv = ld_shared_u32(dst);
+                            const float2 c = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&cv));
+                            v0 += c.x; v1 += c.y;
+                        }
+                        st_shared_u32(dst, pack_bf16x2(v0, v1));
                     }
-                    *reinterpret_cast<__nv_bfloat162*>(dst) = __floats2bfloat162_rn(v0, v1);
+                }
+                fence_async_smem();                        // my st.shared -> visible to the TMA engine
+                named_barrier(bar_id, 128);
+                if (tid == 0) {
+                    // ragged rows / columns fall outside map_d's extents and are dropped by the TMA unit
+                    if (P.atomic) tma_reduce_add_2d(&P.map_d, buf, u.n_blk * BN + s * 64, m0);
+                    else tma_store_2d(&P.map_d, buf, u.n_blk * BN + s * 64, m0);
+                    bulk_commit();
                 }
             }
         }
+        if (tid == 0) bulk_wait<0>();                      // the stores have landed before this CTA retires
         if (cw == 0 && tid == 0) stamp(P, 7);
     }
 
@@ -498,7 +566,8 @@ struct Config {
 
 // Tile / split-K / cluster choice: minimise (waves x per-unit cost).  Per k-block a CTA's tensor cores need 4 * bn cycles
 // (128 x bn x 64 multiply-adds at 2048 per clock on an H100 SM) and the operand bytes must come in through L2 (~64 B/clk/SM
-// assumed); the epilogue is not overlapped with the CTA's own mainloop.  Split-K needs an adding epilogue: accumulating GEMMs
+// assumed); `epi` charges the epilogue as if it were not overlapped (its TMA stores now drain while the next tile's mainloop runs,
+// so this over-estimates it; the picks are kept as they are).  Split-K needs an adding epilogue: accumulating GEMMs
 // (wgrad), or a zero-filled output.
 static Config choose_config(int M, int N, int K, int a_mn, int b_mn, int reduce, int sms, int bn_req, int splits_req, int pm_req, int pn_req) {
     (void)a_mn; (void)b_mn;
@@ -550,6 +619,26 @@ static Config choose_config(int M, int N, int K, int a_mn, int b_mn, int reduce,
     return bc;
 }
 
+// Tile order (decode_unit): bands of G super-tile columns.  When all of A [M, K] fits in a third of L2 it stays resident while
+// the tiles of a band go by, and G is as wide as keeps the band's B blocks (bn_cols x K each) within an eighth of L2: each B block
+// is then read from HBM once.  Otherwise (or when all of B fits anyway) row-major order, G = num_sn.  For the Llama-125M LM-head
+// forward (A = 8192 x 768, B = 50304 x 768, 256-row blocks) on an H100 (50 MB L2) that is G = 16 instead of one 77 MB pass over
+// the weight per 132-tile wave.
+static int tile_band(int M, int K, int bn_cols, int num_sn) {
+    static int l2_cache[64] = {0};
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) { cudaGetLastError(); return num_sn; }
+    if (l2_cache[dev] == 0) {
+        int l2 = 0;
+        if (cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev) != cudaSuccess || l2 <= 0) { cudaGetLastError(); l2 = -1; }
+        l2_cache[dev] = l2;
+    }
+    const double l2 = (double)l2_cache[dev];
+    if (l2 <= 0 || (double)M * K * 2.0 > l2 / 3.0) return num_sn;
+    const long long g = (long long)(l2 / 8.0 / ((double)bn_cols * K * 2.0));
+    return (int)(g < 1 ? 1 : (g > num_sn ? num_sn : g));
+}
+
 struct GatherArgs {
     const void* const* peers;
     int n_peers;
@@ -598,6 +687,9 @@ static int launch(const void* a, long long lda, int a_mn, const void* b, long lo
             P.map_b_peer[i] = P.map_b;
         }
     }
+    // the output map spans exactly the (M, N) view of D: the TMA stores of ragged tiles cannot reach the elements around it
+    rc = make_map(&P.map_d, d, (uint64_t)N, (uint64_t)M, (uint64_t)ldd, 64, 64);
+    if (rc) return rc;
     P.bias = (const __nv_bfloat16*)bias;
     P.out = (__nv_bfloat16*)d;
     P.ldd = ldd;
@@ -629,9 +721,11 @@ static int launch(const void* a, long long lda, int a_mn, const void* b, long lo
     const int num_n = (N + bn - 1) / bn;
     const int num_mb = (M + BM - 1) / BM;
     const int cl = pm * pn;
-    const long long units = (long long)((num_mb + pm - 1) / pm) * ((num_n + pn - 1) / pn) * P.splits;
+    const int num_sn = (num_n + pn - 1) / pn;
+    const long long units = (long long)((num_mb + pm - 1) / pm) * num_sn * P.splits;
     const int slots = cl > 1 ? max_clusters(cl, sms) : sms;
     if (slots <= 0) return -5;
+    P.band = gather ? num_sn : tile_band(M, K, bn * pn, num_sn);
     const int grid = (int)(units < (long long)slots ? units : (long long)slots) * cl;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid);

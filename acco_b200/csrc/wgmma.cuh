@@ -67,6 +67,19 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void*
                  "r"(c0), "r"(c1)
                  : "memory");
 }
+// element-wise add of the box into global memory (the add is done at the destination, in its data type)
+__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* map, const void* smem, int c0, int c1) {
+    asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map),
+                 "r"(smem_u32(smem)), "r"(c0), "r"(c1)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups still read their shared-memory source (their global writes may still be in flight)
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// at most N of this thread's bulk groups are incomplete (global writes done)
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -111,6 +124,17 @@ __device__ __forceinline__ void reg_fence(float (&d)[R]) {
     for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 __device__ __forceinline__ void named_barrier(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+// 32-bit shared-window addresses keep the epilogue's address arithmetic off 64-bit registers
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
+__device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
+    __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+    return *reinterpret_cast<uint32_t*>(&h);
+}
 
 // 8 fp32 -> 8 bf16 (16 bytes)
 __device__ __forceinline__ uint4 pack_bf16x8(const float* f) {

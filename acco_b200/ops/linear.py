@@ -56,7 +56,7 @@ _SIDE_STREAMS = {}
 
 def _wgrad_stream(device):
     """``ACCO_WGRAD_STREAM=1``: run the wgrad GEMM on a side stream next to the dgrad GEMM (fork / join, CUDA-graph capturable).  The
-    backward GEMMs of a 125M-class layer have 48-72 tiles for 74 CTA pairs, so each leaves 20-35 % of the SMs idle on its own; the two
+    backward GEMMs of a 125M-class layer mostly have fewer output tiles than the H100's 132 SMs, so each leaves SMs idle on its own; the two
     are independent (both only read dY) and fill each other's gaps when they run concurrently."""
     if os.environ.get("ACCO_WGRAD_STREAM", "0") != "1" or device.type != "cuda":
         return None

@@ -6,7 +6,7 @@
     python tools/dump_sass.py --check      # exit 1 if the committed summary does not describe the built binary
 
 The summary counts, per listed kernel, the SASS mnemonics that show the Hopper-native path: `HGMMA` = wgmma.mma_async,
-`UTMALDG` / `UTMASTG` = TMA load / store, `SYNCS` = mbarrier operations, `USETMAXREG` = setmaxnreg, `REDG` = the split-K atomic
+`UTMALDG` / `UTMASTG` = TMA load / store, `SYNCS` = mbarrier operations, `USETMAXREG` = setmaxnreg, `REDG` = per-element atomic
 adds, `LDGMC` = multimem.ld_reduce ...  `tests/test_sass_listings.py` runs the --check so a stale summary cannot be committed."""
 import json
 import os

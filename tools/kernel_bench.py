@@ -47,7 +47,7 @@ def main():
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     only = set(x for x in a.only.split(",") if x)
-    peaks = {"hbm_gbs": 6462.4, "bf16_tflops": 1686.0}
+    peaks = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}        # H100 SXM data sheet: HBM3 bandwidth, dense bf16
     try:
         peaks.update(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))))
     except Exception:
