@@ -15,6 +15,10 @@
 //   query heads of the GQA group and the visible 64-query blocks):  S^T = K Q^T, P^T = exp2(S^T c - LSE), dP^T = V dO^T,
 //   dS^T = P^T (dP^T - Delta) * scale;  dV += P^T dO, dK += dS^T Q in registers;  dS goes through shared memory for dQ = dS K,
 //   which is added (fp32 atomics) into a zero-filled dQ accumulator.  P and dS are rounded to bf16 before their products.
+// Document masking (kSeg = true, packed fine-tuning rows): `seg[b*S + s]` is the first position of the sample that holds token s, so
+//   key kv is visible from query q iff  seg[q] <= kv <= q  and  kv > q - window.  Within a row `seg` is non-decreasing; the loop bounds
+//   below depend on that (the first query of a block has the block's smallest segment start).  kSeg = false is the plain causal /
+//   sliding-window kernel.
 // Delta = rowsum(dO * O) comes from `attn_delta_kernel`.  `attention_blockwise_ref` / `attention_blockwise_bwd_ref`
 // (ops/attention.py) give the fp32 reference semantics of the same masking and rounding points.
 #include <cuda.h>
@@ -115,6 +119,7 @@ struct FwdParams {
     float* lse;
     int B, S, Hq, Hk, window;
     float scale;
+    const int* seg;                    // [B*S] segment starts (kSeg only)
 };
 
 constexpr int FWD_Q = 128, FWD_KV = 64, FWD_THREADS = 256;
@@ -137,6 +142,7 @@ __device__ __forceinline__ void wgmma_m64n64k16_rs_tb(float (&d)[32], const uint
 // One CTA = 128 queries of one head = two warpgroups of 64 rows.  Thread 0 TMA-loads Q once and the K / V blocks of 64 keys through a
 // 2-stage ring (128-byte swizzle, mbarrier transaction counts); S = Q K^T and O += P V run as wgmma (P straight from the registers
 // holding S); the CTA barrier at the end of a block is what frees its stage for the block two ahead.
+template <bool kSeg>
 __global__ void __launch_bounds__(FWD_THREADS) attn_fwd_kernel(const __grid_constant__ FwdParams P) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);   // SWIZZLE_128B needs 1024 B alignment
@@ -148,7 +154,8 @@ __global__ void __launch_bounds__(FWD_THREADS) attn_fwd_kernel(const __grid_cons
     const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, t = lane & 3;
     const int q0 = qb * FWD_Q;
     const int row0 = b * P.S;
-    const int lo_key = max(0, q0 - P.window + 1);
+    int lo_key = max(0, q0 - P.window + 1);
+    if constexpr (kSeg) lo_key = max(lo_key, P.seg[row0 + q0]);
     const int j_lo = lo_key / FWD_KV, j_hi = (q0 + FWD_Q - 1) / FWD_KV;
     auto issue = [&](int j) {                                      // thread 0: K_j, V_j into stage (j - j_lo) & 1
         const int s = (j - j_lo) & 1;
@@ -175,12 +182,18 @@ __global__ void __launch_bounds__(FWD_THREADS) attn_fwd_kernel(const __grid_cons
     for (int i = 0; i < 32; ++i) o[i] = 0.f;
     const int wq_lo = q0 + wg * 64, wq_hi = wq_lo + 63;
     const int qr[2] = {wq_lo + warp * 16 + g, wq_lo + warp * 16 + g + 8};
+    int sg[2] = {0, 0}, wseg = 0;                                  // segment starts of this thread's rows / of the warpgroup's first row
+    if constexpr (kSeg) {
+        sg[0] = P.seg[row0 + qr[0]];
+        sg[1] = P.seg[row0 + qr[1]];
+        wseg = P.seg[row0 + wq_lo];
+    }
     const uint32_t q_addr = smem_u32(sQ) + (uint32_t)(wg * 8192);
     for (int j = j_lo; j <= j_hi; ++j) {
         const int kv0 = j * FWD_KV, s = (j - j_lo) & 1;
         mbar_wait(&full[s], (uint32_t)(((j - j_lo) >> 1) & 1));
         // this warpgroup's rows see nothing of this block: skip the math (uniform per warpgroup)
-        if (!(kv0 > wq_hi || kv0 + FWD_KV - 1 <= wq_lo - P.window)) {
+        if (!(kv0 > wq_hi || kv0 + FWD_KV - 1 <= wq_lo - P.window || (kSeg && kv0 + FWD_KV - 1 < wseg))) {
             const uint32_t k_addr = smem_u32(sKV + s * 2 * FWD_TILE_KV), v_addr = k_addr + FWD_TILE_KV;
             float sc[32];
 #pragma unroll
@@ -198,7 +211,7 @@ __global__ void __launch_bounds__(FWD_THREADS) attn_fwd_kernel(const __grid_cons
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
                     const int kv = kv0 + nb * 8 + 2 * t + (e & 1), r = e >> 1;
-                    const float v = visible(qr[r], kv, P.window) ? sc[4 * nb + e] * c : -INFINITY;
+                    const float v = visible(qr[r], kv, P.window) && (!kSeg || kv >= sg[r]) ? sc[4 * nb + e] * c : -INFINITY;
                     sc[4 * nb + e] = v;
                     mx[r] = fmaxf(mx[r], v);
                 }
@@ -270,11 +283,14 @@ struct BwdParams {
     bf16 *dk, *dv;                             // [B*S, Hk*64]
     int B, S, Hq, Hk, window;
     float scale;
+    const int* seg;                            // [B*S] segment starts (kSeg only)
 };
 
 constexpr int BWD_KV = 64, BWD_Q = 64, BWD_THREADS = 128;
 constexpr int BWD_SMEM = 8 * 64 * LDS * 2 + 2 * BWD_Q * 4;
+constexpr int BWD_SMEM_SEG = BWD_SMEM + (BWD_Q + 1) * 4;       // + the 64 queries' segment starts and a stop flag
 
+template <bool kSeg>
 __global__ void __launch_bounds__(BWD_THREADS) attn_bwd_kernel(const BwdParams P) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     bf16* sK = reinterpret_cast<bf16*>(smem_raw);   // [key][d]
@@ -287,6 +303,7 @@ __global__ void __launch_bounds__(BWD_THREADS) attn_bwd_kernel(const BwdParams P
     bf16* sdS = sdOt + 64 * LDS;                    // [q][key]
     float* sL = reinterpret_cast<float*>(sdS + 64 * LDS);   // LSE (log2 domain) of the 64 queries
     float* sD = sL + BWD_Q;                                  // Delta
+    int* sSeg = reinterpret_cast<int*>(sD + BWD_Q);          // kSeg only: segment starts of the 64 queries, then the stop flag
     const int nb_k = blockIdx.x, hk = blockIdx.y, b = blockIdx.z;
     const int G = P.Hq / P.Hk;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
@@ -317,7 +334,11 @@ __global__ void __launch_bounds__(BWD_THREADS) attn_bwd_kernel(const BwdParams P
                 const long long li = ((long long)b * P.Hq + hq) * P.S + q0 + tid;
                 sL[tid] = P.lse[li] * LOG2E;
                 sD[tid] = P.delta[li];
+                if constexpr (kSeg) sSeg[tid] = P.seg[row0 + q0 + tid];
             }
+            // kSeg: q0 >= kv0, so seg[q0] is the smallest segment start of block m and of every later one; the next block (and all
+            // after it) sees no key of this CTA once its first query's sample starts past the last key.  Loaded with this block's tiles.
+            if (kSeg && tid == BWD_Q) sSeg[BWD_Q] = m == m_hi || P.seg[row0 + q0 + BWD_Q] > kv0 + BWD_KV - 1;
             __syncthreads();
             // S^T = K Q^T and dP^T = V dO^T for this warp's 16 keys x 64 queries
             float s[8][4], dp[8][4];
@@ -332,7 +353,7 @@ __global__ void __launch_bounds__(BWD_THREADS) attn_bwd_kernel(const BwdParams P
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
                     const int ql = nb * 8 + 2 * t + (e & 1), q = q0 + ql, r = e >> 1;
-                    const float p = visible(q, kr[r], P.window) ? exp2f(s[nb][e] * c - sL[ql]) : 0.f;
+                    const float p = visible(q, kr[r], P.window) && (!kSeg || kr[r] >= sSeg[ql]) ? exp2f(s[nb][e] * c - sL[ql]) : 0.f;
                     const float pb = __bfloat162float(__float2bfloat16(p));
                     s[nb][e] = pb;                                                          // P^T (bf16 values)
                     dp[nb][e] = __bfloat162float(__float2bfloat16(p * (dp[nb][e] - sD[ql]) * P.scale));   // dS^T
@@ -362,6 +383,7 @@ __global__ void __launch_bounds__(BWD_THREADS) attn_bwd_kernel(const BwdParams P
                     atomicAdd(dst + nb * 8 + 1, dq[nb][2 * r + 1]);
                 }
             }
+            if (kSeg && sSeg[BWD_Q]) break;                // written before the barrier above, rewritten after the next one
         }
     }
 #pragma unroll
@@ -421,13 +443,16 @@ extern "C" int acco_attn_supported(int B, int S, int Hq, int Hk, int D, float sc
 }
 
 // O = softmax(scale * Q K^T + causal/window mask) V.   q, k, v: column blocks (row stride ld elements) of [B*S, .] activations;
-// o [B*S, Hq*64] (row stride ld_o); lse [B, Hq, S] fp32.  window <= 0 or >= S: plain causal.
+// o [B*S, Hq*64] (row stride ld_o); lse [B, Hq, S] fp32.  window <= 0 or >= S: plain causal.  seg: nullptr, or int32 [B*S] segment
+// starts (document masking; non-decreasing within each row, seg[s] <= s).
 extern "C" int acco_attn_fwd(const void* q, const void* k, const void* v, long long ld, void* o, long long ld_o, float* lse, int B, int S, int Hq,
-                             int Hk, int D, float scale, int window, cudaStream_t st) {
+                             int Hk, int D, float scale, int window, const int* seg, cudaStream_t st) {
     using namespace acco_attn;
     if (!shape_ok(B, S, Hq, Hk, D, scale) || !aligned(q, ld) || !aligned(k, ld) || !aligned(v, ld) || !aligned(o, ld_o)) return -1;
-    static int fwd_attr = (int)cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM);
+    static int fwd_attr = (int)cudaFuncSetAttribute(attn_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM);
+    static int fwd_attr_seg = (int)cudaFuncSetAttribute(attn_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM);
     if (fwd_attr) return fwd_attr;
+    if (fwd_attr_seg) return fwd_attr_seg;
     FwdParams P;
     const uint64_t rows = (uint64_t)B * S;
     // each map spans the whole activation (B*S rows, row stride ld); the head's 64 columns are selected by the box coordinate
@@ -436,26 +461,34 @@ extern "C" int acco_attn_fwd(const void* q, const void* k, const void* v, long l
     if (!rc) rc = acco_gemm::make_map_typed(&P.map_v, v, (uint64_t)Hk * HD, rows, (uint64_t)ld, HD, FWD_KV, 2);
     if (rc) return rc;
     P.o = (bf16*)o; P.ld_o = ld_o; P.lse = lse;
-    P.B = B; P.S = S; P.Hq = Hq; P.Hk = Hk; P.window = eff_window(S, window); P.scale = scale;
-    attn_fwd_kernel<<<dim3(S / FWD_Q, Hq, B), FWD_THREADS, FWD_SMEM, st>>>(P);
+    P.B = B; P.S = S; P.Hq = Hq; P.Hk = Hk; P.window = eff_window(S, window); P.scale = scale; P.seg = seg;
+    if (seg)
+        attn_fwd_kernel<true><<<dim3(S / FWD_Q, Hq, B), FWD_THREADS, FWD_SMEM, st>>>(P);
+    else
+        attn_fwd_kernel<false><<<dim3(S / FWD_Q, Hq, B), FWD_THREADS, FWD_SMEM, st>>>(P);
     return (int)cudaGetLastError();
 }
 
 // Gradients of acco_attn_fwd.  d_o [B*S, Hq*64] (row stride ld_do); delta [B, Hq, S] fp32 scratch; dq_acc fp32 [B*S, Hq*64]
-// contiguous (zero-filled here, then added into by the kernel); dk, dv bf16 [B*S, Hk*64] contiguous.
+// contiguous (zero-filled here, then added into by the kernel); dk, dv bf16 [B*S, Hk*64] contiguous.  seg: as for acco_attn_fwd.
 extern "C" int acco_attn_bwd(const void* q, const void* k, const void* v, long long ld, const void* o, long long ld_o, const void* d_o,
                              long long ld_do, const float* lse, float* delta, float* dq_acc, void* dk, void* dv, int B, int S, int Hq, int Hk, int D,
-                             float scale, int window, cudaStream_t st) {
+                             float scale, int window, const int* seg, cudaStream_t st) {
     using namespace acco_attn;
     if (!shape_ok(B, S, Hq, Hk, D, scale) || !aligned(q, ld) || !aligned(k, ld) || !aligned(v, ld) || !aligned(o, ld_o) || !aligned(d_o, ld_do))
         return -1;
-    static int attr_rc = (int)cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
+    static int attr_rc = (int)cudaFuncSetAttribute(attn_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
+    static int attr_rc_seg = (int)cudaFuncSetAttribute(attn_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM_SEG);
     if (attr_rc) return attr_rc;
+    if (attr_rc_seg) return attr_rc_seg;
     const long long items = (long long)B * S * Hq;
     attn_delta_kernel<<<(unsigned)((items * 8 + 255) / 256), 256, 0, st>>>((const bf16*)o, (const bf16*)d_o, ld_o, ld_do, delta, B, S, Hq);
     if (cudaMemsetAsync(dq_acc, 0, (size_t)items * HD * sizeof(float), st) != cudaSuccess) return -6;
     BwdParams P{(const bf16*)q, (const bf16*)k, (const bf16*)v, ld, (const bf16*)d_o, ld_do, lse, delta, dq_acc, (bf16*)dk, (bf16*)dv,
-                B, S, Hq, Hk, eff_window(S, window), scale};
-    attn_bwd_kernel<<<dim3(S / BWD_KV, Hk, B), BWD_THREADS, BWD_SMEM, st>>>(P);
+                B, S, Hq, Hk, eff_window(S, window), scale, seg};
+    if (seg)
+        attn_bwd_kernel<true><<<dim3(S / BWD_KV, Hk, B), BWD_THREADS, BWD_SMEM_SEG, st>>>(P);
+    else
+        attn_bwd_kernel<false><<<dim3(S / BWD_KV, Hk, B), BWD_THREADS, BWD_SMEM, st>>>(P);
     return (int)cudaGetLastError();
 }

@@ -47,10 +47,10 @@ int acco_gemm_tile_n();
 int acco_gemm_tile_k();
 int acco_attn_supported(int B, int S, int Hq, int Hk, int D, float scale);
 int acco_attn_fwd(const void* q, const void* k, const void* v, long long ld, void* o, long long ld_o, float* lse, int B, int S, int Hq, int Hk,
-                  int D, float scale, int window, cudaStream_t st);
+                  int D, float scale, int window, const int* seg, cudaStream_t st);
 int acco_attn_bwd(const void* q, const void* k, const void* v, long long ld, const void* o, long long ld_o, const void* d_o, long long ld_do,
                   const float* lse, float* delta, float* dq_acc, void* dk, void* dv, int B, int S, int Hq, int Hk, int D, float scale, int window,
-                  cudaStream_t st);
+                  const int* seg, cudaStream_t st);
 }
 
 namespace {
@@ -489,21 +489,30 @@ static void check_rows(const torch::Tensor& t, int64_t rows, int64_t cols, const
     TORCH_CHECK(t.is_cuda() && t.scalar_type() == torch::kBFloat16 && t.dim() == 2 && t.size(0) == rows && t.size(1) == cols && t.stride(1) == 1 &&
                 t.stride(0) % 8 == 0 && (uintptr_t)t.data_ptr() % 16 == 0, name, " must be a [", rows, ", ", cols, "] CUDA bf16 matrix with 16-byte aligned rows");
 }
+// seg: None, or int32 [B*S] per-token segment starts (document masking of packed rows: key kv is visible from query s iff
+// seg[s] <= kv <= s; non-decreasing within a row)
+static const int* seg_ptr(const c10::optional<torch::Tensor>& seg, int64_t B, int64_t S) {
+    if (!seg.has_value() || !seg->defined()) return nullptr;
+    TORCH_CHECK(seg->is_cuda() && seg->scalar_type() == torch::kInt32 && seg->is_contiguous() && seg->numel() == B * S,
+                "seg must be a contiguous CUDA int32 tensor of B*S segment starts");
+    return seg->data_ptr<int>();
+}
 // qkv [B*S, (Hq + 2 Hk) * D] (rotary embedding already applied) -> {o [B*S, Hq*D] bf16, lse [B, Hq, S] fp32}.  window <= 0: plain causal.
-std::vector<torch::Tensor> attn_fwd(torch::Tensor qkv, int64_t B, int64_t S, int64_t Hq, int64_t Hk, int64_t D, double scale, int64_t window) {
+std::vector<torch::Tensor> attn_fwd(torch::Tensor qkv, int64_t B, int64_t S, int64_t Hq, int64_t Hk, int64_t D, double scale, int64_t window,
+                                    c10::optional<torch::Tensor> seg) {
     check_rows(qkv, B * S, (Hq + 2 * Hk) * D, "qkv");
     const c10::cuda::CUDAGuard guard(qkv.device());
     auto o = torch::empty({B * S, Hq * D}, qkv.options());
     auto lse = torch::empty({B, Hq, S}, qkv.options().dtype(torch::kFloat32));
     const auto* base = (const char*)qkv.data_ptr();      // bf16: 2 bytes per element
     const int rc = acco_attn_fwd(base, base + 2 * Hq * D, base + 2 * (Hq + Hk) * D, qkv.stride(0), o.data_ptr(), o.stride(0), lse.data_ptr<float>(), (int)B, (int)S,
-                                 (int)Hq, (int)Hk, (int)D, (float)scale, (int)window, stream());
+                                 (int)Hq, (int)Hk, (int)D, (float)scale, (int)window, seg_ptr(seg, B, S), stream());
     TORCH_CHECK(rc == 0, "attn_fwd launch failed, code ", rc, " (B=", B, " S=", S, " Hq=", Hq, " Hk=", Hk, " D=", D, ")");
     return {o, lse};
 }
 // -> {dq fp32 [B*S, Hq*D], dk bf16 [B*S, Hk*D], dv bf16 [B*S, Hk*D]}
 std::vector<torch::Tensor> attn_bwd(torch::Tensor qkv, torch::Tensor o, torch::Tensor d_o, torch::Tensor lse, int64_t B, int64_t S, int64_t Hq, int64_t Hk,
-                                    int64_t D, double scale, int64_t window) {
+                                    int64_t D, double scale, int64_t window, c10::optional<torch::Tensor> seg) {
     check_rows(qkv, B * S, (Hq + 2 * Hk) * D, "qkv");
     check_rows(o, B * S, Hq * D, "o");
     check_rows(d_o, B * S, Hq * D, "d_o");
@@ -518,7 +527,7 @@ std::vector<torch::Tensor> attn_bwd(torch::Tensor qkv, torch::Tensor o, torch::T
     const auto* base = (const char*)qkv.data_ptr();
     const int rc = acco_attn_bwd(base, base + 2 * Hq * D, base + 2 * (Hq + Hk) * D, qkv.stride(0), o.data_ptr(), o.stride(0), d_o.data_ptr(), d_o.stride(0),
                                  lse.data_ptr<float>(), delta.data_ptr<float>(), dq.data_ptr<float>(), dk.data_ptr(), dv.data_ptr(), (int)B, (int)S, (int)Hq,
-                                 (int)Hk, (int)D, (float)scale, (int)window, stream());
+                                 (int)Hk, (int)D, (float)scale, (int)window, seg_ptr(seg, B, S), stream());
     TORCH_CHECK(rc == 0, "attn_bwd launch failed, code ", rc);
     return {dq, dk, dv};
 }
@@ -561,8 +570,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("num_sms", &num_sms);
     m.def("prefer_shared_carveout", &prefer_shared_carveout);
     m.def("attn_supported", &attn_supported);
-    m.def("attn_fwd", &attn_fwd);
-    m.def("attn_bwd", &attn_bwd);
+    m.def("attn_fwd", &attn_fwd, py::arg("qkv"), py::arg("B"), py::arg("S"), py::arg("Hq"), py::arg("Hk"), py::arg("D"), py::arg("scale"),
+          py::arg("window"), py::arg("seg") = py::none());
+    m.def("attn_bwd", &attn_bwd, py::arg("qkv"), py::arg("o"), py::arg("d_o"), py::arg("lse"), py::arg("B"), py::arg("S"), py::arg("Hq"),
+          py::arg("Hk"), py::arg("D"), py::arg("scale"), py::arg("window"), py::arg("seg") = py::none());
     m.def("debug_occupy", &debug_occupy);
     m.def("pack_const_len", &pack_const_len_native);
 }

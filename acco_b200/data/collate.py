@@ -7,6 +7,8 @@
   ``tokenizer.pad_token_id = eos_token_id``, `main.py:46`) HF's
   ``DataCollatorForLanguageModeling(mlm=False)`` masks *every* EOS label ; that is
   reproduced with ``mask_all_pad_tokens=True`` (default) and can be switched off.
+* :class:`PackedCollator` - packed SFT rows (``pack_sft``): fixed ``[B, max_length]`` batches with per-sample ``position_ids``
+  (the models derive document masking from them) and labels that train exactly the (context, target) pairs of ``PadCollator``.
 """
 from __future__ import annotations
 
@@ -15,7 +17,7 @@ from typing import Any, Dict, Sequence
 import numpy as np
 import torch
 
-__all__ = ["stack_collate", "PadCollator"]
+__all__ = ["stack_collate", "PadCollator", "PackedCollator"]
 
 
 def stack_collate(batch: Sequence[Dict[str, Any]]) -> Dict[str, torch.Tensor]:
@@ -49,3 +51,40 @@ class PadCollator:
         else:
             labels[mask == 0] = self.label_pad
         return {"input_ids": ids, "attention_mask": mask, "labels": labels}
+
+
+class PackedCollator:
+    """Rows of several samples (columns ``input_ids`` and ``doc_lens``) -> ``input_ids``, ``labels``, ``position_ids``, each
+    ``[B, max_length]`` int64.  For a sample at ``[a, a+n)``: ``position_ids[a+i] = i``; ``labels[a] = -100`` (the previous
+    sample's last token must not learn to predict this one's first); ``labels[a+i] = input_ids[a+i]`` for ``1 <= i < n``, except
+    pad ids when ``mask_all_pad_tokens`` (the ``PadCollator`` rule).  The tail ``[used, max_length)`` holds pad ids with labels -100
+    and positions restarting at 0: one more segment."""
+
+    def __init__(self, pad_token_id: int, max_length: int, mask_all_pad_tokens: bool = True, label_pad: int = -100):
+        self.pad, self.L, self.label_pad = int(pad_token_id), int(max_length), int(label_pad)
+        self.mask_all = mask_all_pad_tokens
+
+    def __call__(self, batch: Sequence[Dict[str, Any]]) -> Dict[str, torch.Tensor]:
+        B, L = len(batch), self.L
+        ids = np.full((B, L), self.pad, dtype=np.int64)
+        labels = np.full((B, L), self.label_pad, dtype=np.int64)
+        pos = np.zeros((B, L), dtype=np.int64)
+        for b, row in enumerate(batch):
+            toks = np.asarray(row["input_ids"], dtype=np.int64).reshape(-1)
+            lens = [int(n) for n in row["doc_lens"]]
+            if any(n <= 0 for n in lens):
+                raise ValueError(f"packed row {b}: sample lengths must be positive, got {lens}")
+            if sum(lens) != toks.size or toks.size > L:
+                raise ValueError(f"packed row {b}: sample lengths sum to {sum(lens)} for a row of {toks.size} tokens (max_length {L})")
+            used = toks.size
+            ids[b, :used] = toks
+            labels[b, :used] = toks
+            a = 0
+            for n in lens:
+                labels[b, a] = self.label_pad
+                pos[b, a:a + n] = np.arange(n)
+                a += n
+            pos[b, used:] = np.arange(L - used)
+            if self.mask_all:
+                labels[b, :used][toks == self.pad] = self.label_pad
+        return {"input_ids": torch.from_numpy(ids), "labels": torch.from_numpy(labels), "position_ids": torch.from_numpy(pos)}

@@ -4,6 +4,8 @@
   `dl_dataset.py:8-34`): append EOS to every document, concatenate, cut into rows of
   ``max_length`` tokens, drop the tail; no attention mask is produced.
 * :func:`truncate_docs` - the *truncate-only* path for fine-tuning (`trainer_base.py:77-82`).
+* :func:`pack_sft` - sample packing for fine-tuning (``packing: True``): whole truncated samples placed into rows of at most
+  ``max_length`` tokens by first-fit-decreasing; ``PackedCollator`` turns a row into document-masked training inputs.
 
 Implemented with numpy on flat arrays (one concatenate, one reshape) rather than Python list
 appends, since it runs over ~9M documents for openwebtext."""
@@ -13,7 +15,8 @@ from typing import Any, Dict, List, Sequence
 
 import numpy as np
 
-__all__ = ["pack_const_len", "truncate_docs", "make_const_len_tokenize_fn", "make_truncate_tokenize_fn"]
+__all__ = ["pack_const_len", "truncate_docs", "pack_sft", "make_const_len_tokenize_fn", "make_truncate_tokenize_fn",
+           "make_packed_tokenize_fn"]
 
 
 def _native():
@@ -53,6 +56,28 @@ def truncate_docs(docs: Sequence[Sequence[int]], max_length: int) -> List[List[i
     return [list(d[:max_length]) for d in docs]
 
 
+def pack_sft(docs: Sequence[Sequence[int]], max_length: int) -> Dict[str, List[List[int]]]:
+    """Truncate every sample to ``max_length`` and place the samples into rows of at most ``max_length`` tokens by
+    first-fit-decreasing (longest first, ties in input order; each goes into the first row with room, else opens a new row).
+    A sample is never split.  Deterministic, no RNG.
+    -> ``{"input_ids": [row tokens], "doc_lens": [lengths of the row's samples, in row order]}``; empty samples are dropped."""
+    docs = [list(d[:max_length]) for d in docs]
+    order = sorted((i for i in range(len(docs)) if docs[i]), key=lambda i: -len(docs[i]))
+    rows: List[List[int]] = []
+    free: List[int] = []
+    for i in order:
+        n = len(docs[i])
+        r = next((j for j, f in enumerate(free) if f >= n), None)
+        if r is None:
+            rows.append([])
+            free.append(max_length)
+            r = len(rows) - 1
+        rows[r].append(i)
+        free[r] -= n
+    return {"input_ids": [[t for i in row for t in docs[i]] for row in rows],
+            "doc_lens": [[len(docs[i]) for i in row] for row in rows]}
+
+
 def make_const_len_tokenize_fn(tokenizer, text_column: str, max_length: int):
     """Batched ``datasets.map`` function: text -> packed ``input_ids`` rows."""
     def fn(batch: Dict[str, Any]) -> Dict[str, Any]:
@@ -69,4 +94,12 @@ def make_truncate_tokenize_fn(tokenizer, text_column: str, max_length: int):
         if "attention_mask" in out:
             res["attention_mask"] = out["attention_mask"]
         return res
+    return fn
+
+
+def make_packed_tokenize_fn(tokenizer, text_column: str, max_length: int):
+    """Batched ``datasets.map`` function: text -> packed ``input_ids`` / ``doc_lens`` rows (:func:`pack_sft` within each map batch)."""
+    def fn(batch: Dict[str, Any]) -> Dict[str, Any]:
+        ids = tokenizer(batch[text_column], truncation=True, max_length=max_length)["input_ids"]
+        return pack_sft(ids, max_length)
     return fn

@@ -185,9 +185,10 @@ class GPTForCausalLM(nn.Module):
         return n
 
     def forward(self, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor] = None,
-                labels: Optional[torch.Tensor] = None, **unused) -> CausalLMOutput:
+                labels: Optional[torch.Tensor] = None, position_ids: Optional[torch.Tensor] = None, **unused) -> CausalLMOutput:
         """HF-style call; ``attention_mask`` is accepted for API compatibility (right padding + causal attention: logits at
-        non-pad positions do not depend on it; pad positions carry ``labels == -100``)."""
+        non-pad positions do not depend on it; pad positions carry ``labels == -100``).  ``position_ids [B, S]`` marks packed rows
+        (``PackedCollator``): the learned positions are gathered per token and no token attends to another sample."""
         cfg = self.config
         B, S = input_ids.shape
         T = B * S
@@ -195,7 +196,12 @@ class GPTForCausalLM(nn.Module):
         eps = cfg.layer_norm_epsilon
         tr = self.transformer
         scale = (1.0 / math.sqrt(D)) if cfg.scale_attn else 1.0
-        h = (ops.embedding(input_ids.reshape(T), tr.wte).view(B, S, H) + tr.wpe[:S]).view(T, H)
+        seg = None
+        if position_ids is None:
+            h = (ops.embedding(input_ids.reshape(T), tr.wte).view(B, S, H) + tr.wpe[:S]).view(T, H)
+        else:
+            h = ops.embedding(input_ids.reshape(T), tr.wte) + ops.embedding(position_ids.reshape(T), tr.wpe)
+            seg = ops.segment_starts(position_ids)
         branch = None          # output of the previous residual branch, not yet added to h
         for blk in tr.h:
             a = blk.attn.attention
@@ -205,7 +211,7 @@ class GPTForCausalLM(nn.Module):
                 n, h = ops.add_layernorm(branch, h, blk.ln_1.weight, blk.ln_1.bias, eps)
             qkv = ops.linear(n, a.qkv_proj)                                                       # [T, 3H]
             att = ops.packed_causal_attention(qkv, B, S, Hh, Hh, D, scale=scale,
-                                              window=cfg.window_size if blk.kind == "local" else None)   # [T, H]
+                                              window=cfg.window_size if blk.kind == "local" else None, seg=seg)   # [T, H]
             o = ops.linear(att, a.out_proj.weight, a.out_proj.bias)
             n, h = ops.add_layernorm(o, h, blk.ln_2.weight, blk.ln_2.bias, eps)
             f = ops.linear(n, blk.mlp.c_fc.weight, blk.mlp.c_fc.bias)

@@ -187,15 +187,22 @@ class LlamaForCausalLM(nn.Module):
 
     # ------------------------------------------------------------------ forward
     def forward(self, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor] = None,
-                labels: Optional[torch.Tensor] = None, **unused) -> CausalLMOutput:
+                labels: Optional[torch.Tensor] = None, position_ids: Optional[torch.Tensor] = None, **unused) -> CausalLMOutput:
         """HF-style call.  ``attention_mask`` is accepted for API compatibility; with right
         padding and causal attention the logits at non-pad positions do not depend on it, and pad
-        positions carry ``labels == -100`` (the collator's job), so it is not applied."""
+        positions carry ``labels == -100`` (the collator's job), so it is not applied.
+        ``position_ids [B, S]`` marks packed rows (``PackedCollator``): positions restart at 0 for every sample, RoPE uses them
+        and no token attends to another sample."""
         cfg = self.config
         B, S = input_ids.shape
         T = B * S
         D, Hq, Hk = cfg.head_dim, cfg.num_attention_heads, cfg.num_key_value_heads
         cos, sin = self._rope(S, input_ids.device)
+        seg = None
+        if position_ids is not None:
+            pos = position_ids.reshape(T)
+            cos, sin = cos[pos], sin[pos]                                                   # per-token tables [T, D/2]
+            seg = ops.segment_starts(position_ids)
         eps = cfg.rms_norm_eps
 
         h = ops.embedding(input_ids.reshape(T), self.model.embed_tokens)                   # [T, H]
@@ -206,7 +213,7 @@ class LlamaForCausalLM(nn.Module):
             else:
                 n, h = ops.add_rmsnorm(branch, h, layer.input_layernorm.weight, eps)
             qkv = ops.linear(n, layer.self_attn.qkv_proj, gathered=self._gw(layer.self_attn.qkv_proj))   # [T, (Hq+2Hk)D]
-            att = ops.rope_causal_attention(qkv, cos, sin, B, S, Hq, Hk, D)                # [T, Hq*D]
+            att = ops.rope_causal_attention(qkv, cos, sin, B, S, Hq, Hk, D, seg=seg)       # [T, Hq*D]
             o = ops.linear(att, layer.self_attn.o_proj, gathered=self._gw(layer.self_attn.o_proj))
             n, h = ops.add_rmsnorm(o, h, layer.post_attention_layernorm.weight, eps)
             gu = ops.linear(n, layer.mlp.gate_up_proj, gathered=self._gw(layer.mlp.gate_up_proj))

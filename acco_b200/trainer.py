@@ -34,7 +34,8 @@ import torch.distributed as dist
 import torch.nn as nn
 
 from .config import to_container
-from .data import BatchLoader, DeviceFeeder, PadCollator, make_const_len_tokenize_fn, make_truncate_tokenize_fn, stack_collate
+from .data import (BatchLoader, DeviceFeeder, PackedCollator, PadCollator, make_const_len_tokenize_fn, make_packed_tokenize_fn,
+                   make_truncate_tokenize_fn, pack_sft, stack_collate)
 from .launch import DistEnv, discover_env, init_distributed
 from .obs import OverlapMeter, ScalarWriter, TrainingPrinter, create_dict_result, log_training_scalars, nvtx_range, save_result
 from .optim import ShardedAdamW
@@ -62,6 +63,7 @@ TRAIN_DEFAULTS: Dict[str, Any] = dict(
     debug_poison=False,             # True (or ACCO_DEBUG_POISON=1): NaN-fill the parameter buffer a round is about to overwrite (race detector)
     preempt_save=False,             # True: SIGTERM / SIGUSR1 (Slurm pre-emption, `scancel --signal`) -> checkpoint at the next committed round, then stop
     fault_inject=None,              # "rank@count" - that rank kills itself (os._exit) once count_grad_tot >= count; fires once per cwd
+    packing=False,                  # SFT: pack whole samples into full rows (document-masked attention, per-sample positions)
 )
 
 
@@ -274,8 +276,23 @@ class DecoupledTrainer:
         self.writer = ScalarWriter(tb_dir, enabled=(self.rank == 0 and bool(self.args.tensorboard)))
 
     # ------------------------------------------------------------------ data
+    def _check_packing(self) -> None:
+        """``packing`` needs ragged SFT samples, a fixed row order and a model that masks attention by ``position_ids``."""
+        a = self.args
+        if not a.packing:
+            return
+        if a.const_len_batch:
+            raise ValueError("packing=True needs const_len_batch=False: const-len pre-training rows are already full")
+        if a.group_by_length:
+            raise ValueError("packing=True cannot be combined with group_by_length: packed rows all have max_length tokens")
+        from .models import GPTForCausalLM, LlamaForCausalLM
+        if not isinstance(self.model, (LlamaForCausalLM, GPTForCausalLM)):
+            raise ValueError(f"packing=True needs a native model that masks attention by position_ids; {type(self.model).__name__} "
+                             "would attend across the samples of a row")
+
     def prepare_data(self) -> None:
         """Per-rank sharding (`trainer_base.py:183-200`)."""
+        self._check_packing()
         if self.train_dataset is not None and isinstance(self.train_dataset, torch.utils.data.IterableDataset) \
                 and self.args.group_by_length:
             raise ValueError("the `--group_by_length` option is only available for `Dataset`, not `IterableDataset")
@@ -290,16 +307,35 @@ class DecoupledTrainer:
             self.train_dataset = self.train_dataset.map(self.preprocess_dataset_fn, batched=True)
             if self.eval_dataset is not None:
                 self.eval_dataset = self.eval_dataset.map(self.preprocess_dataset_fn, batched=True)
-        if self.train_dataset is None or "input_ids" in self.train_dataset.column_names:
+        if self.train_dataset is None:
+            return
+        if "input_ids" in self.train_dataset.column_names:
+            if a.packing and "doc_lens" not in self.train_dataset.column_names:
+                L = int(a.max_length)
+                self.train_dataset = self.train_dataset.map(lambda b: pack_sft(b["input_ids"], L), batched=True,
+                                                            remove_columns=self.train_dataset.column_names)
+                self._log_packing()
             return
         if self.tokenizer is None:
             raise ValueError("dataset has no 'input_ids' column and no tokenizer was given")
         mk = make_const_len_tokenize_fn if a.const_len_batch else make_truncate_tokenize_fn
         fn = mk(self.tokenizer, self.text_column_name, int(a.max_length))
+        train_fn = make_packed_tokenize_fn(self.tokenizer, self.text_column_name, int(a.max_length)) if a.packing else fn
         nproc = int(a.dataloader_num_workers) or None
-        self.train_dataset = self.train_dataset.map(fn, batched=True, remove_columns=self.train_dataset.column_names, num_proc=nproc)
-        if self.eval_dataset is not None:
+        self.train_dataset = self.train_dataset.map(train_fn, batched=True, remove_columns=self.train_dataset.column_names, num_proc=nproc)
+        if self.eval_dataset is not None:       # eval stays padded: its loss and perplexity compare with unpacked runs
             self.eval_dataset = self.eval_dataset.map(fn, batched=True, remove_columns=self.eval_dataset.column_names, num_proc=nproc)
+        if a.packing:
+            self._log_packing()
+
+    def _log_packing(self) -> None:
+        if self.rank != 0:
+            return
+        lens = self.train_dataset["doc_lens"]
+        rows, samples, tokens = len(lens), sum(len(r) for r in lens), sum(sum(r) for r in lens)
+        eff = tokens / max(rows * int(self.args.max_length), 1)
+        self.log.info(f">>> packing: {samples} samples in {rows} rows of {int(self.args.max_length)} tokens, "
+                      f"efficiency {eff:.3f} (real tokens / processed tokens)")
 
     def _collator(self):
         if self.args.const_len_batch:
@@ -319,7 +355,10 @@ class DecoupledTrainer:
             return None
         seed = (int(self.args.seed) if self.args.seed is not None else 0) * 1000 + self.rank
         grouped = bool(self.args.group_by_length) and not bool(self.args.const_len_batch)
-        return BatchLoader(self.train_dataset, self.batch_size, self._collator(), shuffle=True, drop_last=True, seed=seed,
+        collate = self._collator()
+        if self.args.packing:
+            collate = PackedCollator(pad_token_id=collate.pad, max_length=int(self.args.max_length))
+        return BatchLoader(self.train_dataset, self.batch_size, collate, shuffle=True, drop_last=True, seed=seed,
                            group_by_length=grouped)
 
     def get_eval_dataloader(self) -> Optional[BatchLoader]:
@@ -481,7 +520,8 @@ class DecoupledTrainer:
     def _use_graphs(self) -> bool:
         if getattr(self, "_graphs_disabled", None):
             return False
-        static_shapes = bool(self.args.const_len_batch) or (self.args.pad_to_multiple_of is None) or int(self.args.pad_to_multiple_of) >= 32
+        static_shapes = bool(self.args.const_len_batch) or bool(self.args.packing) or (self.args.pad_to_multiple_of is None) \
+            or int(self.args.pad_to_multiple_of) >= 32
         return bool(self.is_cuda and self.args.cuda_graphs and static_shapes and self.label_smoother is None
                     and os.environ.get("ACCO_NO_GRAPHS") != "1")
 

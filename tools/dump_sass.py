@@ -25,7 +25,10 @@ KERNELS = {
     "rs_adam_ag_multimem_bf16.sass": "_ZN4acco17rs_adam_ag_kernelI13__nv_bfloat16S1_Li2ELb0EEEvNS_11RoundParamsE",
     "rs_adam_ag_p2p_bf16.sass": "_ZN4acco17rs_adam_ag_kernelI13__nv_bfloat16S1_Li1ELb0EEEvNS_11RoundParamsE",
     "round_gate.sass": "_ZN4acco17round_gate_kernelENS_11RoundParamsE",
-    "attn_fwd_wgmma.sass": "_ZN9acco_attn15attn_fwd_kernelENS_9FwdParamsE",
+    "attn_fwd_wgmma.sass": "_ZN9acco_attn15attn_fwd_kernelILb0EEEvNS_9FwdParamsE",
+    "attn_fwd_wgmma_seg.sass": "_ZN9acco_attn15attn_fwd_kernelILb1EEEvNS_9FwdParamsE",      # document-masked (packed rows)
+    "attn_bwd_mma.sass": "_ZN9acco_attn15attn_bwd_kernelILb0EEEvNS_9BwdParamsE",
+    "attn_bwd_mma_seg.sass": "_ZN9acco_attn15attn_bwd_kernelILb1EEEvNS_9BwdParamsE",
 }
 MNEMONICS = ["HGMMA", "UTMALDG", "UTMALDG.2D.MULTICAST", "UTMASTG", "UTMACMDFLUSH", "SYNCS", "USETMAXREG", "REDG", "LDGMC", "HMMA", "MUFU.SQRT",
              "MUFU.EX2", "CCTL"]
