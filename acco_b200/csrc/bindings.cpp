@@ -81,6 +81,7 @@ struct RoundParams {   // must mirror acco::RoundParams in rs_adam_ag.cu
     int commit, add_stash, write_stash;
 };
 extern "C" int acco_rs_adam_ag(const RoundParams* P, int grad_bf16, int out_bf16, int mode, int grid, cudaStream_t st);
+extern "C" int acco_round_norm(const RoundParams* P, int grad_bf16, int mode, int grid, float max_norm, float* out, cudaStream_t st);
 
 int sm_count() {
     static int n = 0;
@@ -334,49 +335,86 @@ void adamw_shard(torch::Tensor grad_sum, torch::Tensor master, torch::Tensor exp
     TORCH_CHECK(acco_rs_adam_ag(&P, gb, ob, 0, default_grid(0, S), stream()) == 0, "adamw_shard launch failed");
 }
 
-// Multi-GPU fused round (also valid for world == 1 with mode 0, counts handled in-kernel).
-void rs_adam_ag(std::vector<int64_t> acc_ptrs, std::vector<int64_t> theta_ptrs, std::vector<int64_t> pad_ptrs, int64_t acc_mc, int64_t theta_mc,
-                torch::Tensor master, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, torch::Tensor stash,
-                torch::Tensor scratch /* int32[4] */, int64_t slice, int64_t rank, int64_t world, int64_t local_count,
-                double lr, double b1, double b2, double eps, double wd, int64_t step, int64_t commit, bool add_stash, bool write_stash,
-                bool grad_bf16, bool out_bf16, int64_t mode, int64_t grid, c10::optional<torch::Tensor> skip_ranges) {
-    check_f32(master, "master"); check_f32(exp_avg, "exp_avg"); check_f32(exp_avg_sq, "exp_avg_sq"); check_f32(stash, "stash");
-    const c10::cuda::CUDAGuard guard(master.device());
+// Transport, counts and barrier state of one round (shared by rs_adam_ag and round_norm).
+RoundParams round_params(const std::vector<int64_t>& acc_ptrs, const std::vector<int64_t>& theta_ptrs, const std::vector<int64_t>& pad_ptrs,
+                         int64_t acc_mc, int64_t theta_mc, const torch::Tensor& stash, const torch::Tensor& scratch, int64_t slice, int64_t rank,
+                         int64_t world, int64_t local_count, int64_t mode) {
+    check_f32(stash, "stash");
     TORCH_CHECK(world >= 1 && world <= kMaxWorld, "world size out of range");
-    TORCH_CHECK((int64_t)acc_ptrs.size() >= (mode == 0 ? 1 : world) && (int64_t)theta_ptrs.size() >= (mode == 0 ? 1 : world), "peer pointer tables too short");
+    TORCH_CHECK(mode >= 0 && mode <= 2, "mode must be 0 (local), 1 (p2p) or 2 (multimem)");
+    TORCH_CHECK((int64_t)acc_ptrs.size() >= (mode == 0 ? 1 : world), "peer pointer table too short");
     TORCH_CHECK(mode == 0 || (int64_t)pad_ptrs.size() >= world, "signal pad table too short");
-    TORCH_CHECK(slice % 8 == 0 && master.numel() == slice, "slice must be a multiple of 8 and match the shard state");
-    TORCH_CHECK(mode != 2 || (acc_mc != 0 && theta_mc != 0), "multicast mode needs multicast pointers");
+    TORCH_CHECK(slice % 8 == 0 && stash.numel() == slice, "slice must be a multiple of 8 and match the shard state");
+    TORCH_CHECK(mode != 2 || acc_mc != 0, "multicast mode needs multicast pointers");
     TORCH_CHECK(scratch.scalar_type() == torch::kInt32 && scratch.numel() >= 4, "scratch must be int32[4]");
     RoundParams P{};
     for (size_t i = 0; i < acc_ptrs.size() && i < (size_t)kMaxWorld; ++i) P.acc_peer[i] = (const void*)acc_ptrs[i];
     for (size_t i = 0; i < theta_ptrs.size() && i < (size_t)kMaxWorld; ++i) P.theta_peer[i] = (void*)theta_ptrs[i];
     for (size_t i = 0; i < pad_ptrs.size() && i < (size_t)kMaxWorld; ++i) P.pad_peer[i] = (uint32_t*)pad_ptrs[i];
     P.acc_mc = (const void*)acc_mc; P.theta_mc = (void*)theta_mc;
-    P.master = master.data_ptr<float>(); P.exp_avg = exp_avg.data_ptr<float>(); P.exp_avg_sq = exp_avg_sq.data_ptr<float>(); P.stash = stash.data_ptr<float>();
+    P.stash = stash.data_ptr<float>();
     int* sc = scratch.data_ptr<int>();
     P.stash_count = sc; P.total_out = sc + 1; P.epoch = (uint32_t*)(sc + 2); P.done_ctas = (uint32_t*)(sc + 3);
     P.inv_count_in = nullptr;
+    P.slice = slice; P.rank = (int)rank; P.world = (int)world; P.local_count = (int)local_count;
+    static int watchdog = -1;
+    if (watchdog < 0) { const char* e = std::getenv("ACCO_ROUND_WATCHDOG_S"); watchdog = e ? std::atoi(e) : 1800; }
+    P.watchdog_s = watchdog;
+    static int gated = -1;
+    // default ON: the start barrier runs as a one-warp kernel, so a rank that is ahead of its peers waits with 32 threads instead
+    // of a resident grid and its next micro-batches keep the SMs (ACCO_ROUND_GATE=0: barrier inside the round kernel)
+    if (gated < 0) { const char* e = std::getenv("ACCO_ROUND_GATE"); gated = (e && e[0] == '0') ? 0 : 1; }
+    P.gated = mode != 0 ? gated : 0;
+    return P;
+}
+
+// Multi-GPU fused round (also valid for world == 1 with mode 0, counts handled in-kernel).
+// inv_count: None, or the fp32 scratch of a round_norm launched just before on this stream for the same round.  The update then
+// scales the gradient sum by its inv_eff (1/count * clip coefficient), and the start barrier, which round_norm ran, is not repeated.
+void rs_adam_ag(std::vector<int64_t> acc_ptrs, std::vector<int64_t> theta_ptrs, std::vector<int64_t> pad_ptrs, int64_t acc_mc, int64_t theta_mc,
+                torch::Tensor master, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, torch::Tensor stash,
+                torch::Tensor scratch /* int32[4] */, int64_t slice, int64_t rank, int64_t world, int64_t local_count,
+                double lr, double b1, double b2, double eps, double wd, int64_t step, int64_t commit, bool add_stash, bool write_stash,
+                bool grad_bf16, bool out_bf16, int64_t mode, int64_t grid, c10::optional<torch::Tensor> skip_ranges,
+                c10::optional<torch::Tensor> inv_count) {
+    check_f32(master, "master"); check_f32(exp_avg, "exp_avg"); check_f32(exp_avg_sq, "exp_avg_sq");
+    const c10::cuda::CUDAGuard guard(master.device());
+    TORCH_CHECK(master.numel() == slice, "slice must match the shard state");
+    TORCH_CHECK((int64_t)theta_ptrs.size() >= (mode == 0 ? 1 : world), "peer pointer tables too short");
+    TORCH_CHECK(mode != 2 || theta_mc != 0, "multicast mode needs multicast pointers");
+    RoundParams P = round_params(acc_ptrs, theta_ptrs, pad_ptrs, acc_mc, theta_mc, stash, scratch, slice, rank, world, local_count, mode);
+    P.master = master.data_ptr<float>(); P.exp_avg = exp_avg.data_ptr<float>(); P.exp_avg_sq = exp_avg_sq.data_ptr<float>();
     if (skip_ranges.has_value() && skip_ranges->defined() && skip_ranges->numel() > 0) {
         TORCH_CHECK(skip_ranges->is_cuda() && skip_ranges->scalar_type() == torch::kInt64 && skip_ranges->is_contiguous() && skip_ranges->numel() % 2 == 0,
                     "skip_ranges must be a contiguous CUDA int64 [n, 2] tensor");
         P.skip = (const long long*)skip_ranges->data_ptr<int64_t>();
         P.n_skip = (int)(skip_ranges->numel() / 2);
     }
-    P.slice = slice; P.rank = (int)rank; P.world = (int)world; P.local_count = (int)local_count;
-    {
-        static int watchdog = -1;
-        if (watchdog < 0) { const char* e = std::getenv("ACCO_ROUND_WATCHDOG_S"); watchdog = e ? std::atoi(e) : 1800; }
-        P.watchdog_s = watchdog;
-        static int gated = -1;
-        // default ON: the start barrier runs as a one-warp kernel, so a rank that is ahead of its peers waits with 32 threads instead
-        // of a resident grid and its next micro-batches keep the SMs (ACCO_ROUND_GATE=0: barrier inside the round kernel)
-        if (gated < 0) { const char* e = std::getenv("ACCO_ROUND_GATE"); gated = (e && e[0] == '0') ? 0 : 1; }
-        P.gated = mode != 0 ? gated : 0;
+    if (inv_count.has_value() && inv_count->defined()) {
+        check_f32(*inv_count, "inv_count");
+        TORCH_CHECK(inv_count->numel() >= 2, "inv_count must be the scratch of round_norm (inv_eff at index 1)");
+        P.inv_count_in = inv_count->data_ptr<float>() + 1;
+        if (mode != 0) P.gated = 2;
     }
     fill_hyper(P, lr, b1, b2, eps, wd, step, commit, add_stash, write_stash);
     const int g = grid > 0 ? (int)grid : default_grid((int)mode, slice);
     TORCH_CHECK(acco_rs_adam_ag(&P, grad_bf16, out_bf16, (int)mode, g, stream()) == 0, "rs_adam_ag launch failed");
+}
+
+// Norm pass of a clipped round: reads the round's reduced gradient (+ stash) like rs_adam_ag, runs the start barrier (round gate or
+// in-kernel, as rs_adam_ag would) and writes out = {norm, inv_eff, sum of squares, per-CTA partials...} (fp32, >= 3 + grid).  Pass
+// `out` to the round's rs_adam_ag as `inv_count`.
+void round_norm(std::vector<int64_t> acc_ptrs, std::vector<int64_t> pad_ptrs, int64_t acc_mc, torch::Tensor stash, torch::Tensor scratch,
+                torch::Tensor out, int64_t slice, int64_t rank, int64_t world, int64_t local_count, bool add_stash, bool grad_bf16, int64_t mode,
+                int64_t grid, double max_norm) {
+    check_f32(out, "out");
+    const c10::cuda::CUDAGuard guard(stash.device());
+    TORCH_CHECK(max_norm > 0, "max_norm must be positive");
+    RoundParams P = round_params(acc_ptrs, std::vector<int64_t>(), pad_ptrs, acc_mc, 0, stash, scratch, slice, rank, world, local_count, mode);
+    P.add_stash = add_stash ? 1 : 0;
+    const int g = grid > 0 ? (int)grid : default_grid((int)mode, slice);
+    TORCH_CHECK(out.numel() >= 3 + g, "out must hold 3 + grid floats (", 3 + g, ")");
+    TORCH_CHECK(acco_round_norm(&P, grad_bf16, (int)mode, g, (float)max_norm, out.data_ptr<float>(), stream()) == 0, "round_norm launch failed");
 }
 
 // ---------------------------------------------------------------- wgmma GEMM (+ fused weight all-gather)
@@ -560,7 +598,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("ce_fwd", &ce_fwd);
     m.def("ce_bwd_inplace", &ce_bwd_inplace);
     m.def("adamw_shard", &adamw_shard);
-    m.def("rs_adam_ag", &rs_adam_ag);
+    m.def("rs_adam_ag", &rs_adam_ag, py::arg("acc_ptrs"), py::arg("theta_ptrs"), py::arg("pad_ptrs"), py::arg("acc_mc"), py::arg("theta_mc"),
+          py::arg("master"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("stash"), py::arg("scratch"), py::arg("slice"), py::arg("rank"),
+          py::arg("world"), py::arg("local_count"), py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"), py::arg("wd"), py::arg("step"),
+          py::arg("commit"), py::arg("add_stash"), py::arg("write_stash"), py::arg("grad_bf16"), py::arg("out_bf16"), py::arg("mode"),
+          py::arg("grid"), py::arg("skip_ranges"), py::arg("inv_count") = py::none());
+    m.def("round_norm", &round_norm, py::arg("acc_ptrs"), py::arg("pad_ptrs"), py::arg("acc_mc"), py::arg("stash"), py::arg("scratch"),
+          py::arg("out"), py::arg("slice"), py::arg("rank"), py::arg("world"), py::arg("local_count"), py::arg("add_stash"), py::arg("grad_bf16"),
+          py::arg("mode"), py::arg("grid"), py::arg("max_norm"));
     m.def("gemm_tn", &gemm_tn);
     m.def("gemm", &gemm);
     m.def("gemm_choose", &gemm_choose);

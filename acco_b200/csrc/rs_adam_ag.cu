@@ -18,6 +18,9 @@
 //     registers; W 16-byte stores.
 //   * W == 1         : the same kernel on local pointers (also used after an NCCL reduce-scatter by
 //     the library-baseline backend).
+// Optional global gradient-norm clipping (train key `max_grad_norm`): round_norm_kernel streams the same slice first, exchanges
+// the per-rank sums of squares through the signal pad and hands rs_adam_ag_kernel 1/count * clip_coef through `inv_count_in`,
+// so the AdamW pass itself is unchanged.
 // Cross-GPU ordering: a start barrier (every rank's accumulator is final; also carries the counts)
 // and an end barrier (every rank's pushes have landed) on flag words in a symmetric signal pad,
 // written with st.release.sys and polled with ld.acquire.sys; the epoch lives in device memory so
@@ -56,13 +59,15 @@ struct RoundParams {
     int watchdog_s;                    // trap if a peer has not reached a barrier after this many seconds (0 = wait forever)
     int gated;                         // 1: the start barrier already ran in round_gate_kernel (tiny, so waiting for a slow peer
                                        //    does not pin registers / SM slots that the overlapping compute needs)
+                                       // 2: it already ran in round_norm_kernel (or in a gate launched before it): launch no gate
     long long slice;                   // elements per rank (multiple of 8)
     int rank, world, local_count;
     float lr, beta1, beta2, eps, weight_decay, bc1, bc2_rsqrt;   // bc1 = 1-b1^t ; bc2_rsqrt = 1/sqrt(1-b2^t)
     int commit, add_stash, write_stash;
 };
 
-// signal pad layout (uint32 words): [0,W) start flags, [W,2W) end flags, [2W,3W) counts
+// signal pad layout (uint32 words): [0,W) start flags, [W,2W) end flags, [2W,3W) counts,
+// [3W,4W) sums of squares of the round's gradient slices (float bits), [4W,5W) their flags (round_norm_kernel)
 ACCO_DEVINL void st_release_sys(uint32_t* p, uint32_t v) {
     asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
@@ -229,18 +234,42 @@ ACCO_DEVINL void store_param8(const RoundParams& P, long long e, const float (&p
     }
 }
 
+// rs_adam_ag_kernel keeps its own copy of the next two functions: calling them there changes its register assignment, and its SASS is
+// kept as it was measured.
+// Start barrier + count exchange (unless `gated`: it already ran): every CTA that calls this waits (threads < W poll the local pad) until every peer has
+// published "my accumulator is final for round `epoch`" and its micro-batch count; `publish` (one CTA) also publishes mine.
+ACCO_DEVINL void start_barrier(const RoundParams& P, uint32_t epoch, int gated, bool publish) {
+    const int W = P.world;
+    if (!gated && publish && threadIdx.x < W) {
+        uint32_t* pad = P.pad_peer[threadIdx.x];                       // peer's pad
+        st_relaxed_sys(pad + 2 * W + P.rank, (uint32_t)P.local_count);  // my count, then my flag (release orders both)
+        st_release_sys(pad + P.rank, epoch);
+    }
+    if (!gated && threadIdx.x < W) {
+        const uint32_t* mine = P.pad_peer[P.rank];
+        wait_flag(mine + threadIdx.x, epoch, P.watchdog_s);
+    }
+}
+
+// Global micro-batch count of the update this round applies (the start barrier must have completed for MODE != 0).
+template <int MODE>
+ACCO_DEVINL int round_total(const RoundParams& P) {
+    int total = 0;
+    if (MODE != 0) {
+        const uint32_t* mine = P.pad_peer[P.rank];
+        for (int q = 0; q < P.world; ++q) total += (int)ld_acquire_sys(mine + 2 * P.world + q);
+    } else {
+        total = P.local_count;
+    }
+    return total + (P.add_stash ? *P.stash_count : 0);
+}
+
 // Start barrier of a round as its own one-warp kernel: publish my micro-batch count + "my accumulator is final" to every
 // peer, then wait until every peer has done the same.  A rank that is ahead of its peers (heterogeneous speeds are the whole
 // point of ACCO) waits HERE, holding 32 threads instead of a grid of 512-thread CTAs, so its next micro-batches keep the SMs.
 __global__ void __launch_bounds__(32) round_gate_kernel(const __grid_constant__ RoundParams P) {
-    const int W = P.world;
     const uint32_t epoch = *((volatile uint32_t*)P.epoch) + 1;
-    if (threadIdx.x < W) {
-        uint32_t* pad = P.pad_peer[threadIdx.x];
-        st_relaxed_sys(pad + 2 * W + P.rank, (uint32_t)P.local_count);
-        st_release_sys(pad + P.rank, epoch);
-        wait_flag(P.pad_peer[P.rank] + threadIdx.x, epoch, P.watchdog_s);
-    }
+    start_barrier(P, epoch, 0, true);
 }
 
 // NVLS rounds run as 256-thread x 64-register CTAs (16 K registers), one per SM.  The wgmma GEMM CTA (384 threads x 168 registers)
@@ -399,6 +428,105 @@ __global__ void __launch_bounds__(round_threads<MODE, kSmall>(), (MODE == 2 || k
     }
 }
 
+// Global L2 norm of the gradient the round is about to apply, and the factor rs_adam_ag_kernel then scales it with:
+//   g = (sum over ranks of the accumulators [+ stash]) / count,  norm = ||g||_2 over the whole flat vector,
+//   out[0] = norm,  out[1] = 1/count * min(1, max_norm / (norm + 1e-6)),  out[2] = sum of squares of the unscaled sum,
+//   out[3 + b] = CTA b's partial (scratch).
+// The gradient is read exactly as rs_adam_ag_kernel reads it (load_grad8).  Each CTA writes one partial; the last CTA sums them in CTA
+// order and, for W > 1, exchanges the rank's partial through the signal pad and sums the W partials in rank order, so every rank gets
+// the same bits for a fixed grid.  Only the last CTA waits, as in the end barrier: no grid-wide co-residency is needed.
+// Slot reuse: a peer overwrites my [3W + q] / [4W + q] words for round e + 1 only after it passed round e's end barrier, which needs my
+// end flag of round e, which rs_adam_ag_kernel sets after this kernel has read them.
+constexpr int kNormThreads = 256;
+
+template <typename G, int MODE>
+__global__ void __launch_bounds__(kNormThreads, MODE == 1 ? 2 : 4) round_norm_kernel(const __grid_constant__ RoundParams P, float* out, float max_norm) {
+    const int W = P.world;
+    uint32_t epoch = 0;
+    if (MODE != 0) {
+        epoch = *((volatile uint32_t*)P.epoch) + 1;
+        start_barrier(P, epoch, P.gated, blockIdx.x == 0);
+        __syncthreads();
+    }
+    const long long base = (long long)P.rank * P.slice;
+    const long long nvec = P.slice >> 3;
+    constexpr int kU = MODE == 1 ? 1 : 4;          // independent 16-byte loads in flight per thread (p2p already has W of them)
+    const long long vstride = (long long)gridDim.x * blockDim.x;
+    float ss = 0.f;
+    for (long long v0 = (long long)blockIdx.x * blockDim.x + threadIdx.x; v0 < nvec; v0 += vstride * kU) {
+        float g[kU][8];
+#pragma unroll
+        for (int u = 0; u < kU; ++u) {
+            const long long v = v0 + u * vstride;
+            if (v < nvec) load_grad8<G, MODE>(P, base + (v << 3), g[u]);
+        }
+#pragma unroll
+        for (int u = 0; u < kU; ++u) {
+            const long long v = v0 + u * vstride;
+            if (v >= nvec) continue;
+            float (&gg)[8] = g[u];
+            if (P.add_stash) {
+                const float4* s4 = reinterpret_cast<const float4*>(P.stash + (v << 3));
+                const float4 sa = s4[0], sb = s4[1];
+                gg[0] += sa.x; gg[1] += sa.y; gg[2] += sa.z; gg[3] += sa.w;
+                gg[4] += sb.x; gg[5] += sb.y; gg[6] += sb.z; gg[7] += sb.w;
+            }
+#pragma unroll
+            for (int j = 0; j < 8; ++j) ss = fmaf(gg[j], gg[j], ss);
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+    __shared__ float s_warp[kNormThreads / 32];
+    __shared__ float s_sum;
+    __shared__ bool s_last;
+    if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = ss;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float cta = 0.f;
+#pragma unroll
+        for (int w = 0; w < kNormThreads / 32; ++w) cta += s_warp[w];
+        out[3 + blockIdx.x] = cta;
+        __threadfence();
+        const uint32_t prev = atomicAdd(P.done_ctas, 1u);
+        s_last = (prev == gridDim.x - 1);
+    }
+    __syncthreads();
+    if (!s_last) return;
+    if (threadIdx.x == 0) {
+        __threadfence();
+        *P.done_ctas = 0;
+        float local = 0.f;
+        for (unsigned b = 0; b < gridDim.x; ++b) local += __ldcg(out + 3 + b);
+        s_sum = local;
+    }
+    __syncthreads();
+    if (MODE != 0) {
+        if (threadIdx.x < W) {
+            uint32_t* pad = P.pad_peer[threadIdx.x];
+            st_relaxed_sys(pad + 3 * W + P.rank, __float_as_uint(s_sum));   // my partial, then its flag (release orders both)
+            st_release_sys(pad + 4 * W + P.rank, epoch);
+            wait_flag(P.pad_peer[P.rank] + 4 * W + threadIdx.x, epoch, P.watchdog_s);
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        float sumsq = s_sum;
+        if (MODE != 0) {
+            const uint32_t* mine = P.pad_peer[P.rank];
+            sumsq = 0.f;
+            for (int q = 0; q < W; ++q) sumsq += __uint_as_float(ld_acquire_sys(mine + 3 * W + q));
+        }
+        const float inv_count = 1.f / (float)max(round_total<MODE>(P), 1);     // the expression rs_adam_ag_kernel uses
+        const float norm = sqrtf(sumsq) * inv_count;
+        const float c = max_norm / (norm + 1e-6f);
+        const float coef = c > 1.f ? 1.f : c;       // NaN stays NaN, as torch.clamp(max=1) in clip_grad_norm_
+        out[0] = norm;
+        out[1] = inv_count * coef;
+        out[2] = sumsq;
+    }
+}
+
 // The round shares SMs with the wgmma GEMMs, which run with the maximum shared-memory carve-out.  An SM is only
 // re-partitioned between L1 and shared memory when it is idle, so a kernel that prefers another carve-out can never be co-resident with
 // them - it waits for the SM to drain (tools/coresidency_check.py checks this).
@@ -440,6 +568,22 @@ static void launch_mode(const RoundParams& P, int mode, int grid, cudaStream_t s
     else rs_adam_ag_kernel<G, O, 2><<<grid, round_threads<2>(), 0, st>>>(P);
 }
 
+static void launch_gate(const RoundParams& P, cudaStream_t st) {
+    static bool gate_attr = false;
+    if (!gate_attr) { cudaFuncSetAttribute(round_gate_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared); gate_attr = true; }
+    round_gate_kernel<<<1, 32, 0, st>>>(P);
+}
+
+template <typename G, int MODE>
+static void launch_norm(const RoundParams& P, int grid, float max_norm, float* out, cudaStream_t st) {
+    static bool attr = false;
+    if (MODE != 0 && !attr) {
+        cudaFuncSetAttribute(round_norm_kernel<G, MODE>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        attr = true;
+    }
+    round_norm_kernel<G, MODE><<<grid, kNormThreads, 0, st>>>(P, out, max_norm);
+}
+
 }  // namespace acco
 
 // grad_bf16 / out_bf16: element types of accumulator and shadow parameter buffer.
@@ -447,15 +591,29 @@ static void launch_mode(const RoundParams& P, int mode, int grid, cudaStream_t s
 extern "C" int acco_rs_adam_ag(const acco::RoundParams* P, int grad_bf16, int out_bf16, int mode, int grid, cudaStream_t st) {
     using namespace acco;
     if (P->slice % 8 != 0 || P->world > kMaxWorld) return -1;
-    if (mode != 0 && P->gated) {
-        static bool gate_attr = false;
-        if (!gate_attr) { cudaFuncSetAttribute(round_gate_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared); gate_attr = true; }
-        round_gate_kernel<<<1, 32, 0, st>>>(*P);
-    }
+    if (mode != 0 && P->gated == 1) launch_gate(*P, st);
     if (grad_bf16 && out_bf16) launch_mode<__nv_bfloat16, __nv_bfloat16>(*P, mode, grid, st);
     else if (!grad_bf16 && !out_bf16) launch_mode<float, float>(*P, mode, grid, st);
     else if (grad_bf16 && !out_bf16) launch_mode<__nv_bfloat16, float>(*P, mode, grid, st);
     else launch_mode<float, __nv_bfloat16>(*P, mode, grid, st);
+    return (int)cudaGetLastError();
+}
+
+// Norm pass of a clipped round (see round_norm_kernel); `out` holds 3 + grid floats.  With P->gated == 1 the round's start barrier
+// runs in round_gate_kernel first, with 0 inside the norm kernel; either way rs_adam_ag must then be launched with gated = 2.
+extern "C" int acco_round_norm(const acco::RoundParams* P, int grad_bf16, int mode, int grid, float max_norm, float* out, cudaStream_t st) {
+    using namespace acco;
+    if (P->slice % 8 != 0 || P->world > kMaxWorld || mode < 0 || mode > 2) return -1;
+    if (mode != 0 && P->gated == 1) launch_gate(*P, st);
+    if (grad_bf16) {
+        if (mode == 0) launch_norm<__nv_bfloat16, 0>(*P, grid, max_norm, out, st);
+        else if (mode == 1) launch_norm<__nv_bfloat16, 1>(*P, grid, max_norm, out, st);
+        else launch_norm<__nv_bfloat16, 2>(*P, grid, max_norm, out, st);
+    } else {
+        if (mode == 0) launch_norm<float, 0>(*P, grid, max_norm, out, st);
+        else if (mode == 1) launch_norm<float, 1>(*P, grid, max_norm, out, st);
+        else launch_norm<float, 2>(*P, grid, max_norm, out, st);
+    }
     return (int)cudaGetLastError();
 }
 

@@ -109,7 +109,7 @@ from .swiglu import swiglu, swiglu_ref  # noqa: E402
 from .cross_entropy import softmax_cross_entropy, softmax_cross_entropy_ref  # noqa: E402
 from .linear import linear, LinearFn  # noqa: E402
 from .attention import causal_attention, causal_attention_ref, rope_causal_attention, packed_causal_attention, segment_starts  # noqa: E402
-from .adam import fused_adamw_shard  # noqa: E402
+from .adam import fused_adamw_shard, grad_sumsq  # noqa: E402
 
 __all__ = [
     "load_ext", "have_ext", "use_kernels", "ext_path",
@@ -121,5 +121,5 @@ __all__ = [
     "softmax_cross_entropy", "softmax_cross_entropy_ref",
     "linear", "LinearFn",
     "causal_attention", "causal_attention_ref", "rope_causal_attention", "packed_causal_attention", "segment_starts",
-    "fused_adamw_shard",
+    "fused_adamw_shard", "grad_sumsq",
 ]

@@ -11,6 +11,7 @@ from . import count_launch, load_ext, use_kernels
 
 
 _SCRATCH = {}
+_NORM = {}
 
 
 def _scratch(device) -> torch.Tensor:
@@ -32,3 +33,24 @@ def fused_adamw_shard(grad_sum, master, exp_avg, exp_avg_sq, stash, out, hp) -> 
                   float(hp.lr), float(hp.beta1), float(hp.beta2), float(hp.eps), float(hp.weight_decay),
                   int(hp.step), int(hp.commit), bool(hp.add_stash), bool(hp.write_stash))
     count_launch("adamw_shard")
+
+
+def grad_sumsq(grad_sum, stash, add_stash: bool) -> torch.Tensor:
+    """fp32 ``[1]``: sum of squares of ``grad_sum (+ stash)`` over the shard, on the device (the local part of a clipped round's
+    norm; the NCCL path all-reduces it).  CUDA: ``round_norm_kernel`` in local mode, dispatched like :func:`fused_adamw_shard`."""
+    S = stash.numel()
+    if not use_kernels(grad_sum, stash, bf16_only=False) or S % 8 != 0:
+        g = grad_sum[:S].to(torch.float32)
+        if add_stash:
+            g = g + stash
+        return (g * g).sum().reshape(1)
+    C = load_ext(required=True)
+    key = str(stash.device)
+    if key not in _NORM:
+        _NORM[key] = (torch.zeros(4, dtype=torch.int32, device=stash.device),
+                      torch.zeros(3 + 4 * int(C.num_sms()), dtype=torch.float32, device=stash.device))
+    scratch, out = _NORM[key]
+    C.round_norm([grad_sum.data_ptr()], [], 0, stash, scratch, out, S, 0, 1, 1, bool(add_stash),
+                 grad_sum.dtype == torch.bfloat16, 0, 0, float("inf"))
+    count_launch("round_norm")
+    return out[2:3].clone()

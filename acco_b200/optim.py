@@ -17,17 +17,29 @@ stash``) and an update is *one* pass described by :class:`AdamHyper`:
 which is exactly ``torch.optim.AdamW`` (decoupled weight decay, bias-corrected) - verified in
 ``tests/test_optim.py``.  :func:`adamw_shard_update_` below is the plain-PyTorch implementation
 (CPU / gloo path and numerics oracle for the sm_90a kernel in ``csrc/rs_adam_ag.cu``).
+
+Gradient clipping (train key ``max_grad_norm``) is a scalar on ``g``, so it never touches the update
+math: every round, whatever its kind, with ``s`` the round's reduced sum (+ stash when ``add_stash``),
+
+    norm    = ||s * inv_count||_2 over the whole flat parameter vector (all ranks' slices)
+    inv_eff = inv_count * min(1, max_grad_norm / (norm + 1e-6))      # torch.nn.utils.clip_grad_norm_
+
+and the update runs with ``inv_count = inv_eff`` (:func:`clip_scale`).  The stash keeps the
+*unclipped* sum, so a real ACCO round clips the norm of the whole two-half batch, and a tentative
+round clips its own half-batch gradient.  ``max_grad_norm = inf`` measures without clipping
+(the coefficient is exactly 1).
 """
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass
-from typing import Dict, Optional
+from typing import Dict, Optional, Tuple
 
 import torch
 
 from .parallel.schedule import COMMIT_ALL, COMMIT_PARAM, COMMIT_STATE
 
-__all__ = ["AdamHyper", "ShardedAdamW", "adamw_shard_update_"]
+__all__ = ["AdamHyper", "ShardedAdamW", "adamw_shard_update_", "clip_scale", "check_max_grad_norm"]
 
 
 @dataclass
@@ -73,6 +85,29 @@ def adamw_shard_update_(
     if hp.commit & COMMIT_STATE:
         exp_avg.copy_(m)
         exp_avg_sq.copy_(v)
+
+
+def check_max_grad_norm(value) -> Optional[float]:
+    """``max_grad_norm`` as the trainer uses it: ``None`` (off) or a positive float (``inf``: log the norm, never clip)."""
+    if value is None:
+        return None
+    if isinstance(value, bool) or not isinstance(value, (int, float)):
+        raise ValueError(f"max_grad_norm must be null or a positive number, got {value!r}")
+    v = float(value)
+    if math.isnan(v) or v <= 0:
+        raise ValueError(f"max_grad_norm must be null or a positive number, got {value!r}")
+    return v
+
+
+def clip_scale(sumsq, inv_count, max_norm: float) -> Tuple[torch.Tensor, torch.Tensor]:
+    """``(norm, inv_eff)`` of a round from the global sum of squares of its gradient *sum* (fp32, 1-element tensor or float).
+    ``norm = sqrt(sumsq) * inv_count``; ``inv_eff = inv_count * clamp(max_norm / (norm + 1e-6), max=1)``, the coefficient
+    of ``torch.nn.utils.clip_grad_norm_`` (a NaN norm propagates, as there).  Device ops only: the host is not synchronised."""
+    sumsq = torch.as_tensor(sumsq, dtype=torch.float32)
+    inv = torch.as_tensor(inv_count, dtype=torch.float32, device=sumsq.device)
+    norm = torch.sqrt(sumsq) * inv
+    coef = torch.clamp(max_norm / (norm + 1e-6), max=1.0)
+    return norm, inv * coef
 
 
 class ShardedAdamW:

@@ -25,7 +25,7 @@ from typing import Callable, Optional
 import torch
 import torch.distributed as dist
 
-from ..optim import ShardedAdamW, adamw_shard_update_
+from ..optim import ShardedAdamW, adamw_shard_update_, clip_scale
 from .arena import FlatArena
 from .schedule import RoundPlan
 
@@ -49,8 +49,12 @@ class CommBackend:
         """Required alignment (elements) of ``size_slice``; 1 reproduces the reference math."""
         return 1
 
-    def attach(self, arena: FlatArena, opt: ShardedAdamW) -> None:
+    def attach(self, arena: FlatArena, opt: ShardedAdamW, max_grad_norm: Optional[float] = None) -> None:
+        """``max_grad_norm``: ``None`` (no clipping) or a positive float (global-norm clipping of every round's gradient,
+        :func:`acco_b200.optim.clip_scale`); the pre-clip norm of a finished round is then :attr:`last_grad_norm`."""
         self.arena, self.opt = arena, opt
+        self.max_grad_norm = max_grad_norm
+        self.last_grad_norm: Optional[float] = None
 
     # collectives -----------------------------------------------------------------------
     def init_sync(self, flat: torch.Tensor, mode: str = "broadcast") -> None:
@@ -74,6 +78,7 @@ class CommBackend:
         raise NotImplementedError
 
     def finish_round(self, plan: RoundPlan) -> int:
+        """Global micro-gradient count of the finished round's update; also sets :attr:`last_grad_norm` when clipping."""
         raise NotImplementedError
 
     def barrier(self) -> None:
@@ -104,8 +109,8 @@ class TorchDistBackend(CommBackend):
         self._fused_adam = fused_adam
         self._launches = 0
 
-    def attach(self, arena: FlatArena, opt: ShardedAdamW) -> None:
-        super().attach(arena, opt)
+    def attach(self, arena: FlatArena, opt: ShardedAdamW, max_grad_norm: Optional[float] = None) -> None:
+        super().attach(arena, opt, max_grad_norm)
         S = arena.layout.size_slice
         dev = self.device
         self.count = torch.zeros(1, dtype=torch.int32, device=dev)
@@ -117,6 +122,10 @@ class TorchDistBackend(CommBackend):
             self.total_host = torch.zeros(1, dtype=torch.int32).pin_memory()
         else:
             self.total_host = torch.zeros(1, dtype=torch.int32)
+        if max_grad_norm is not None:
+            self.norm_host = torch.zeros(1, dtype=torch.float32)
+            if dev.type == "cuda":
+                self.norm_host = self.norm_host.pin_memory()
 
     @torch.no_grad()
     def launch_round(self, plan: RoundPlan, lr: float, local_count: int) -> None:
@@ -138,6 +147,13 @@ class TorchDistBackend(CommBackend):
         if plan.write_stash:
             self.stash_count.copy_(self.count)
         inv = 1.0 / self.total.clamp(min=1).to(torch.float32)
+        if self.max_grad_norm is not None:
+            from ..ops.adam import grad_sumsq
+            sumsq = grad_sumsq(gsum, opt.stash, plan.add_stash)
+            if self.world > 1:
+                dist.all_reduce(sumsq, op=dist.ReduceOp.SUM)
+            norm, inv = clip_scale(sumsq, inv, self.max_grad_norm)
+            self.norm_host.copy_(norm, non_blocking=True)
         hp = opt.hyper(lr, plan, inv)
         if self._fused_adam is not None:
             self._fused_adam(gsum, opt.master, opt.exp_avg, opt.exp_avg_sq, opt.stash, self.shard_out, hp)
@@ -153,6 +169,8 @@ class TorchDistBackend(CommBackend):
         self.total_host.copy_(self.total, non_blocking=True)
 
     def finish_round(self, plan: RoundPlan) -> int:
+        if self.max_grad_norm is not None:
+            self.last_grad_norm = float(self.norm_host.item())
         return int(self.total_host.item())
 
     def kernel_launches_per_round(self) -> int:

@@ -38,7 +38,7 @@ def merge_ranges(ranges):
             merged.append([a, b])
     return merged
 
-_CTRL_WORDS = 1024     # uint32 words in the private signal pad (3*W used)
+_CTRL_WORDS = 1024     # uint32 words in the private signal pad (3*W used, 5*W with max_grad_norm)
 
 
 class SymmBackend(CommBackend):
@@ -86,10 +86,15 @@ class SymmBackend(CommBackend):
     def slice_alignment(self) -> int:
         return 1024
 
-    def attach(self, arena: FlatArena, opt: ShardedAdamW) -> None:
-        super().attach(arena, opt)
+    def attach(self, arena: FlatArena, opt: ShardedAdamW, max_grad_norm: Optional[float] = None) -> None:
+        super().attach(arena, opt, max_grad_norm)
         self.scratch = torch.zeros(4, dtype=torch.int32, device=self.device)   # stash_count, total, epoch, done
         self.total_host = torch.zeros(1, dtype=torch.int32).pin_memory()
+        if max_grad_norm is not None:
+            # round_norm output: norm, inv_eff, sum of squares, one partial per CTA of its grid
+            grid = self.grid if self.grid > 0 else 4 * int(self.C.num_sms())
+            self.norm_out = torch.zeros(3 + grid, dtype=torch.float32, device=self.device)
+            self.norm_host = torch.zeros(1, dtype=torch.float32).pin_memory()
         self._grad_bf16 = arena.grad_dtype == torch.bfloat16
         self._out_bf16 = arena.dtype == torch.bfloat16
         if self.world > 1:
@@ -116,19 +121,31 @@ class SymmBackend(CommBackend):
             pads = self._pads
         else:
             acc_ptrs, acc_mc, th_ptrs, th_mc, pads = [acc.data_ptr()], 0, [theta.data_ptr()], 0, []
+        inv_eff = None
+        if self.max_grad_norm is not None:
+            # gate (W > 1, gated) + start barrier, then the global norm; the update below reads inv_eff = 1/count * clip coefficient
+            self.C.round_norm(acc_ptrs, pads, acc_mc, opt.stash, self.scratch, self.norm_out, arena.layout.size_slice, self.rank,
+                              self.world, int(local_count), bool(plan.add_stash), self._grad_bf16, self.mode, self.grid,
+                              self.max_grad_norm)
+            self._ops.count_launch("round_norm")
+            inv_eff = self.norm_out
         self.C.rs_adam_ag(acc_ptrs, th_ptrs, pads, acc_mc, th_mc, opt.master, opt.exp_avg, opt.exp_avg_sq, opt.stash,
                           self.scratch, arena.layout.size_slice, self.rank, self.world, int(local_count),
                           float(lr), opt.beta1, opt.beta2, opt.eps, opt.weight_decay, opt.step + 1, int(plan.commit),
                           bool(plan.add_stash), bool(plan.write_stash), self._grad_bf16, self._out_bf16, self.mode, self.grid,
-                          self._skip)
+                          self._skip, inv_eff)
         self._ops.count_launch("rs_adam_ag")
         if self.world > 1 and os.environ.get("ACCO_ROUND_GATE", "1") != "0":
             self._ops.count_launch("round_gate")
         opt.after_launch(plan)
         acc.zero_()
         self.total_host.copy_(self.scratch[1:2], non_blocking=True)
+        if inv_eff is not None:
+            self.norm_host.copy_(self.norm_out[0:1], non_blocking=True)
 
     def finish_round(self, plan: RoundPlan) -> int:
+        if self.max_grad_norm is not None:
+            self.last_grad_norm = float(self.norm_host.item())
         return int(self.total_host.item())
 
     # ------------------------------------------------------------------ fused all-gather + GEMM support (KERNEL B)
@@ -144,4 +161,4 @@ class SymmBackend(CommBackend):
         self._skip = torch.tensor(merged, dtype=torch.int64, device=self.device).contiguous() if merged else None
 
     def kernel_launches_per_round(self) -> int:
-        return 1
+        return 1 if self.max_grad_norm is None else 2

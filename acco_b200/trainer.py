@@ -38,7 +38,7 @@ from .data import (BatchLoader, DeviceFeeder, PackedCollator, PadCollator, make_
                    make_truncate_tokenize_fn, pack_sft, stack_collate)
 from .launch import DistEnv, discover_env, init_distributed
 from .obs import OverlapMeter, ScalarWriter, TrainingPrinter, create_dict_result, log_training_scalars, nvtx_range, save_result
-from .optim import ShardedAdamW
+from .optim import ShardedAdamW, check_max_grad_norm
 from .parallel.arena import FlatArena
 from .parallel.backend import CommBackend, make_backend
 from .parallel.graphs import MicroBatchGraphs
@@ -64,6 +64,7 @@ TRAIN_DEFAULTS: Dict[str, Any] = dict(
     preempt_save=False,             # True: SIGTERM / SIGUSR1 (Slurm pre-emption, `scancel --signal`) -> checkpoint at the next committed round, then stop
     fault_inject=None,              # "rank@count" - that rank kills itself (os._exit) once count_grad_tot >= count; fires once per cwd
     packing=False,                  # SFT: pack whole samples into full rows (document-masked attention, per-sample positions)
+    max_grad_norm=None,             # global gradient-norm clipping of every round (.inf: log the norm only); logged as grad_norm
 )
 
 
@@ -149,6 +150,8 @@ class DecoupledTrainer:
         self.method = str(self.args.method_name)
         if self.method not in ("acco", "dpu", "ddp"):
             raise ValueError("You must select one of the following method_name: 'acco', 'ddp', 'dpu'")
+        self.max_grad_norm = check_max_grad_norm(self.args.max_grad_norm)
+        self._grad_norm: Optional[float] = None     # pre-clip norm of the last committed round (max_grad_norm set)
 
         self.initialize_com(env)
         self._init_writer()
@@ -386,7 +389,7 @@ class DecoupledTrainer:
             self.arena.shard(self.arena.theta[0]), lr=float(a.learning_rate),
             betas=(float(a.adam_beta1), float(a.adam_beta2)), eps=float(a.adam_eps), weight_decay=float(a.weight_decay))
         self.params_opt = self.sharded_optimizer.master
-        self.backend.attach(self.arena, self.sharded_optimizer)
+        self.backend.attach(self.arena, self.sharded_optimizer, self.max_grad_norm)
         self._setup_fused_ag()
         self.lr_schedule = LRSchedule(float(a.learning_rate), str(a.scheduler_name), int(a.warmup), self.nb_grad_tot, str(a.lr_unit))
         n_warm = int(a.n_warmup_steps) if self.method in ("acco", "dpu") else 0
@@ -643,6 +646,8 @@ class DecoupledTrainer:
                     w1.record(self.grad_stream)
             fl.wait_host()          # already complete when reached through the poll; blocks in sync mode
         total = self.backend.finish_round(fl.plan)
+        if self.max_grad_norm is not None and fl.plan.kind != "tentative":
+            self._grad_norm = self.backend.last_grad_norm
         self.sched.complete(fl.plan, total)
         if getattr(self, "_ag_on", False):
             self._ag_stale[fl.plan.write_theta] = True   # fresh weights: remote row-blocks of the GEMM weights still on their owners
@@ -820,6 +825,8 @@ class DecoupledTrainer:
             lr = self.lr_schedule.lr_at(sched)
             for g in self.optimizer.param_groups:
                 g["lr"] = lr
+            if self.max_grad_norm is not None:
+                self._grad_norm = float(torch.nn.utils.clip_grad_norm_(self.ddp_model.parameters(), self.max_grad_norm))
             self.optimizer.step()
             self.optimizer.zero_grad(set_to_none=False)
             sched.round += 1
@@ -884,17 +891,19 @@ class DecoupledTrainer:
             if pr.due(sched.count_grad_tot) or eval_loss is not None:
                 loss = float(self.loss_host.item())
                 nb_step = sched.count_com // 2 if self.method == "acco" else sched.count_com
+                gn = {} if self._grad_norm is None else {"grad_norm": self._grad_norm}
                 log_training_scalars(self.writer, nb_step, sched.count_grad_tot, self.rank, loss, eval_loss, self.t_beg,
-                                     extra={"lr": getattr(self, "_last_lr", 0.0)})
+                                     extra={"lr": getattr(self, "_last_lr", 0.0), **gn})
                 self._fire("on_log", {"step": nb_step, "count_grad_tot": sched.count_grad_tot, "loss": loss,
-                                      "eval_loss": None if eval_loss is None else float(eval_loss), "lr": getattr(self, "_last_lr", 0.0)})
+                                      "eval_loss": None if eval_loss is None else float(eval_loss), "lr": getattr(self, "_last_lr", 0.0), **gn})
                 if pr.due(sched.count_grad_tot):
                     # same line as the reference (`utils/logs_utils.py:155-183`) + this rank's throughput since the previous line and the LR
                     now, seen = time.time(), self._tokens_seen
                     t0, n0 = st.get("rate_mark", (self.t_beg, 0))
                     st["rate_mark"] = (now, seen)
                     rate = (seen - n0) / max(now - t0, 1e-9)
-                    pr.emit(sched.count_grad_tot, sched.count_com, loss, extra=f" | {rate:,.0f} tok/s/rank | lr {getattr(self, '_last_lr', 0.0):.3e}")
+                    gn_txt = "" if self._grad_norm is None else f" | grad_norm {self._grad_norm:.4g}"
+                    pr.emit(sched.count_grad_tot, sched.count_com, loss, extra=f" | {rate:,.0f} tok/s/rank | lr {getattr(self, '_last_lr', 0.0):.3e}{gn_txt}")
                 self.epoch = pr.epoch
         if committed and plan is not None and self.callbacks:
             self._fire("on_round_end", plan)

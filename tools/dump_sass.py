@@ -25,6 +25,8 @@ KERNELS = {
     "rs_adam_ag_multimem_bf16.sass": "_ZN4acco17rs_adam_ag_kernelI13__nv_bfloat16S1_Li2ELb0EEEvNS_11RoundParamsE",
     "rs_adam_ag_p2p_bf16.sass": "_ZN4acco17rs_adam_ag_kernelI13__nv_bfloat16S1_Li1ELb0EEEvNS_11RoundParamsE",
     "round_gate.sass": "_ZN4acco17round_gate_kernelENS_11RoundParamsE",
+    "round_norm_multimem_bf16.sass": "_ZN4acco17round_norm_kernelI13__nv_bfloat16Li2EEEvNS_11RoundParamsEPff",   # max_grad_norm
+    "round_norm_local_bf16.sass": "_ZN4acco17round_norm_kernelI13__nv_bfloat16Li0EEEvNS_11RoundParamsEPff",
     "attn_fwd_wgmma.sass": "_ZN9acco_attn15attn_fwd_kernelILb0EEEvNS_9FwdParamsE",
     "attn_fwd_wgmma_seg.sass": "_ZN9acco_attn15attn_fwd_kernelILb1EEEvNS_9FwdParamsE",      # document-masked (packed rows)
     "attn_bwd_mma.sass": "_ZN9acco_attn15attn_bwd_kernelILb0EEEvNS_9BwdParamsE",
