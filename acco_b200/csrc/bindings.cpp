@@ -12,10 +12,10 @@
 
 extern "C" {
 int acco_norm_grid(int T, int H, int sms, int backward);
-int acco_rmsnorm_fwd(const void* a, const void* r, const void* w, void* y, void* h, float* rstd, int T, int H, float eps,
-                     int grid, cudaStream_t st);
-int acco_rmsnorm_bwd(const void* dy, const void* dh_extra, const void* h, const void* w, const float* rstd, void* dh,
-                     float* dw_partial, float* dw_out, void* dw_accum_bf16, int T, int H, int grid, cudaStream_t st);
+int acco_norm_fwd(const void* a, const void* r, const void* w, const void* b, void* y, void* h, float* mean, float* rstd, int T, int H,
+                  float eps, int grid, cudaStream_t st);
+int acco_norm_bwd(const void* dy, const void* dh_extra, const void* h, const void* w, const float* mean, const float* rstd, void* dh,
+                  float* partial, float* dwdb_out, void* dw_accum, void* db_accum, int T, int H, int grid, cudaStream_t st);
 int acco_rope_pack_bwd(const void* dq, const void* dk, const void* dv, const long long* strides, void* dqkv, const float* cos_t,
                        const float* sin_t, int B, int S, int Hq, int Hk, int D, int sms, cudaStream_t st);
 int acco_rope_qkv(void* qkv, const float* cos_t, const float* sin_t, int T, int S, int n_rot, int n_total, int D, int inverse,
@@ -26,11 +26,6 @@ int acco_ce_fwd(const void* logits, const long long* labels, float* lse, float* 
                 int V, int Vp, long long ignore_index, cudaStream_t st);
 int acco_ce_bwd(void* logits, const long long* labels, const float* lse, const float* scale, long long T, int V, int Vp,
                 long long ignore_index, cudaStream_t st);
-int acco_layernorm_grid(int T, int H, int sms, int backward);
-int acco_layernorm_fwd(const void* a, const void* r, const void* w, const void* b, void* y, void* h, float* mean, float* rstd, int T, int H,
-                       float eps, int grid, cudaStream_t st);
-int acco_layernorm_bwd(const void* dy, const void* dh_extra, const void* h, const void* w, const float* mean, const float* rstd, void* dh,
-                       float* partial, float* dwdb_out, void* dw_accum_bf16, void* db_accum_bf16, int T, int H, int grid, cudaStream_t st);
 int acco_gelu_fwd(const void* x, void* y, long long n, int sms, cudaStream_t st);
 int acco_gelu_bwd(const void* dy, const void* x, void* dx, long long n, int sms, cudaStream_t st);
 int acco_debug_occupy(unsigned long long ns, int ctas, float* sink, cudaStream_t st);
@@ -98,113 +93,67 @@ void check_f32(const torch::Tensor& t, const char* name) {
 }
 
 // ---------------------------------------------------------------- norms
-std::vector<torch::Tensor> rmsnorm_fwd(torch::Tensor x, torch::Tensor w, double eps) {
-    check_bf16(x, "x"); check_bf16(w, "weight");
-    const c10::cuda::CUDAGuard guard(x.device());
-    const int T = x.size(0), H = x.size(1);
-    auto y = torch::empty_like(x);
-    auto rstd = torch::empty({T}, x.options().dtype(torch::kFloat32));
-    const int grid = acco_norm_grid(T, H, sm_count(), 0);
-    TORCH_CHECK(acco_rmsnorm_fwd(x.data_ptr(), nullptr, w.data_ptr(), y.data_ptr(), nullptr, rstd.data_ptr<float>(), T, H, (float)eps, grid, stream()) == 0,
-                "rmsnorm_fwd: unsupported hidden size ", H);
-    return {y, rstd};
-}
-
-std::vector<torch::Tensor> add_rmsnorm_fwd(torch::Tensor a, torch::Tensor r, torch::Tensor w, double eps) {
-    check_bf16(a, "a"); check_bf16(r, "r"); check_bf16(w, "weight");
-    const c10::cuda::CUDAGuard guard(a.device());
-    const int T = a.size(0), H = a.size(1);
-    auto y = torch::empty_like(a);
-    auto h = torch::empty_like(a);
-    auto rstd = torch::empty({T}, a.options().dtype(torch::kFloat32));
-    const int grid = acco_norm_grid(T, H, sm_count(), 0);
-    TORCH_CHECK(acco_rmsnorm_fwd(a.data_ptr(), r.data_ptr(), w.data_ptr(), y.data_ptr(), h.data_ptr(), rstd.data_ptr<float>(), T, H, (float)eps, grid, stream()) == 0,
-                "add_rmsnorm_fwd: unsupported hidden size ", H);
-    return {y, h, rstd};
-}
-
-// If `wgrad` (the weight's existing bf16 .grad) is defined, dw is accumulated into it and the returned dw is empty.
-std::vector<torch::Tensor> norm_bwd_impl(torch::Tensor dy, const torch::Tensor* de, torch::Tensor h, torch::Tensor w, torch::Tensor rstd,
-                                         c10::optional<torch::Tensor> wgrad) {
-    check_bf16(dy, "dy"); check_bf16(h, "h"); check_bf16(w, "weight"); check_f32(rstd, "rstd");
-    const c10::cuda::CUDAGuard guard(dy.device());
-    const int T = dy.size(0), H = dy.size(1);
-    auto dh = torch::empty_like(dy);
-    const int grid = acco_norm_grid(T, H, sm_count(), 1);
-    auto partial = torch::empty({grid, H}, dy.options().dtype(torch::kFloat32));
-    torch::Tensor dw;
-    void* accum = nullptr;
-    if (wgrad.has_value() && wgrad->defined()) {
-        check_bf16(*wgrad, "weight.grad");
-        TORCH_CHECK(wgrad->numel() == H, "weight.grad has the wrong size");
-        accum = wgrad->data_ptr();
-        dw = torch::empty({0}, dy.options().dtype(torch::kFloat32));
-    } else {
-        dw = torch::empty({H}, dy.options().dtype(torch::kFloat32));
-    }
-    TORCH_CHECK(acco_rmsnorm_bwd(dy.data_ptr(), de ? de->data_ptr() : nullptr, h.data_ptr(), w.data_ptr(), rstd.data_ptr<float>(), dh.data_ptr(),
-                                 partial.data_ptr<float>(), accum ? nullptr : dw.data_ptr<float>(), accum, T, H, grid, stream()) == 0,
-                "rmsnorm_bwd: unsupported hidden size ", H);
-    return {dh, dw};
-}
-std::vector<torch::Tensor> rmsnorm_bwd(torch::Tensor dy, torch::Tensor x, torch::Tensor w, torch::Tensor rstd, c10::optional<torch::Tensor> wgrad) {
-    return norm_bwd_impl(dy, nullptr, x, w, rstd, wgrad);
-}
-std::vector<torch::Tensor> add_rmsnorm_bwd(torch::Tensor dy, torch::Tensor dh_extra, torch::Tensor h, torch::Tensor w, torch::Tensor rstd,
-                                           c10::optional<torch::Tensor> wgrad) {
-    check_bf16(dh_extra, "dh_extra");
-    return norm_bwd_impl(dy, &dh_extra, h, w, rstd, wgrad);
-}
-
-// ---------------------------------------------------------------- layernorm / gelu (GPT family)
-// r undefined: plain LayerNorm (returns {y, mean, rstd}); else {y, h = a + r, mean, rstd}
-std::vector<torch::Tensor> layernorm_fwd(torch::Tensor a, c10::optional<torch::Tensor> r, torch::Tensor w, torch::Tensor b, double eps) {
-    check_bf16(a, "a"); check_bf16(w, "weight"); check_bf16(b, "bias");
-    const bool has_r = r.has_value() && r->defined();
+// RMSNorm when b is undefined, LayerNorm otherwise; r defined: fused residual add.  Returns {y, h = a + r, mean, rstd};
+// h is None without r and mean is None for RMSNorm.
+std::vector<torch::Tensor> norm_fwd(torch::Tensor a, c10::optional<torch::Tensor> r, torch::Tensor w, c10::optional<torch::Tensor> b,
+                                    double eps) {
+    check_bf16(a, "a"); check_bf16(w, "weight");
+    const bool has_r = r.has_value() && r->defined(), layer = b.has_value() && b->defined();
     if (has_r) check_bf16(*r, "r");
+    if (layer) check_bf16(*b, "bias");
     const c10::cuda::CUDAGuard guard(a.device());
     const int T = a.size(0), H = a.size(1);
-    TORCH_CHECK(w.numel() == H && b.numel() == H, "layernorm: weight/bias size");
+    TORCH_CHECK(w.numel() == H && (!layer || b->numel() == H), "norm: weight/bias size");
     auto y = torch::empty_like(a);
     auto f32 = a.options().dtype(torch::kFloat32);
-    auto mean = torch::empty({T}, f32), rstd = torch::empty({T}, f32);
+    auto rstd = torch::empty({T}, f32);
+    torch::Tensor mean = layer ? torch::empty({T}, f32) : torch::Tensor();
     torch::Tensor h = has_r ? torch::empty_like(a) : torch::Tensor();
-    const int grid = acco_layernorm_grid(T, H, sm_count(), 0);
-    TORCH_CHECK(acco_layernorm_fwd(a.data_ptr(), has_r ? r->data_ptr() : nullptr, w.data_ptr(), b.data_ptr(), y.data_ptr(), has_r ? h.data_ptr() : nullptr,
-                                   mean.data_ptr<float>(), rstd.data_ptr<float>(), T, H, (float)eps, grid, stream()) == 0,
-                "layernorm_fwd: unsupported hidden size ", H);
-    if (has_r) return {y, h, mean, rstd};
-    return {y, mean, rstd};
+    const int grid = acco_norm_grid(T, H, sm_count(), 0);
+    TORCH_CHECK(acco_norm_fwd(a.data_ptr(), has_r ? r->data_ptr() : nullptr, w.data_ptr(), layer ? b->data_ptr() : nullptr, y.data_ptr(),
+                              has_r ? h.data_ptr() : nullptr, layer ? mean.data_ptr<float>() : nullptr, rstd.data_ptr<float>(), T, H,
+                              (float)eps, grid, stream()) == 0,
+                "norm_fwd: unsupported hidden size ", H);
+    return {y, h, mean, rstd};
 }
 
-// Returns {dh, dwdb}: dwdb is fp32 [2H] (dw | db), or empty when both bf16 accumulation targets (the parameters' .grad views) are given.
-std::vector<torch::Tensor> layernorm_bwd(torch::Tensor dy, c10::optional<torch::Tensor> dh_extra, torch::Tensor h, torch::Tensor w, torch::Tensor mean,
-                                         torch::Tensor rstd, c10::optional<torch::Tensor> wgrad, c10::optional<torch::Tensor> bgrad) {
-    check_bf16(dy, "dy"); check_bf16(h, "h"); check_bf16(w, "weight"); check_f32(mean, "mean"); check_f32(rstd, "rstd");
-    const bool has_e = dh_extra.has_value() && dh_extra->defined();
+// RMSNorm when mean is undefined, LayerNorm otherwise.  Returns {dh, dwdb}: dwdb is fp32 [H] (dw) or [2H] (dw | db), or
+// empty when the parameters' existing bf16 .grad (wgrad, and bgrad for LayerNorm) are given: the sums are then added to them.
+std::vector<torch::Tensor> norm_bwd(torch::Tensor dy, c10::optional<torch::Tensor> dh_extra, torch::Tensor h, torch::Tensor w,
+                                    c10::optional<torch::Tensor> mean, torch::Tensor rstd, c10::optional<torch::Tensor> wgrad,
+                                    c10::optional<torch::Tensor> bgrad) {
+    check_bf16(dy, "dy"); check_bf16(h, "h"); check_bf16(w, "weight"); check_f32(rstd, "rstd");
+    const bool has_e = dh_extra.has_value() && dh_extra->defined(), layer = mean.has_value() && mean->defined();
     if (has_e) check_bf16(*dh_extra, "dh_extra");
+    if (layer) check_f32(*mean, "mean");
     const c10::cuda::CUDAGuard guard(dy.device());
-    const int T = dy.size(0), H = dy.size(1);
+    const int T = dy.size(0), H = dy.size(1), np = layer ? 2 : 1;
     auto dh = torch::empty_like(dy);
-    const int grid = acco_layernorm_grid(T, H, sm_count(), 1);
+    const int grid = acco_norm_grid(T, H, sm_count(), 1);
     auto f32 = dy.options().dtype(torch::kFloat32);
-    auto partial = torch::empty({grid, 2 * H}, f32);
-    const bool accum = wgrad.has_value() && wgrad->defined() && bgrad.has_value() && bgrad->defined();
+    auto partial = torch::empty({grid, np * H}, f32);
+    const bool accum = wgrad.has_value() && wgrad->defined() && (!layer || (bgrad.has_value() && bgrad->defined()));
     torch::Tensor dwdb;
     if (accum) {
-        check_bf16(*wgrad, "weight.grad"); check_bf16(*bgrad, "bias.grad");
-        TORCH_CHECK(wgrad->numel() == H && bgrad->numel() == H, "grad sizes");
+        check_bf16(*wgrad, "weight.grad");
+        TORCH_CHECK(wgrad->numel() == H, "weight.grad has the wrong size");
+        if (layer) {
+            check_bf16(*bgrad, "bias.grad");
+            TORCH_CHECK(bgrad->numel() == H, "bias.grad has the wrong size");
+        }
         dwdb = torch::empty({0}, f32);
     } else {
-        dwdb = torch::empty({2 * H}, f32);
+        dwdb = torch::empty({np * H}, f32);
     }
-    TORCH_CHECK(acco_layernorm_bwd(dy.data_ptr(), has_e ? dh_extra->data_ptr() : nullptr, h.data_ptr(), w.data_ptr(), mean.data_ptr<float>(),
-                                   rstd.data_ptr<float>(), dh.data_ptr(), partial.data_ptr<float>(), accum ? nullptr : dwdb.data_ptr<float>(),
-                                   accum ? wgrad->data_ptr() : nullptr, accum ? bgrad->data_ptr() : nullptr, T, H, grid, stream()) == 0,
-                "layernorm_bwd: unsupported hidden size ", H);
+    TORCH_CHECK(acco_norm_bwd(dy.data_ptr(), has_e ? dh_extra->data_ptr() : nullptr, h.data_ptr(), w.data_ptr(),
+                              layer ? mean->data_ptr<float>() : nullptr, rstd.data_ptr<float>(), dh.data_ptr(), partial.data_ptr<float>(),
+                              accum ? nullptr : dwdb.data_ptr<float>(), accum ? wgrad->data_ptr() : nullptr,
+                              accum && layer ? bgrad->data_ptr() : nullptr, T, H, grid, stream()) == 0,
+                "norm_bwd: unsupported hidden size ", H);
     return {dh, dwdb};
 }
 
+// ---------------------------------------------------------------- gelu (GPT family)
 torch::Tensor gelu_fwd(torch::Tensor x) {
     check_bf16(x, "x");
     const c10::cuda::CUDAGuard guard(x.device());
@@ -583,12 +532,8 @@ torch::Tensor pack_const_len_native(torch::Tensor flat_tokens, torch::Tensor doc
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     TORCH_CHECK(acco_round_params_size() == (int)sizeof(RoundParams), "RoundParams layout mismatch between bindings.cpp and rs_adam_ag.cu");
-    m.def("rmsnorm_fwd", &rmsnorm_fwd);
-    m.def("rmsnorm_bwd", &rmsnorm_bwd);
-    m.def("add_rmsnorm_fwd", &add_rmsnorm_fwd);
-    m.def("add_rmsnorm_bwd", &add_rmsnorm_bwd);
-    m.def("layernorm_fwd", &layernorm_fwd);
-    m.def("layernorm_bwd", &layernorm_bwd);
+    m.def("norm_fwd", &norm_fwd);
+    m.def("norm_bwd", &norm_bwd);
     m.def("gelu_fwd", &gelu_fwd);
     m.def("gelu_bwd", &gelu_bwd);
     m.def("rope_qkv_inplace", &rope_qkv_inplace);

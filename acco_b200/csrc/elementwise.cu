@@ -1,4 +1,4 @@
-// RoPE (in place on the fused QKV buffer) and SwiGLU forward/backward.  Pure streaming kernels:
+// RoPE (in place on the fused QKV buffer), SwiGLU and GELU-new forward/backward.  Pure streaming kernels:
 // 16-byte vector accesses, one pass, grid sized by the caller's element count.
 #include <stdlib.h>
 
@@ -148,6 +148,40 @@ __global__ void __launch_bounds__(256) swiglu_bwd_kernel(const __nv_bfloat16* __
     }
 }
 
+// ---- GELU (tanh approximation, "gelu_new") --------------------------------------------------------------------------
+ACCO_DEVINL float gelu_new_f(float x) {
+    const float k0 = 0.7978845608028654f, k1 = 0.044715f;
+    const float t = tanhf(k0 * (x + k1 * x * x * x));
+    return 0.5f * x * (1.f + t);
+}
+ACCO_DEVINL float gelu_new_grad(float x) {
+    const float k0 = 0.7978845608028654f, k1 = 0.044715f;
+    const float u = k0 * (x + k1 * x * x * x);
+    const float t = tanhf(u);
+    return 0.5f * (1.f + t) + 0.5f * x * (1.f - t * t) * k0 * (1.f + 3.f * k1 * x * x);
+}
+
+__global__ void __launch_bounds__(256) gelu_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y, long long nvec) {
+    for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += (long long)gridDim.x * blockDim.x) {
+        float f[8];
+        unpack8(ld_stream(x + 8 * v), f);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) f[j] = gelu_new_f(f[j]);
+        st_stream(y + 8 * v, pack8(f));
+    }
+}
+__global__ void __launch_bounds__(256) gelu_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
+                                                       __nv_bfloat16* __restrict__ dx, long long nvec) {
+    for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += (long long)gridDim.x * blockDim.x) {
+        float f[8], g[8];
+        unpack8(ld_stream(x + 8 * v), f);
+        unpack8(ld_stream(dy + 8 * v), g);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) g[j] *= gelu_new_grad(f[j]);
+        st_stream(dx + 8 * v, pack8(g));
+    }
+}
+
 static int grid_for(long long work_items, int threads, int sms) {
     long long want = (work_items + threads - 1) / threads;
     long long cap = (long long)sms * (2048 / threads) * 4;  // a few waves; kernels are grid-stride
@@ -190,6 +224,24 @@ extern "C" int acco_swiglu_bwd(const void* dout, const void* gu, void* dgu, long
     acco::swiglu_bwd_kernel<<<acco::grid_for(T * (I / 8), 256, sms), 256, 0, st>>>(
         (const __nv_bfloat16*)dout, (const __nv_bfloat16*)gu, (__nv_bfloat16*)dgu, T, I);
     return 0;
+}
+
+extern "C" int acco_gelu_fwd(const void* x, void* y, long long n, int sms, cudaStream_t st) {
+    if (n % 8) return -1;
+    const long long nvec = n / 8;
+    long long want = (nvec + 255) / 256;
+    const long long cap = (long long)sms * 16;
+    acco::gelu_fwd_kernel<<<(int)(want < cap ? (want < 1 ? 1 : want) : cap), 256, 0, st>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, nvec);
+    return (int)cudaGetLastError();
+}
+extern "C" int acco_gelu_bwd(const void* dy, const void* x, void* dx, long long n, int sms, cudaStream_t st) {
+    if (n % 8) return -1;
+    const long long nvec = n / 8;
+    long long want = (nvec + 255) / 256;
+    const long long cap = (long long)sms * 16;
+    acco::gelu_bwd_kernel<<<(int)(want < cap ? (want < 1 ? 1 : want) : cap), 256, 0, st>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x,
+                                                                                           (__nv_bfloat16*)dx, nvec);
+    return (int)cudaGetLastError();
 }
 
 // ---- debug: an SM "occupier" with the resource footprint of the NVLS round kernel (256 threads x 64 registers, no dynamic smem),

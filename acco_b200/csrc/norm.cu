@@ -1,176 +1,229 @@
-// RMSNorm / fused residual-add + RMSNorm, forward and backward, bf16 I/O with fp32 statistics.
+// RMSNorm and LayerNorm (weight + bias), each with an optional fused residual add: forward and backward, bf16 I/O with
+// fp32 statistics.  One kernel pair serves both norms; LAYER = false is RMSNorm, whose mean, bias and db disappear at
+// compile time.
 //
-// Replaces HF Llama's ~7 eager kernels per norm (modeling_llama.py:53-70).
-// Layout: x [T, H] row-major bf16.  A row is owned by `tpr` consecutive threads (a multiple of
-// 32), each holding VPT 16-byte vectors of the row in registers as packed bf16, so every element
-// is read from HBM exactly once per pass; a CTA of 256..512 threads processes several rows at a
-// time and walks the rows grid-stride (persistent).
-//   fwd :  h = a (+ r);  rstd = rsqrt(mean(h^2) + eps);  y = h * rstd * w
-//   bwd :  xh = h*rstd;  wdy = dy*w;  c = mean(wdy * xh);  dh = rstd*(wdy - xh*c) (+ dh_extra)
-//          dw = sum_rows dy * xh  -> per-CTA fp32 partials, reduced by a second tiny kernel
-//          (deterministic, no atomics)
+//   fwd :  h = a (+ r);  RMSNorm:   rstd = rsqrt(mean(h^2) + eps);                       y = h * rstd * w
+//                        LayerNorm: mu = mean(h);  rstd = rsqrt(mean((h-mu)^2) + eps);   y = (h-mu) * rstd * w + b
+//   bwd :  xh = (h-mu)*rstd (mu = 0 for RMSNorm);  g = dy*w;  c1 = mean(g*xh);  c2 = mean(g) (LayerNorm only)
+//          dh = rstd*(g - c2 - xh*c1) (+ dh_extra)
+//          dw = sum_rows dy*xh,  db = sum_rows dy  -> per-CTA fp32 partials [grid][NP*H] (NP = 1: dw; NP = 2: dw | db),
+//          reduced by a second tiny kernel (deterministic, no atomics)
+//
+// One WARP per row for H <= 1024 (every 16-byte vector of the row in flight at once, no block barrier in the row loop);
+// one CTA per row above that, up to H = 16384.  Both walk the rows grid-stride (persistent).
 #include "common.cuh"
 
 namespace acco {
 
-// sum `v` over the `tpr` threads that own one row.  `red` has one float per warp of the CTA.
-ACCO_DEVINL float row_sum(float v, float* red, int tpr) {
-    v = warp_sum(v);
-    if (tpr == 32) return v;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    __syncthreads();
-    if (lane == 0) red[warp] = v;
-    __syncthreads();
-    const int wpr = tpr >> 5;
-    const int w0 = (warp / wpr) * wpr;
-    float s = 0.f;
-    for (int k = 0; k < wpr; ++k) s += red[w0 + k];
-    return s;
+constexpr int kWarpsPerCta = 8;        // warp-per-row CTAs: 8 rows per CTA per iteration
+constexpr int kMaxCtaThreads = 512;    // CTA-per-row CTAs: up to 512 threads, each holding VPT vectors of the row
+constexpr int kMaxH = 16384;
+
+// sum over the owners of one row: a warp (CTA_ROW = false) or the whole CTA (CTA_ROW = true)
+template <bool CTA_ROW>
+ACCO_DEVINL float row_sum(float v, float* red) {
+    if constexpr (CTA_ROW) return block_sum(v, red);
+    else return warp_sum(v);
 }
 
-template <int VPT, bool HAS_RES>
-__global__ void __launch_bounds__(512) rmsnorm_fwd_kernel(
+template <int VPT, bool HAS_RES, bool CTA_ROW, bool LAYER>
+__global__ void __launch_bounds__(CTA_ROW ? kMaxCtaThreads : kWarpsPerCta * 32) norm_fwd_kernel(
     const __nv_bfloat16* __restrict__ a, const __nv_bfloat16* __restrict__ r, const __nv_bfloat16* __restrict__ w,
-    __nv_bfloat16* __restrict__ y, __nv_bfloat16* __restrict__ h_out, float* __restrict__ rstd_out, int T, int H,
-    float eps, int tpr) {
+    const __nv_bfloat16* __restrict__ b, __nv_bfloat16* __restrict__ y, __nv_bfloat16* __restrict__ h_out,
+    float* __restrict__ mean_out, float* __restrict__ rstd_out, int T, int H, float eps) {
     __shared__ float red[32];
-    const int rpc = blockDim.x / tpr;           // rows per CTA iteration
-    const int lrow = threadIdx.x / tpr, t = threadIdx.x % tpr;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int tid = CTA_ROW ? threadIdx.x : lane;               // index among the owners of a row
+    const int stride = CTA_ROW ? blockDim.x : 32;
     const int nvec = H >> 3;
-    bf16x8 wv[VPT];
-#pragma unroll
-    for (int i = 0; i < VPT; ++i) {
-        const int v = t + tpr * i;
-        if (v < nvec) wv[i] = ld_vec(w + 8 * v);
-    }
-    for (int row0 = blockIdx.x * rpc; row0 < T; row0 += gridDim.x * rpc) {
-        const int row = row0 + lrow;
-        const bool rv_ok = row < T;
+    const int row_step = CTA_ROW ? gridDim.x : gridDim.x * kWarpsPerCta;
+    for (int row = CTA_ROW ? blockIdx.x : blockIdx.x * kWarpsPerCta + warp; row < T; row += row_step) {
         const size_t base = (size_t)row * H;
-        bf16x8 hv[VPT];
-        float ss = 0.f;
+        bf16x8 av[VPT], rv[VPT];
 #pragma unroll
-        for (int i = 0; i < VPT; ++i) {
-            const int v = t + tpr * i;
-            if (rv_ok && v < nvec) {
-                bf16x8 av = ld_stream(a + base + 8 * v);
-                if (HAS_RES) {
-                    bf16x8 rv = ld_stream(r + base + 8 * v);
-                    float fa[8], fr[8];
-                    unpack8(av, fa);
-                    unpack8(rv, fr);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) fa[j] += fr[j];
-                    av = pack8(fa);  // h is *stored* in bf16: normalise exactly what is stored
-                    st_vec(h_out + base + 8 * v, av);
-                }
-                hv[i] = av;
-                float f[8];
-                unpack8(av, f);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) ss += f[j] * f[j];
+        for (int i = 0; i < VPT; ++i) {            // issue every load of the row before touching any
+            const int v = tid + stride * i;
+            if (v < nvec) {
+                av[i] = ld_stream(a + base + 8 * v);
+                if (HAS_RES) rv[i] = ld_stream(r + base + 8 * v);
             }
         }
-        ss = row_sum(ss, red, tpr);
-        const float rstd = rsqrtf(ss / (float)H + eps);
-        if (rv_ok && t == 0) rstd_out[row] = rstd;
+        float s = 0.f;                             // sum(h) for LayerNorm, sum(h^2) for RMSNorm
 #pragma unroll
         for (int i = 0; i < VPT; ++i) {
-            const int v = t + tpr * i;
-            if (rv_ok && v < nvec) {
-                float f[8], fw[8];
-                unpack8(hv[i], f);
-                unpack8(wv[i], fw);
+            const int v = tid + stride * i;
+            if (v < nvec) {
+                float fa[8];
+                unpack8(av[i], fa);
+                if (HAS_RES) {
+                    float fr[8];
+                    unpack8(rv[i], fr);
 #pragma unroll
-                for (int j = 0; j < 8; ++j) f[j] = f[j] * rstd * fw[j];
+                    for (int j = 0; j < 8; ++j) fa[j] += fr[j];
+                    av[i] = pack8(fa);
+                    st_vec(h_out + base + 8 * v, av[i]);
+                    unpack8(av[i], fa);            // normalise exactly what was stored (bf16)
+                }
+#pragma unroll
+                for (int j = 0; j < 8; ++j) s += LAYER ? fa[j] : fa[j] * fa[j];
+            }
+        }
+        float mu = 0.f, rstd;
+        if constexpr (LAYER) {
+            mu = row_sum<CTA_ROW>(s, red) / (float)H;
+            float ss = 0.f;
+#pragma unroll
+            for (int i = 0; i < VPT; ++i) {
+                const int v = tid + stride * i;
+                if (v < nvec) {
+                    float fa[8];
+                    unpack8(av[i], fa);
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) ss += (fa[j] - mu) * (fa[j] - mu);
+                }
+            }
+            rstd = rsqrtf(row_sum<CTA_ROW>(ss, red) / (float)H + eps);
+        } else {
+            rstd = rsqrtf(row_sum<CTA_ROW>(s, red) / (float)H + eps);
+        }
+        if (tid == 0) {
+            if constexpr (LAYER) mean_out[row] = mu;
+            rstd_out[row] = rstd;
+        }
+#pragma unroll
+        for (int i = 0; i < VPT; ++i) {
+            const int v = tid + stride * i;
+            if (v < nvec) {
+                float f[8], fw[8];
+                unpack8(av[i], f);
+                unpack8(ld_vec(w + 8 * v), fw);
+                if constexpr (LAYER) {
+                    float fb[8];
+                    unpack8(ld_vec(b + 8 * v), fb);
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) f[j] = (f[j] - mu) * rstd * fw[j] + fb[j];
+                } else {
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) f[j] = f[j] * rstd * fw[j];
+                }
                 st_stream(y + base + 8 * v, pack8(f));
             }
         }
     }
 }
 
-template <int VPT, bool HAS_EXTRA>
-__global__ void __launch_bounds__(512) rmsnorm_bwd_kernel(
-    const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ dh_extra,
-    const __nv_bfloat16* __restrict__ h, const __nv_bfloat16* __restrict__ w, const float* __restrict__ rstd_in,
-    __nv_bfloat16* __restrict__ dh, float* __restrict__ dw_partial, int T, int H, int tpr) {
-    extern __shared__ float dyn[];              // [blockDim.x * 8] staging for the CTA-level dw reduction
+// partial layout: [grid][NP][H] (dw, then db for LayerNorm)
+template <int VPT, bool HAS_EXTRA, bool CTA_ROW, bool LAYER>
+__global__ void __launch_bounds__(CTA_ROW ? kMaxCtaThreads : kWarpsPerCta * 32) norm_bwd_kernel(
+    const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ dh_extra, const __nv_bfloat16* __restrict__ h,
+    const __nv_bfloat16* __restrict__ w, const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
+    __nv_bfloat16* __restrict__ dh, float* __restrict__ partial, int T, int H) {
+    constexpr int NP = LAYER ? 2 : 1;
+    extern __shared__ float dyn[];                 // warp rows: [kWarpsPerCta][256] staging for the CTA-level reduction
     __shared__ float red[32];
-    const int rpc = blockDim.x / tpr;
-    const int lrow = threadIdx.x / tpr, t = threadIdx.x % tpr;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int tid = CTA_ROW ? threadIdx.x : lane;
+    const int stride = CTA_ROW ? blockDim.x : 32;
     const int nvec = H >> 3;
-    bf16x8 wv[VPT];
-    float dw[VPT][8];
+    const int row_step = CTA_ROW ? gridDim.x : gridDim.x * kWarpsPerCta;
+    float acc[NP][VPT][8];                         // acc[0] = dw, acc[1] = db
 #pragma unroll
-    for (int i = 0; i < VPT; ++i) {
-        const int v = t + tpr * i;
-        if (v < nvec) wv[i] = ld_vec(w + 8 * v);
+    for (int p = 0; p < NP; ++p)
 #pragma unroll
-        for (int j = 0; j < 8; ++j) dw[i][j] = 0.f;
-    }
-    for (int row0 = blockIdx.x * rpc; row0 < T; row0 += gridDim.x * rpc) {
-        const int row = row0 + lrow;
-        const bool rv_ok = row < T;
+        for (int i = 0; i < VPT; ++i)
+#pragma unroll
+            for (int j = 0; j < 8; ++j) acc[p][i][j] = 0.f;
+    for (int row = CTA_ROW ? blockIdx.x : blockIdx.x * kWarpsPerCta + warp; row < T; row += row_step) {
         const size_t base = (size_t)row * H;
-        const float rstd = rv_ok ? rstd_in[row] : 0.f;
-        bf16x8 dyv[VPT], hv[VPT];
-        float c = 0.f;
+        bf16x8 dyv[VPT], hv[VPT], ev[VPT];
 #pragma unroll
         for (int i = 0; i < VPT; ++i) {
-            const int v = t + tpr * i;
-            if (rv_ok && v < nvec) {
+            const int v = tid + stride * i;
+            if (v < nvec) {
                 dyv[i] = ld_stream(dy + base + 8 * v);
                 hv[i] = ld_stream(h + base + 8 * v);
+                if (HAS_EXTRA && !CTA_ROW) ev[i] = ld_stream(dh_extra + base + 8 * v);
+            }
+        }
+        const float mu = LAYER ? mean_in[row] : 0.f, rstd = rstd_in[row];
+        float c1 = 0.f, c2 = 0.f;
+#pragma unroll
+        for (int i = 0; i < VPT; ++i) {
+            const int v = tid + stride * i;
+            if (v < nvec) {
                 float fd[8], fh[8], fw[8];
                 unpack8(dyv[i], fd);
                 unpack8(hv[i], fh);
-                unpack8(wv[i], fw);
+                unpack8(ld_vec(w + 8 * v), fw);
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
-                    const float xh = fh[j] * rstd;
-                    c += fd[j] * fw[j] * xh;
-                    dw[i][j] += fd[j] * xh;
+                    const float xh = (LAYER ? fh[j] - mu : fh[j]) * rstd, g = fd[j] * fw[j];
+                    c1 += g * xh;
+                    acc[0][i][j] += fd[j] * xh;
+                    if constexpr (LAYER) {
+                        c2 += g;
+                        acc[1][i][j] += fd[j];
+                    }
                 }
             }
         }
-        c = row_sum(c, red, tpr) / (float)H;
+        c1 = row_sum<CTA_ROW>(c1, red) / (float)H;
+        if constexpr (LAYER) c2 = row_sum<CTA_ROW>(c2, red) / (float)H;
 #pragma unroll
         for (int i = 0; i < VPT; ++i) {
-            const int v = t + tpr * i;
-            if (rv_ok && v < nvec) {
+            const int v = tid + stride * i;
+            if (v < nvec) {
                 float fd[8], fh[8], fw[8], o[8];
                 unpack8(dyv[i], fd);
                 unpack8(hv[i], fh);
-                unpack8(wv[i], fw);
-                if (HAS_EXTRA) {
-                    float fe[8];
-                    unpack8(ld_stream(dh_extra + base + 8 * v), fe);
+                unpack8(ld_vec(w + 8 * v), fw);
+                if constexpr (LAYER) {
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) o[j] = fe[j] + rstd * (fd[j] * fw[j] - fh[j] * rstd * c);
+                    for (int j = 0; j < 8; ++j) o[j] = rstd * (fd[j] * fw[j] - c2 - (fh[j] - mu) * rstd * c1);
                 } else {
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) o[j] = rstd * (fd[j] * fw[j] - fh[j] * rstd * c);
+                    for (int j = 0; j < 8; ++j) o[j] = rstd * (fd[j] * fw[j] - fh[j] * rstd * c1);
+                }
+                if (HAS_EXTRA) {
+                    // a CTA row reads dh_extra only here: held from the start it would make the LayerNorm VPT = 4 kernel spill
+                    float fe[8];
+                    unpack8(CTA_ROW ? ld_stream(dh_extra + base + 8 * v) : ev[i], fe);
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) o[j] += fe[j];
                 }
                 st_stream(dh + base + 8 * v, pack8(o));
             }
         }
     }
-    // reduce dw over the rpc row-groups of the CTA, then emit this CTA's partial
+    float* my = partial + (size_t)blockIdx.x * NP * H;
+    if constexpr (CTA_ROW) {
+        // every thread owns distinct columns: write its sums directly
 #pragma unroll
-    for (int i = 0; i < VPT; ++i) {
-        __syncthreads();
-#pragma unroll
-        for (int j = 0; j < 8; ++j) dyn[(lrow * tpr + t) * 8 + j] = dw[i][j];
-        __syncthreads();
-        if (lrow == 0) {
-            const int v = t + tpr * i;
+        for (int i = 0; i < VPT; ++i) {
+            const int v = tid + stride * i;
             if (v < nvec) {
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    float s = 0.f;
-                    for (int k = 0; k < rpc; ++k) s += dyn[(k * tpr + t) * 8 + j];
-                    dw_partial[(size_t)blockIdx.x * H + 8 * v + j] = s;
-                }
+                for (int p = 0; p < NP; ++p)
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) my[p * H + 8 * v + j] = acc[p][i][j];
+            }
+        }
+    } else {
+        // the warps of the CTA own the same columns of different rows: reduce over warps through smem
+#pragma unroll
+        for (int p = 0; p < NP; ++p) {
+#pragma unroll
+            for (int i = 0; i < VPT; ++i) {
+                __syncthreads();
+#pragma unroll
+                for (int j = 0; j < 8; ++j) dyn[warp * 256 + lane * 8 + j] = acc[p][i][j];
+                __syncthreads();
+                const int col = threadIdx.x;               // 256 threads <-> the 256 columns of chunk i
+                float s = 0.f;
+#pragma unroll
+                for (int k = 0; k < kWarpsPerCta; ++k) s += dyn[k * 256 + col];
+                const int gcol = 256 * i + col;
+                if (gcol < H) my[p * H + gcol] = s;
             }
         }
     }
@@ -204,267 +257,123 @@ __global__ void __launch_bounds__(1024) reduce_partials_kernel(const float* __re
     }
 }
 
-// ------------------------------------------------------------------------------------------------------------
-// Warp-per-row variants for H <= 1024 (VPT <= 4 vectors per lane): no __syncthreads in the row loop, the whole row
-// of every tensor is in flight per warp (Little's law: ~35 KB/SM must be outstanding to saturate HBM3e).
-// ------------------------------------------------------------------------------------------------------------
-constexpr int kWarpsPerCta = 8;
-
-template <int VPT, bool HAS_RES>
-__global__ void __launch_bounds__(kWarpsPerCta * 32) rmsnorm_fwd_warp_kernel(
-    const __nv_bfloat16* __restrict__ a, const __nv_bfloat16* __restrict__ r, const __nv_bfloat16* __restrict__ w,
-    __nv_bfloat16* __restrict__ y, __nv_bfloat16* __restrict__ h_out, float* __restrict__ rstd_out, int T, int H, float eps) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int nvec = H >> 3;
-    bf16x8 wv[VPT];
-#pragma unroll
-    for (int i = 0; i < VPT; ++i) {
-        const int v = lane + 32 * i;
-        if (v < nvec) wv[i] = ld_vec(w + 8 * v);
-    }
-    for (int row = blockIdx.x * kWarpsPerCta + warp; row < T; row += gridDim.x * kWarpsPerCta) {
-        const size_t base = (size_t)row * H;
-        bf16x8 av[VPT], rv[VPT];
-#pragma unroll
-        for (int i = 0; i < VPT; ++i) {            // issue every load of the row before touching any
-            const int v = lane + 32 * i;
-            if (v < nvec) {
-                av[i] = ld_stream(a + base + 8 * v);
-                if (HAS_RES) rv[i] = ld_stream(r + base + 8 * v);
-            }
-        }
-        float ss = 0.f;
-#pragma unroll
-        for (int i = 0; i < VPT; ++i) {
-            const int v = lane + 32 * i;
-            if (v < nvec) {
-                float fa[8];
-                unpack8(av[i], fa);
-                if (HAS_RES) {
-                    float fr[8];
-                    unpack8(rv[i], fr);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) fa[j] += fr[j];
-                    av[i] = pack8(fa);
-                    st_vec(h_out + base + 8 * v, av[i]);
-                    unpack8(av[i], fa);            // normalise exactly what was stored (bf16)
-                }
-#pragma unroll
-                for (int j = 0; j < 8; ++j) ss += fa[j] * fa[j];
-            }
-        }
-        ss = warp_sum(ss);
-        const float rstd = rsqrtf(ss / (float)H + eps);
-        if (lane == 0) rstd_out[row] = rstd;
-#pragma unroll
-        for (int i = 0; i < VPT; ++i) {
-            const int v = lane + 32 * i;
-            if (v < nvec) {
-                float f[8], fw[8];
-                unpack8(av[i], f);
-                unpack8(wv[i], fw);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) f[j] = f[j] * rstd * fw[j];
-                st_stream(y + base + 8 * v, pack8(f));
-            }
-        }
-    }
+// out[col] (fp32) = or accum[col] (bf16) += sum_p partial[p * pitch + col], col < width
+static void reduce_partials(const float* partial, float* out, void* accum_bf16, int nparts, int width, int pitch, cudaStream_t st) {
+    reduce_partials_kernel<<<(width + 31) / 32, 1024, 0, st>>>(partial, out, (__nv_bfloat16*)accum_bf16, nparts, width, pitch);
 }
 
-template <int VPT, bool HAS_EXTRA>
-__global__ void __launch_bounds__(kWarpsPerCta * 32) rmsnorm_bwd_warp_kernel(
-    const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ dh_extra, const __nv_bfloat16* __restrict__ h,
-    const __nv_bfloat16* __restrict__ w, const float* __restrict__ rstd_in, __nv_bfloat16* __restrict__ dh,
-    float* __restrict__ dw_partial, int T, int H) {
-    extern __shared__ float dyn[];                 // [kWarpsPerCta][32*8] staging for the CTA-level dw reduction
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int nvec = H >> 3;
-    bf16x8 wv[VPT];
-    float dw[VPT][8];
-#pragma unroll
-    for (int i = 0; i < VPT; ++i) {
-        const int v = lane + 32 * i;
-        if (v < nvec) wv[i] = ld_vec(w + 8 * v);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) dw[i][j] = 0.f;
-    }
-    for (int row = blockIdx.x * kWarpsPerCta + warp; row < T; row += gridDim.x * kWarpsPerCta) {
-        const size_t base = (size_t)row * H;
-        bf16x8 dyv[VPT], hv[VPT], ev[VPT];
-#pragma unroll
-        for (int i = 0; i < VPT; ++i) {
-            const int v = lane + 32 * i;
-            if (v < nvec) {
-                dyv[i] = ld_stream(dy + base + 8 * v);
-                hv[i] = ld_stream(h + base + 8 * v);
-                if (HAS_EXTRA) ev[i] = ld_stream(dh_extra + base + 8 * v);
-            }
-        }
-        const float rstd = rstd_in[row];
-        float c = 0.f;
-#pragma unroll
-        for (int i = 0; i < VPT; ++i) {
-            const int v = lane + 32 * i;
-            if (v < nvec) {
-                float fd[8], fh[8], fw[8];
-                unpack8(dyv[i], fd);
-                unpack8(hv[i], fh);
-                unpack8(wv[i], fw);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const float xh = fh[j] * rstd;
-                    c += fd[j] * fw[j] * xh;
-                    dw[i][j] += fd[j] * xh;
-                }
-            }
-        }
-        c = warp_sum(c) / (float)H;
-#pragma unroll
-        for (int i = 0; i < VPT; ++i) {
-            const int v = lane + 32 * i;
-            if (v < nvec) {
-                float fd[8], fh[8], fw[8], o[8];
-                unpack8(dyv[i], fd);
-                unpack8(hv[i], fh);
-                unpack8(wv[i], fw);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) o[j] = rstd * (fd[j] * fw[j] - fh[j] * rstd * c);
-                if (HAS_EXTRA) {
-                    float fe[8];
-                    unpack8(ev[i], fe);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) o[j] += fe[j];
-                }
-                st_stream(dh + base + 8 * v, pack8(o));
-            }
-        }
-    }
-#pragma unroll
-    for (int i = 0; i < VPT; ++i) {
-        __syncthreads();
-#pragma unroll
-        for (int j = 0; j < 8; ++j) dyn[warp * 256 + lane * 8 + j] = dw[i][j];
-        __syncthreads();
-        const int col = threadIdx.x;               // 256 threads <-> the 256 columns of chunk i
-        float s = 0.f;
-#pragma unroll
-        for (int k = 0; k < kWarpsPerCta; ++k) s += dyn[k * 256 + col];
-        const int gcol = 256 * i + col;
-        if (gcol < H) dw_partial[(size_t)blockIdx.x * H + gcol] = s;
-    }
-}
-
-struct NormGeom {
-    int vpt, tpr, threads;
+// CTA-per-row geometry (H > 1024): the fewest 16-byte vectors per thread (a power of two) that keep the row within
+// kMaxCtaThreads threads, and the thread count (a multiple of 32) that covers the row with them.
+struct CtaGeom {
+    int vpt, threads;
 };
-
-static NormGeom geom(int H) {
+static CtaGeom cta_geom(int H) {
     const int nvec = H / 8;
     int vpt = 1;
-    while ((nvec + vpt - 1) / vpt > 512) vpt *= 2;
-    int tpr = (((nvec + vpt - 1) / vpt) + 31) / 32 * 32;
-    int rows = tpr >= 256 ? 1 : 256 / tpr;
-    return {vpt, tpr, tpr * rows};
+    while ((nvec + vpt - 1) / vpt > kMaxCtaThreads) vpt *= 2;
+    return {vpt, ((nvec + vpt - 1) / vpt + 31) / 32 * 32};
 }
 
-}  // namespace acco
+static bool supported(int H) { return H % 8 == 0 && H > 0 && H <= kMaxH; }
 
-#define ACCO_DISPATCH_WVPT(H, ...)                                    \
-    do {                                                              \
-        const int _v = ((H) / 8 + 31) / 32;                           \
-        if (_v <= 1) { constexpr int VPT = 1; __VA_ARGS__; }          \
-        else if (_v <= 2) { constexpr int VPT = 2; __VA_ARGS__; }     \
-        else if (_v <= 3) { constexpr int VPT = 3; __VA_ARGS__; }     \
-        else if (_v <= 4) { constexpr int VPT = 4; __VA_ARGS__; }     \
-        else { constexpr int VPT = 8; __VA_ARGS__; }                  \
-    } while (0)
-
-#define ACCO_DISPATCH_VPT(vpt, ...)                                  \
-    do {                                                             \
-        if ((vpt) == 1) { constexpr int VPT = 1; __VA_ARGS__; }      \
-        else if ((vpt) == 2) { constexpr int VPT = 2; __VA_ARGS__; } \
-        else if ((vpt) == 4) { constexpr int VPT = 4; __VA_ARGS__; } \
-        else return -1;                                              \
-    } while (0)
-
-// Number of CTAs to launch for T rows of width H on a device with `sms` SMs (also the number of
-// dw partials the backward needs room for).
-extern "C" int acco_norm_grid(int T, int H, int sms, int backward) {
-    if (H <= 1024) {   // warp-per-row kernels: 8 rows per CTA per iteration
-        int want = (T + acco::kWarpsPerCta - 1) / acco::kWarpsPerCta;
-        int cap = sms * (backward ? 2 : 8);
-        if (want < 1) want = 1;
-        return want < cap ? want : cap;
-    }
-    acco::NormGeom g = acco::geom(H);
-    const int rpc = g.threads / g.tpr;
-    int want = (T + rpc - 1) / rpc;
-    // forward: fill the machine; backward: every CTA emits one dw partial, so stay at ~4 CTAs per SM
-    int per_sm = 2048 / g.threads;
-    if (backward && per_sm > 4) per_sm = 4;
-    int cap = sms * per_sm;
-    if (want < 1) want = 1;
-    return want < cap ? want : cap;
-}
-
-// r == nullptr: plain rmsnorm (h is not written).  Returns 0 on success, -1 if H is unsupported.
-extern "C" int acco_rmsnorm_fwd(const void* a, const void* r, const void* w, void* y, void* h, float* rstd, int T, int H,
-                                float eps, int grid, cudaStream_t st) {
-    using namespace acco;
-    if (H % 8 != 0 || H > 8 * 512 * 4) return -1;
-    NormGeom g = geom(H);
+template <int VPT, bool CTA_ROW>
+static void launch_fwd(const void* a, const void* r, const void* w, const void* b, void* y, void* h, float* mean, float* rstd, int T,
+                       int H, float eps, int grid, cudaStream_t st) {
+    const int threads = CTA_ROW ? cta_geom(H).threads : kWarpsPerCta * 32;
     auto A = (const __nv_bfloat16*)a;
     auto R = (const __nv_bfloat16*)r;
     auto W = (const __nv_bfloat16*)w;
+    auto B = (const __nv_bfloat16*)b;
     auto Y = (__nv_bfloat16*)y;
     auto Ho = (__nv_bfloat16*)h;
-    if (H <= 1024) {
-        ACCO_DISPATCH_WVPT(H, {
-            if (r) rmsnorm_fwd_warp_kernel<VPT, true><<<grid, kWarpsPerCta * 32, 0, st>>>(A, R, W, Y, Ho, rstd, T, H, eps);
-            else rmsnorm_fwd_warp_kernel<VPT, false><<<grid, kWarpsPerCta * 32, 0, st>>>(A, R, W, Y, nullptr, rstd, T, H, eps);
-        });
-        return 0;
+    if (b) {
+        if (r) norm_fwd_kernel<VPT, true, CTA_ROW, true><<<grid, threads, 0, st>>>(A, R, W, B, Y, Ho, mean, rstd, T, H, eps);
+        else norm_fwd_kernel<VPT, false, CTA_ROW, true><<<grid, threads, 0, st>>>(A, R, W, B, Y, Ho, mean, rstd, T, H, eps);
+    } else {
+        if (r) norm_fwd_kernel<VPT, true, CTA_ROW, false><<<grid, threads, 0, st>>>(A, R, W, B, Y, Ho, mean, rstd, T, H, eps);
+        else norm_fwd_kernel<VPT, false, CTA_ROW, false><<<grid, threads, 0, st>>>(A, R, W, B, Y, Ho, mean, rstd, T, H, eps);
     }
-    ACCO_DISPATCH_VPT(g.vpt, {
-        if (r) rmsnorm_fwd_kernel<VPT, true><<<grid, g.threads, 0, st>>>(A, R, W, Y, Ho, rstd, T, H, eps, g.tpr);
-        else rmsnorm_fwd_kernel<VPT, false><<<grid, g.threads, 0, st>>>(A, R, W, Y, nullptr, rstd, T, H, eps, g.tpr);
-    });
-    return 0;
 }
 
-// dw_partial must hold grid*H floats; dw_out H floats (ignored when dw_accum_bf16 != nullptr: the
-// reduced dw is then added to that bf16 gradient in place).
-extern "C" int acco_rmsnorm_bwd(const void* dy, const void* dh_extra, const void* h, const void* w, const float* rstd,
-                                void* dh, float* dw_partial, float* dw_out, void* dw_accum_bf16, int T, int H, int grid,
-                                cudaStream_t st) {
-    using namespace acco;
-    if (H % 8 != 0 || H > 8 * 512 * 4) return -1;
-    NormGeom g = geom(H);
+template <int VPT, bool CTA_ROW>
+static void launch_bwd(const void* dy, const void* dh_extra, const void* h, const void* w, const float* mean, const float* rstd, void* dh,
+                       float* partial, int T, int H, int grid, cudaStream_t st) {
+    const int threads = CTA_ROW ? cta_geom(H).threads : kWarpsPerCta * 32;
     auto DY = (const __nv_bfloat16*)dy;
     auto DE = (const __nv_bfloat16*)dh_extra;
     auto Hh = (const __nv_bfloat16*)h;
     auto W = (const __nv_bfloat16*)w;
     auto DH = (__nv_bfloat16*)dh;
-    if (H <= 1024) {
-        const size_t wsmem = (size_t)kWarpsPerCta * 256 * sizeof(float);
-        ACCO_DISPATCH_WVPT(H, {
-            if (dh_extra) rmsnorm_bwd_warp_kernel<VPT, true><<<grid, kWarpsPerCta * 32, wsmem, st>>>(DY, DE, Hh, W, rstd, DH, dw_partial, T, H);
-            else rmsnorm_bwd_warp_kernel<VPT, false><<<grid, kWarpsPerCta * 32, wsmem, st>>>(DY, DE, Hh, W, rstd, DH, dw_partial, T, H);
-        });
-        reduce_partials_kernel<<<(H + 31) / 32, 1024, 0, st>>>(dw_partial, dw_out, (__nv_bfloat16*)dw_accum_bf16, grid, H, H);
-        return 0;
+    const size_t smem = CTA_ROW ? 0 : (size_t)kWarpsPerCta * 256 * sizeof(float);
+    if (mean) {
+        if (dh_extra) norm_bwd_kernel<VPT, true, CTA_ROW, true><<<grid, threads, smem, st>>>(DY, DE, Hh, W, mean, rstd, DH, partial, T, H);
+        else norm_bwd_kernel<VPT, false, CTA_ROW, true><<<grid, threads, smem, st>>>(DY, DE, Hh, W, mean, rstd, DH, partial, T, H);
+    } else {
+        if (dh_extra) norm_bwd_kernel<VPT, true, CTA_ROW, false><<<grid, threads, smem, st>>>(DY, DE, Hh, W, mean, rstd, DH, partial, T, H);
+        else norm_bwd_kernel<VPT, false, CTA_ROW, false><<<grid, threads, smem, st>>>(DY, DE, Hh, W, mean, rstd, DH, partial, T, H);
     }
-    const size_t smem = (size_t)g.threads * 8 * sizeof(float);
-    ACCO_DISPATCH_VPT(g.vpt, {
-        if (dh_extra) rmsnorm_bwd_kernel<VPT, true><<<grid, g.threads, smem, st>>>(DY, DE, Hh, W, rstd, DH, dw_partial, T, H, g.tpr);
-        else rmsnorm_bwd_kernel<VPT, false><<<grid, g.threads, smem, st>>>(DY, DE, Hh, W, rstd, DH, dw_partial, T, H, g.tpr);
-    });
-    reduce_partials_kernel<<<(H + 31) / 32, 1024, 0, st>>>(dw_partial, dw_out, (__nv_bfloat16*)dw_accum_bf16, grid, H, H);
-    return 0;
 }
 
-// out[col] (fp32) = or accum[col] (bf16) += sum_p partial[p * pitch + col], col < width  (shared with layernorm.cu)
-extern "C" int acco_reduce_partials(const float* partial, float* out, void* accum_bf16, int nparts, int width, int pitch, cudaStream_t st) {
-    acco::reduce_partials_kernel<<<(width + 31) / 32, 1024, 0, st>>>(partial, out, (__nv_bfloat16*)accum_bf16, nparts, width, pitch);
+}  // namespace acco
+
+// Runs `launch<VPT, CTA_ROW>(...)` for width H: one warp per row with VPT = ceil(H / 256) for H <= 1024, else one CTA
+// per row with cta_geom(H).vpt.
+#define ACCO_NORM_DISPATCH(H, launch, ...)                                                           \
+    do {                                                                                             \
+        if ((H) <= 1024) {                                                                           \
+            const int _v = ((H) / 8 + 31) / 32;                                                      \
+            if (_v <= 1) launch<1, false>(__VA_ARGS__);                                              \
+            else if (_v == 2) launch<2, false>(__VA_ARGS__);                                         \
+            else if (_v == 3) launch<3, false>(__VA_ARGS__);                                         \
+            else launch<4, false>(__VA_ARGS__);                                                      \
+        } else {                                                                                     \
+            const int _v = acco::cta_geom(H).vpt;                                                    \
+            if (_v == 1) launch<1, true>(__VA_ARGS__);                                               \
+            else if (_v == 2) launch<2, true>(__VA_ARGS__);                                          \
+            else launch<4, true>(__VA_ARGS__);                                                       \
+        }                                                                                            \
+    } while (0)
+
+// Number of CTAs to launch for T rows of width H on a device with `sms` SMs (also the number of dw / db partials the
+// backward needs room for).
+extern "C" int acco_norm_grid(int T, int H, int sms, int backward) {
+    int want, per_sm;
+    if (H <= 1024) {   // warp-per-row: 8 rows per CTA per iteration
+        want = (T + acco::kWarpsPerCta - 1) / acco::kWarpsPerCta;
+        per_sm = backward ? 2 : 8;
+    } else {           // CTA-per-row.  forward: fill the machine; backward: every CTA emits one partial, so stay at 4 CTAs per SM
+        want = T;
+        per_sm = 2048 / acco::cta_geom(H).threads;
+        if (backward && per_sm > 4) per_sm = 4;
+    }
+    const int cap = sms * per_sm;
+    if (want < 1) want = 1;
+    return want < cap ? want : cap;
+}
+
+// RMSNorm when b == nullptr (mean is then not written), LayerNorm otherwise.  r == nullptr: no residual (h is not
+// written).  Returns cudaSuccess, or -1 if H is not supported.
+extern "C" int acco_norm_fwd(const void* a, const void* r, const void* w, const void* b, void* y, void* h, float* mean, float* rstd, int T,
+                             int H, float eps, int grid, cudaStream_t st) {
+    if (!acco::supported(H)) return -1;
+    ACCO_NORM_DISPATCH(H, acco::launch_fwd, a, r, w, b, y, h, mean, rstd, T, H, eps, grid, st);
+    return (int)cudaGetLastError();
+}
+
+// RMSNorm when mean == nullptr, LayerNorm otherwise.  partial: grid * NP * H floats.  dw (| db) are written to fp32
+// `dwdb_out` [NP * H], or, when `dw_accum` is given (and `db_accum` for LayerNorm), added in place to those bf16 gradients.
+extern "C" int acco_norm_bwd(const void* dy, const void* dh_extra, const void* h, const void* w, const float* mean, const float* rstd,
+                             void* dh, float* partial, float* dwdb_out, void* dw_accum, void* db_accum, int T, int H, int grid,
+                             cudaStream_t st) {
+    if (!acco::supported(H)) return -1;
+    ACCO_NORM_DISPATCH(H, acco::launch_bwd, dy, dh_extra, h, w, mean, rstd, dh, partial, T, H, grid, st);
+    const int width = (mean ? 2 : 1) * H;
+    // one reduction over the whole partial row when it lands in fp32, one per parameter when accumulated into the arena
+    if (dw_accum) {
+        acco::reduce_partials(partial, nullptr, dw_accum, grid, H, width, st);
+        if (mean) acco::reduce_partials(partial + H, nullptr, db_accum, grid, H, width, st);
+    } else {
+        acco::reduce_partials(partial, dwdb_out, nullptr, grid, width, width, st);
+    }
     return (int)cudaGetLastError();
 }

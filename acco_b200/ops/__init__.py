@@ -101,11 +101,10 @@ def use_kernels(*tensors: torch.Tensor, bf16_only: bool = True) -> bool:
         f"({_EXT_ERR}). Build it with __graft_entry__.build() or set ACCO_ALLOW_FALLBACK=1.")
 
 
-from .norm import rmsnorm, add_rmsnorm, rmsnorm_ref, add_rmsnorm_ref  # noqa: E402
-from .layernorm import layernorm, add_layernorm, gelu_new, layernorm_ref, add_layernorm_ref, gelu_new_ref  # noqa: E402
+from .norm import rmsnorm, add_rmsnorm, rmsnorm_ref, add_rmsnorm_ref, layernorm, add_layernorm, layernorm_ref, add_layernorm_ref  # noqa: E402
 from .rope import rope_qkv, rope_qkv_ref, apply_rope_ref, rope_tables  # noqa: E402
 from .embedding import embedding  # noqa: E402
-from .swiglu import swiglu, swiglu_ref  # noqa: E402
+from .activation import swiglu, swiglu_ref, gelu_new, gelu_new_ref  # noqa: E402
 from .cross_entropy import softmax_cross_entropy, softmax_cross_entropy_ref  # noqa: E402
 from .linear import linear, LinearFn  # noqa: E402
 from .attention import causal_attention, causal_attention_ref, rope_causal_attention, packed_causal_attention, segment_starts  # noqa: E402

@@ -1,16 +1,21 @@
-"""RMSNorm and fused residual-add + RMSNorm (fp32 statistics, bf16 I/O).
+"""RMSNorm and LayerNorm (weight + bias), each with an optional fused residual add (fp32 statistics, bf16 I/O).
 
-HF Llama computes the norm as ~7 eager kernels with an fp32 round trip
-(`transformers/models/llama/modeling_llama.py:53-70`); here forward is one pass
-(``csrc/norm.cu``) that also emits ``rstd`` for the backward, and the residual add of the
-surrounding block is folded in (``h = a + r; y = norm(h) * w``)."""
+HF Llama computes RMSNorm as ~7 eager kernels with an fp32 round trip
+(`transformers/models/llama/modeling_llama.py:53-70`), and GPT-2 / GPT-Neo run LayerNorm as eager ATen ops
+(`modeling_gpt_neo.py`).  Here each direction is one sm_90a pass (``csrc/norm.cu``, one kernel template for both norms):
+the forward also emits ``rstd`` (and ``mean`` for LayerNorm) for the backward, the residual add of the surrounding block
+is folded in (``h = a + r; y = norm(h)``), and dw / db are reduced deterministically and accumulated straight into the
+gradient arena."""
 from __future__ import annotations
 
 from typing import Tuple
 
 import torch
+import torch.nn.functional as F
 
 from . import count_launch, load_ext, use_kernels
+
+_KERNEL_MAX_H = 16384
 
 
 def rmsnorm_ref(x: torch.Tensor, weight: torch.Tensor, eps: float) -> torch.Tensor:
@@ -24,6 +29,19 @@ def add_rmsnorm_ref(a: torch.Tensor, r: torch.Tensor, weight: torch.Tensor, eps:
     return rmsnorm_ref(h, weight, eps), h
 
 
+def layernorm_ref(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, eps: float) -> torch.Tensor:
+    return F.layer_norm(x.float(), (x.shape[-1],), weight.float(), bias.float(), eps).to(x.dtype)
+
+
+def add_layernorm_ref(a: torch.Tensor, r: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, eps: float) -> Tuple[torch.Tensor, torch.Tensor]:
+    h = (a.float() + r.float()).to(a.dtype)
+    return layernorm_ref(h, weight, bias, eps), h
+
+
+def _kernel_covers(H: int) -> bool:
+    return H % 8 == 0 and H <= _KERNEL_MAX_H
+
+
 def _accum_target(weight):
     """The weight's existing bf16 ``.grad`` (a view of the flat gradient arena) if dw can be
     accumulated into it inside the reduction kernel (fused AccumulateGrad), else None."""
@@ -33,63 +51,73 @@ def _accum_target(weight):
     return None
 
 
-class _RMSNormFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, x, weight, eps):
-        C = load_ext(required=True)
-        x2 = x.reshape(-1, x.shape[-1]).contiguous()
-        y, rstd = C.rmsnorm_fwd(x2, weight, float(eps))
-        count_launch("rmsnorm_fwd")
-        ctx.save_for_backward(x2, weight, rstd)
-        ctx.weight_ref = weight
-        return y.view(x.shape)
+class _NormFn(torch.autograd.Function):
+    """``norm(a (+ r)) * weight (+ bias)``: RMSNorm when ``bias`` is None, LayerNorm otherwise.  With a residual ``r`` it
+    returns ``(y, a + r)``, else ``y``."""
 
     @staticmethod
-    def backward(ctx, dy):
-        C = load_ext(required=True)
-        x2, weight, rstd = ctx.saved_tensors
-        dy2 = dy.reshape(-1, dy.shape[-1]).contiguous()
-        wg = _accum_target(ctx.weight_ref)
-        dx, dw = C.rmsnorm_bwd(dy2, x2, weight, rstd, wg)
-        count_launch("rmsnorm_bwd", 2)
-        return dx.view(dy.shape), (None if wg is not None else dw.to(weight.dtype)), None
-
-
-class _AddRMSNormFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, a, r, weight, eps):
+    def forward(ctx, a, r, weight, bias, eps):
         C = load_ext(required=True)
         shp = a.shape
         a2 = a.reshape(-1, shp[-1]).contiguous()
-        r2 = r.reshape(-1, shp[-1]).contiguous()
-        y, h, rstd = C.add_rmsnorm_fwd(a2, r2, weight, float(eps))
-        count_launch("add_rmsnorm_fwd")
-        ctx.save_for_backward(h, weight, rstd)
-        ctx.weight_ref = weight
+        r2 = None if r is None else r.reshape(-1, shp[-1]).contiguous()
+        y, h, mean, rstd = C.norm_fwd(a2, r2, weight, bias, float(eps))
+        count_launch(("add_" if r is not None else "") + ("layernorm_fwd" if bias is not None else "rmsnorm_fwd"))
+        ctx.save_for_backward(a2 if h is None else h, weight, mean, rstd)
+        ctx.weight_ref, ctx.bias_ref = weight, bias
+        ctx.residual = r is not None
+        if r is None:
+            return y.view(shp)
         return y.view(shp), h.view(shp)
 
     @staticmethod
-    def backward(ctx, dy, dh_extra):
+    def backward(ctx, dy, dh_extra=None):
         C = load_ext(required=True)
-        h, weight, rstd = ctx.saved_tensors
+        h, weight, mean, rstd = ctx.saved_tensors
+        layer = ctx.bias_ref is not None
         shp = dy.shape
         dy2 = dy.reshape(-1, shp[-1]).contiguous()
-        de2 = dh_extra.reshape(-1, shp[-1]).contiguous()
+        de2 = None if dh_extra is None else dh_extra.reshape(-1, shp[-1]).contiguous()
         wg = _accum_target(ctx.weight_ref)
-        dh, dw = C.add_rmsnorm_bwd(dy2, de2, h, weight, rstd, wg)
-        count_launch("add_rmsnorm_bwd", 2)
+        bg = _accum_target(ctx.bias_ref)
+        if layer and (wg is None or bg is None):     # LayerNorm accumulates both parameters or neither
+            wg = bg = None
+        dh, dwdb = C.norm_bwd(dy2, de2, h, weight, mean, rstd, wg, bg)
+        if layer:
+            count_launch("layernorm_bwd", 3 if wg is not None else 2)
+        else:
+            count_launch("add_rmsnorm_bwd" if ctx.residual else "rmsnorm_bwd", 2)
         dh = dh.view(shp)
-        return dh, dh, (None if wg is not None else dw.to(weight.dtype)), None
+        dw = db = None
+        if wg is None:
+            H = shp[-1]
+            dw = dwdb[:H].to(weight.dtype)
+            if layer:
+                db = dwdb[H:].to(weight.dtype)
+        return dh, (dh if ctx.residual else None), dw, db, None
 
 
 def rmsnorm(x: torch.Tensor, weight: torch.Tensor, eps: float = 1e-5) -> torch.Tensor:
-    if use_kernels(x, weight):
-        return _RMSNormFn.apply(x, weight, eps)
+    if use_kernels(x, weight) and _kernel_covers(x.shape[-1]):
+        return _NormFn.apply(x, None, weight, None, eps)
     return rmsnorm_ref(x, weight, eps)
 
 
 def add_rmsnorm(a: torch.Tensor, r: torch.Tensor, weight: torch.Tensor, eps: float = 1e-5):
     """Returns ``(rmsnorm(a + r) * weight, a + r)``."""
-    if use_kernels(a, r, weight):
-        return _AddRMSNormFn.apply(a, r, weight, eps)
+    if use_kernels(a, r, weight) and _kernel_covers(a.shape[-1]):
+        return _NormFn.apply(a, r, weight, None, eps)
     return add_rmsnorm_ref(a, r, weight, eps)
+
+
+def layernorm(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, eps: float = 1e-5) -> torch.Tensor:
+    if use_kernels(x, weight, bias) and _kernel_covers(x.shape[-1]):
+        return _NormFn.apply(x, None, weight, bias, eps)
+    return layernorm_ref(x, weight, bias, eps)
+
+
+def add_layernorm(a: torch.Tensor, r: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, eps: float = 1e-5):
+    """Returns ``(layernorm(a + r), a + r)``."""
+    if use_kernels(a, r, weight, bias) and _kernel_covers(a.shape[-1]):
+        return _NormFn.apply(a, r, weight, bias, eps)
+    return add_layernorm_ref(a, r, weight, bias, eps)

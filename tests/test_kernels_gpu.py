@@ -24,7 +24,7 @@ def test_extension_is_loaded_and_native():
     assert ops.ext_path().endswith("_C.so")
 
 
-@pytest.mark.parametrize("T,H", [(64, 64), (1000, 768), (257, 2048), (33, 4096), (16, 8192)])
+@pytest.mark.parametrize("T,H", [(64, 64), (1000, 768), (257, 2048), (33, 4096), (16, 8192), (8, 12288), (64, 100)])
 def test_rmsnorm_fwd_bwd(T, H):
     x = bf(T, H, seed=1).requires_grad_(True)
     w = (1 + 0.1 * torch.randn(H)).to(DEV, torch.bfloat16).requires_grad_(True)
@@ -432,7 +432,7 @@ def test_tcgen05_tensor_maps_are_cached():
 # ------------------------------------------------------------------------------------------------------------------
 # GPT family kernels
 # ------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("T,H", [(64, 64), (1000, 768), (257, 1024), (100, 2048), (33, 4096)])
+@pytest.mark.parametrize("T,H", [(64, 64), (1000, 768), (257, 1024), (100, 2048), (33, 4096), (16, 8192), (64, 100)])
 @pytest.mark.parametrize("residual", [False, True])
 def test_layernorm_fwd_bwd(T, H, residual):
     a = bf(T, H, seed=1).requires_grad_(True)

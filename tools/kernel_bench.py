@@ -71,14 +71,15 @@ def main():
         res[name] = r
         print(name, json.dumps(r), flush=True)
 
-    x, r_, w = bf(T, H), bf(T, H), torch.ones(H, device=DEV, dtype=torch.bfloat16)
-    y, rstd = C.rmsnorm_fwd(x, w, 1e-5)
-    rec("rmsnorm_fwd", lambda: C.rmsnorm_fwd(x, w, 1e-5), bytes_=2 * T * H * 2)
-    rec("add_rmsnorm_fwd", lambda: C.add_rmsnorm_fwd(x, r_, w, 1e-5), bytes_=4 * T * H * 2)
-    dy = bf(T, H)
-    wg = torch.zeros(H, device=DEV, dtype=torch.bfloat16)
-    rec("rmsnorm_bwd", lambda: C.rmsnorm_bwd(dy, x, w, rstd, wg), bytes_=3 * T * H * 2)
-    rec("add_rmsnorm_bwd", lambda: C.add_rmsnorm_bwd(dy, r_, x, w, rstd, wg), bytes_=4 * T * H * 2)
+    x, r_, w, dy = bf(T, H), bf(T, H), torch.ones(H, device=DEV, dtype=torch.bfloat16), bf(T, H)
+    for kind, b in (("rmsnorm", None), ("layernorm", torch.zeros(H, device=DEV, dtype=torch.bfloat16))):
+        _, _, mean, rstd = C.norm_fwd(x, None, w, b, 1e-5)
+        rec(f"{kind}_fwd", lambda: C.norm_fwd(x, None, w, b, 1e-5), bytes_=2 * T * H * 2)
+        rec(f"add_{kind}_fwd", lambda: C.norm_fwd(x, r_, w, b, 1e-5), bytes_=4 * T * H * 2)
+        wg = torch.zeros(H, device=DEV, dtype=torch.bfloat16)           # parameter gradients accumulated into bf16 .grad
+        bg = None if b is None else torch.zeros_like(wg)
+        rec(f"{kind}_bwd", lambda: C.norm_bwd(dy, None, x, w, mean, rstd, wg, bg), bytes_=3 * T * H * 2)
+        rec(f"add_{kind}_bwd", lambda: C.norm_bwd(dy, r_, x, w, mean, rstd, wg, bg), bytes_=4 * T * H * 2)
     qkv = bf(T, 3 * Hq * D)
     cos, sin = ops.rope_tables(S, D, 10000.0, DEV)
     rec("rope_qkv", lambda: C.rope_qkv_inplace(qkv, cos, sin, B, S, 2 * Hq, 3 * Hq, D, False), bytes_=2 * T * 2 * Hq * D * 2)

@@ -33,6 +33,6 @@ elif which == "ce":
 elif which == "norm":
     x, r, w = bf(T, H), bf(T, H), torch.ones(H, device="cuda", dtype=torch.bfloat16)
     for _ in range(3):
-        y, h, rstd = C.add_rmsnorm_fwd(x, r, w, 1e-5)
-        C.add_rmsnorm_bwd(x, r, h, w, rstd, None)
+        y, h, _, rstd = C.norm_fwd(x, r, w, None, 1e-5)
+        C.norm_bwd(x, r, h, w, None, rstd, None, None)
 torch.cuda.synchronize()
