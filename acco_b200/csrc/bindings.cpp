@@ -38,6 +38,10 @@ long long acco_gemm_map_encodes();
 int acco_gemm_max_clusters(int cl, int sms);
 void acco_gemm_set_debug(unsigned long long* buf);
 void acco_gemm_choose(int M, int N, int K, int a_mn, int b_mn, int accumulate, int sms, int* out5);
+int acco_gemm_fp8_run(const void* a, long long lda, const void* b, long long ldb, void* d, long long ldd, const void* bias, int M, int N, int K,
+                      int accumulate, int a_e5m2, const float* inv_a, const float* inv_b, int bn_req, int splits_req, int sms, cudaStream_t st);
+int acco_fp8_amax_ctas(long long n, int sms);
+int acco_fp8_quantize(const void* t, int R, int C, int e5m2, void* q, void* qT, float* scale_out, int ctas, cudaStream_t st);
 int acco_gemm_tile_n();
 int acco_gemm_tile_k();
 int acco_attn_supported(int B, int S, int Hq, int Hk, int D, float scale);
@@ -443,6 +447,63 @@ torch::Tensor gemm(torch::Tensor a, torch::Tensor b, c10::optional<torch::Tensor
     return y;
 }
 
+// ---------------------------------------------------------------- FP8 (per-tensor current scaling)
+// t [R, C] bf16 -> {q [R, C] or None, qT [C, R] or None, scale fp32 [3 + ctas] = {s, 1/s, amax, per-CTA maxima...}}; e4m3 or (e5m2) e5m2.
+std::vector<torch::Tensor> fp8_quantize(torch::Tensor t, bool e5m2, bool rowmajor, bool transposed) {
+    check_bf16(t, "t");
+    TORCH_CHECK(t.dim() == 2 && t.size(0) % 16 == 0 && t.size(1) % 16 == 0 && t.numel() > 0, "fp8_quantize: t must be [R, C] with R, C multiples of 16");
+    TORCH_CHECK((uintptr_t)t.data_ptr() % 16 == 0, "fp8_quantize: 16-byte aligned input required");
+    const c10::cuda::CUDAGuard guard(t.device());
+    const int64_t R = t.size(0), C = t.size(1);
+    const auto f8 = t.options().dtype(e5m2 ? torch::kFloat8_e5m2 : torch::kFloat8_e4m3fn);
+    torch::Tensor q = rowmajor ? torch::empty({R, C}, f8) : torch::Tensor();
+    torch::Tensor qT = transposed ? torch::empty({C, R}, f8) : torch::Tensor();
+    const int ctas = acco_fp8_amax_ctas(t.numel(), sm_count());
+    auto scale = torch::empty({3 + ctas}, t.options().dtype(torch::kFloat32));
+    TORCH_CHECK(acco_fp8_quantize(t.data_ptr(), (int)R, (int)C, e5m2 ? 1 : 0, rowmajor ? q.data_ptr() : nullptr, transposed ? qT.data_ptr() : nullptr,
+                                  scale.data_ptr<float>(), ctas, stream()) == 0,
+                "fp8_quantize launch failed");
+    return {q, qT, scale};
+}
+
+// out[M,N] (+)= a[M,K] * b[N,K]^T / (s_a s_b) (+ bias).  a: e4m3 or e5m2, b: e4m3, both K-major with 16-byte aligned rows; scale_a / scale_b:
+// the scale tensors of fp8_quantize (1/s read on the device).  accumulate: out += (bf16 reduce-add epilogue, split-K allowed).
+torch::Tensor gemm_fp8(torch::Tensor a, torch::Tensor b, torch::Tensor scale_a, torch::Tensor scale_b, c10::optional<torch::Tensor> out,
+                       c10::optional<torch::Tensor> bias, bool accumulate, int64_t bn, int64_t splits) {
+    auto ok2d = [](const torch::Tensor& t) {
+        return t.is_cuda() && t.dim() == 2 && t.stride(1) == 1 && t.stride(0) % 16 == 0 && t.stride(0) >= t.size(1) && (uintptr_t)t.data_ptr() % 16 == 0;
+    };
+    TORCH_CHECK(ok2d(a) && ok2d(b), "gemm_fp8: operands must be 2-D CUDA, unit inner stride, 16-byte aligned rows");
+    TORCH_CHECK(a.scalar_type() == torch::kFloat8_e4m3fn || a.scalar_type() == torch::kFloat8_e5m2, "gemm_fp8: a must be e4m3 or e5m2");
+    TORCH_CHECK(b.scalar_type() == torch::kFloat8_e4m3fn, "gemm_fp8: b must be e4m3");
+    check_f32(scale_a, "scale_a"); check_f32(scale_b, "scale_b");
+    TORCH_CHECK(scale_a.numel() >= 2 && scale_b.numel() >= 2, "gemm_fp8: scales must be {s, 1/s, ...}");
+    const c10::cuda::CUDAGuard guard(a.device());
+    const int64_t M = a.size(0), K = a.size(1), N = b.size(0);
+    TORCH_CHECK(b.size(1) == K, "gemm_fp8: contraction sizes differ (", K, " vs ", b.size(1), ")");
+    TORCH_CHECK(K % 16 == 0 && N % 8 == 0, "gemm_fp8: K must be a multiple of 16 and N of 8");
+    torch::Tensor y;
+    if (out.has_value() && out->defined()) {
+        y = *out;
+        TORCH_CHECK(y.is_cuda() && y.scalar_type() == torch::kBFloat16 && y.dim() == 2 && y.size(0) == M && y.size(1) == N && y.stride(1) == 1 &&
+                    y.stride(0) % 8 == 0 && (uintptr_t)y.data_ptr() % 16 == 0, "gemm_fp8: out must be a [M,N] CUDA bf16 matrix with 16-byte aligned rows");
+    } else {
+        TORCH_CHECK(!accumulate, "gemm_fp8: accumulate needs `out`");
+        y = torch::empty({M, N}, a.options().dtype(torch::kBFloat16));
+    }
+    const void* bias_p = nullptr;
+    if (bias.has_value() && bias->defined()) {
+        TORCH_CHECK(bias->is_cuda() && bias->scalar_type() == torch::kBFloat16 && bias->is_contiguous() && bias->numel() == N &&
+                    (uintptr_t)bias->data_ptr() % 16 == 0, "gemm_fp8: bias must be a contiguous, 16-byte aligned CUDA bf16 [N] vector");
+        bias_p = bias->data_ptr();
+    }
+    const int rc = acco_gemm_fp8_run(a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), y.data_ptr(), y.stride(0), bias_p, (int)M, (int)N, (int)K,
+                                     accumulate ? 1 : 0, a.scalar_type() == torch::kFloat8_e5m2 ? 1 : 0, scale_a.data_ptr<float>() + 1,
+                                     scale_b.data_ptr<float>() + 1, (int)bn, (int)splits, sm_count(), stream());
+    TORCH_CHECK(rc == 0, "gemm_fp8 launch failed, code ", rc, " (M=", M, " N=", N, " K=", K, ")");
+    return y;
+}
+
 // heuristic's pick for a shape: {bn, splits, pm, pn, rows per CTA / 128}
 std::vector<int64_t> gemm_choose(int64_t M, int64_t N, int64_t K, bool a_mn, bool b_mn, bool accumulate) {
     int o[5] = {0, 0, 0, 0, 0};
@@ -554,6 +615,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("gemm_tn", &gemm_tn);
     m.def("gemm", &gemm);
     m.def("gemm_choose", &gemm_choose);
+    m.def("fp8_quantize", &fp8_quantize);
+    m.def("gemm_fp8", &gemm_fp8);
     m.def("gemm_map_encodes", &gemm_map_encodes);
     m.def("gemm_max_clusters", &gemm_max_clusters);
     m.def("gemm_set_debug", &gemm_set_debug);

@@ -84,7 +84,14 @@ struct Params {
     int pm, pn;                        // cluster = pm x pn CTAs: the pn CTAs of a row share A, the pm CTAs of a column share B
     int band;                          // tile order: bands of `band` super-tile columns (decode_unit)
     unsigned long long* dbg;          // optional: CTA 0 writes %globaltimer stamps of its phases (tools/gemm_timeline.py)
+    const float* inv_scale_a;          // FP8: 1 / s of each operand (device memory, written by the quantiser); unused in bf16
+    const float* inv_scale_b;
 };
+
+// Operand format of an instantiation.  FP8 (both operands K-major, B e4m3): a k-block is 128 one-byte k, so rows stay 128 B and
+// the swizzle, stage bytes and ring geometry are those of bf16.  Each k-block accumulates into a fresh fp32 fragment that is then
+// added to the tile's sum in registers ("promotion": the FP8 tensor-core accumulator keeps fewer bits than fp32).
+constexpr int OP_BF16 = 0, OP_E4M3 = 1, OP_E5M2 = 2;    // A operand e4m3 (forward) / e5m2 (gradients)
 
 __device__ __forceinline__ void wait_flag_gpu(const uint32_t* f, uint32_t epoch) {
     uint32_t v;
@@ -143,8 +150,17 @@ __device__ __forceinline__ void mma_k16(float (&acc)[BN / 2], uint64_t da, uint6
     else wgmma_m64n64k16<TA, TB>(acc, da, db, scale_d);
 }
 
-template <int BN, int A_MN, int B_MN>
-__global__ void __launch_bounds__(THREADS, 1) gemm_kernel(const __grid_constant__ Params P) {
+template <int BN, int OP>
+__device__ __forceinline__ void mma_k32(float (&acc)[BN / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
+    static_assert(BN <= 128, "FP8 tiles: the promoted fragment doubles the accumulator registers");
+    if constexpr (BN == 128) wgmma_m64n128k32_f8<OP == OP_E5M2>(acc, da, db, scale_d);
+    else wgmma_m64n64k32_f8<OP == OP_E5M2>(acc, da, db, scale_d);
+}
+
+template <int BN, int A_MN, int B_MN, int OP>
+__device__ __forceinline__ void gemm_body(const Params& P) {
+    static_assert(OP == OP_BF16 || (A_MN == 0 && B_MN == 0), "FP8 wgmma has no transpose: both operands K-major");
+    constexpr int BKE = OP ? 2 * BK : BK;                  // elements per k-block (128 bytes per row in both formats)
     extern __shared__ uint8_t smem_raw[];
     if (threadIdx.x == 0) stamp(P, 0);
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);   // SWIZZLE_128B needs 1024 B alignment
@@ -160,7 +176,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_kernel(const __grid_constant_
     const uint32_t cl_rank = cl_size > 1 ? cluster_ctarank() : 0u;
     const int pi = (int)cl_rank / pn, pj = (int)cl_rank - pi * pn;
     const int unit0 = blockIdx.x / cl_size, unit_stride = gridDim.x / cl_size;
-    const int num_n = (P.N + BN - 1) / BN, num_k = (P.K + BK - 1) / BK, num_mb = (P.M + BM - 1) / BM;
+    const int num_n = (P.N + BN - 1) / BN, num_k = (P.K + BKE - 1) / BKE, num_mb = (P.M + BM - 1) / BM;
     const int num_sn = (num_n + pn - 1) / pn, num_smb = (num_mb + pm - 1) / pm;
     const int band = P.band;
     const int tiles = num_smb * num_sn;
@@ -237,27 +253,27 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_kernel(const __grid_constant_
                     mbar_expect_tx(&full_bar[stage], (uint32_t)(A_BYTES + B_BYTES));   // everything landing in MY stage
                     if (A_MN) {
                         for (int c = a_ch0; c < a_ch0 + nach; ++c) {
-                            if (mc_a) tma_load_2d_mc(&P.map_a, &full_bar[stage], sa + c * MN_CHUNK_BYTES, m0 + c * 64, kb * BK, mask_a);
-                            else tma_load_2d(&P.map_a, &full_bar[stage], sa + c * MN_CHUNK_BYTES, m0 + c * 64, kb * BK);
+                            if (mc_a) tma_load_2d_mc(&P.map_a, &full_bar[stage], sa + c * MN_CHUNK_BYTES, m0 + c * 64, kb * BKE, mask_a);
+                            else tma_load_2d(&P.map_a, &full_bar[stage], sa + c * MN_CHUNK_BYTES, m0 + c * 64, kb * BKE);
                         }
                     } else {
-                        if (mc_a) tma_load_2d_mc(&P.map_a, &full_bar[stage], sa + a_off * 128, kb * BK, m0 + a_off, mask_a);
-                        else tma_load_2d(&P.map_a, &full_bar[stage], sa, kb * BK, m0);
+                        if (mc_a) tma_load_2d_mc(&P.map_a, &full_bar[stage], sa + a_off * 128, kb * BKE, m0 + a_off, mask_a);
+                        else tma_load_2d(&P.map_a, &full_bar[stage], sa, kb * BKE, m0);
                     }
                     if (B_MN) {
                         for (int c = b_ch0; c < b_ch0 + nbch; ++c) {
-                            if (mc_b) tma_load_2d_mc(bmap, &full_bar[stage], sb + c * MN_CHUNK_BYTES, n0 + c * 64, kb * BK, mask_b);
-                            else tma_load_2d(bmap, &full_bar[stage], sb + c * MN_CHUNK_BYTES, n0 + c * 64, kb * BK);
+                            if (mc_b) tma_load_2d_mc(bmap, &full_bar[stage], sb + c * MN_CHUNK_BYTES, n0 + c * 64, kb * BKE, mask_b);
+                            else tma_load_2d(bmap, &full_bar[stage], sb + c * MN_CHUNK_BYTES, n0 + c * 64, kb * BKE);
                         }
                     } else {
-                        if (mc_b) tma_load_2d_mc(bmap, &full_bar[stage], sb + b_off * 128, kb * BK, n0 + b_off, mask_b);
-                        else tma_load_2d(bmap, &full_bar[stage], sb, kb * BK, n0);
+                        if (mc_b) tma_load_2d_mc(bmap, &full_bar[stage], sb + b_off * 128, kb * BKE, n0 + b_off, mask_b);
+                        else tma_load_2d(bmap, &full_bar[stage], sb, kb * BKE, n0);
                     }
                     if (gatherer) {
                         // write the pulled tile through to the local copy of W, then publish it (both halves of the 256-row tile)
                         mbar_wait(&full_bar[stage], phase);
                         fence_async_smem();
-                        tma_store_2d(&P.map_b, sb, kb * BK, n0);
+                        tma_store_2d(&P.map_b, sb, kb * BKE, n0);
                         asm volatile("cp.async.bulk.commit_group;" ::: "memory");
                         asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");       // writes complete (not just smem read)
                         asm volatile("fence.proxy.async;" ::: "memory");
@@ -305,22 +321,38 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_kernel(const __grid_constant_
         float acc[BN / 2];
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        float part[OP ? BN / 2 : 1];                       // FP8: the current k-block's fragment
+        float out_scale = 1.f;
+        if constexpr (OP != OP_BF16) out_scale = P.inv_scale_a[0] * P.inv_scale_b[0];   // powers of two: exact
         int stage = 0;
         uint32_t phase = 0;
         for (int t = unit0; t < num_units; t += unit_stride) {
             const Unit u = decode_unit(t, tiles, num_smb, num_sn, band, num_k, kbs, pm, pn, pi, pj);
             int prev = -1;
+            if constexpr (OP != OP_BF16) {
+#pragma unroll
+                for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+            }
             for (int kb = u.kb0; kb < u.kb1; ++kb) {
                 mbar_wait(&full_bar[stage], phase);
                 if (cw == 0 && tid == 0 && t == unit0 && kb == u.kb0) stamp(P, 4);
                 const uint32_t a_addr = smem_u32(smem + stage * stage_bytes) + (uint32_t)(cw * 8192);
                 const uint32_t b_addr = smem_u32(smem + stage * stage_bytes + A_BYTES);
                 wgmma_fence();
+                if constexpr (OP != OP_BF16) {
 #pragma unroll
-                for (int k = 0; k < BK / 16; ++k) {
-                    const uint64_t da = make_smem_desc(a_addr + k * a_kstep, a_lbo, a_sbo);
-                    const uint64_t db = make_smem_desc(b_addr + k * b_kstep, b_lbo, b_sbo);
-                    mma_k16<BN, A_MN, B_MN>(acc, da, db, (uint32_t)((kb > u.kb0) | (k != 0)));
+                    for (int k = 0; k < BKE / 32; ++k) {
+                        const uint64_t da = make_smem_desc(a_addr + k * 32, 1, 1024 >> 4);
+                        const uint64_t db = make_smem_desc(b_addr + k * 32, 1, 1024 >> 4);
+                        mma_k32<BN, OP>(part, da, db, (uint32_t)(k != 0));
+                    }
+                } else {
+#pragma unroll
+                    for (int k = 0; k < BK / 16; ++k) {
+                        const uint64_t da = make_smem_desc(a_addr + k * a_kstep, a_lbo, a_sbo);
+                        const uint64_t db = make_smem_desc(b_addr + k * b_kstep, b_lbo, b_sbo);
+                        mma_k16<BN, A_MN, B_MN>(acc, da, db, (uint32_t)((kb > u.kb0) | (k != 0)));
+                    }
                 }
                 wgmma_commit();
                 if (load_c && kb == u.kb0 && tid == 0) {
@@ -328,16 +360,28 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_kernel(const __grid_constant_
                     bulk_wait_read<0>();
                     for (int s = 0; s < NPRE; ++s) load_c_sub(u, s);
                 }
-                if (prev >= 0) {
-                    wgmma_wait<1>();                   // the previous stage's wgmmas have retired: hand it back
-                    release(prev);
+                if constexpr (OP != OP_BF16) {
+                    // promotion: the k-block's fragment is complete, add it to the tile's fp32 sum (the other consumer
+                    // warpgroup's wgmmas keep the tensor cores busy meanwhile)
+                    wgmma_wait<0>();
+                    reg_fence(part);
+                    release(stage);
+#pragma unroll
+                    for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+                } else {
+                    if (prev >= 0) {
+                        wgmma_wait<1>();                   // the previous stage's wgmmas have retired: hand it back
+                        release(prev);
+                    }
+                    prev = stage;
                 }
-                prev = stage;
                 if (++stage == n_stages) { stage = 0; phase ^= 1; }
             }
-            wgmma_wait<0>();
-            reg_fence(acc);
-            release(prev);
+            if constexpr (OP == OP_BF16) {
+                wgmma_wait<0>();
+                reg_fence(acc);
+                release(prev);
+            }
             // ---------------- epilogue: fragment (row 16 warp + lane/4 (+8), columns 8 j + 2 (lane % 4) (+1)) -> staging -> TMA
             const int m0 = u.mb * BM + cw * 64;
             // my rows r = 16 warp + lane / 4 (+8) of the 64-row half; r % 8 = lane / 4 sets the swizzle of both
@@ -372,7 +416,14 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_kernel(const __grid_constant_
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
                         const uint32_t dst = chunk_addr + h * 8 * 128;
-                        float v0 = acc[4 * j + 2 * h] + b0, v1 = acc[4 * j + 2 * h + 1] + b1;
+                        float v0, v1;
+                        if constexpr (OP != OP_BF16) {
+                            v0 = acc[4 * j + 2 * h] * out_scale + b0;
+                            v1 = acc[4 * j + 2 * h + 1] * out_scale + b1;
+                        } else {
+                            v0 = acc[4 * j + 2 * h] + b0;
+                            v1 = acc[4 * j + 2 * h + 1] + b1;
+                        }
                         if (load_c) {
                             // beta = 1 with a single K split: exact fp32 accumulate (one rounding), nobody else touches this tile
                             const uint32_t cv = ld_shared_u32(dst);
@@ -409,6 +460,17 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_kernel(const __grid_constant_
             *P.epoch = epoch;
         }
     }
+}
+
+template <int BN, int A_MN, int B_MN>
+__global__ void __launch_bounds__(THREADS, 1) gemm_kernel(const __grid_constant__ Params P) {
+    gemm_body<BN, A_MN, B_MN, OP_BF16>(P);
+}
+
+// FP8 (OP = OP_E4M3 / OP_E5M2): D = A * B^T / (s_a s_b) (+ bias), both operands K-major one-byte [rows, K]; BN 64 or 128
+template <int BN, int OP>
+__global__ void __launch_bounds__(THREADS, 1) gemm_fp8_kernel(const __grid_constant__ Params P) {
+    gemm_body<BN, 0, 0, OP>(P);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -469,7 +531,7 @@ static std::mutex g_map_mu;
 static std::unordered_map<MapKey, CUtensorMap, MapKeyHash> g_maps;
 static long long g_map_encodes = 0;
 
-// row-major matrix (bf16: elem_bytes 2, fp32: 4) with `outer` rows of `inner` contiguous elements (row stride `ld` elements),
+// row-major matrix (fp8: elem_bytes 1, bf16: 2, fp32: 4) with `outer` rows of `inner` contiguous elements (row stride `ld` elements),
 // box {box_inner, box_outer}, 128-byte swizzle (box_inner * elem_bytes = 128 B)
 int make_map_typed(CUtensorMap* m, const void* base, uint64_t inner, uint64_t outer, uint64_t ld, uint32_t box_inner, uint32_t box_outer,
                    int elem_bytes) {
@@ -485,10 +547,12 @@ int make_map_typed(CUtensorMap* m, const void* base, uint64_t inner, uint64_t ou
     cuuint64_t strides[1] = {ld * (uint64_t)elem_bytes};
     cuuint32_t box[2] = {box_inner, box_outer};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(m, elem_bytes == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    const CUtensorMapDataType dt = elem_bytes == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                   : elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+    CUresult r = enc(m, dt, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r == CUDA_ERROR_INVALID_CONTEXT && bind_primary_context()) {
-        r = enc(m, elem_bytes == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
+        r = enc(m, dt, 2, const_cast<void*>(base), dims, strides, box, estr,
                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     }
     if (r != CUDA_SUCCESS) return -3;
@@ -514,6 +578,11 @@ static KernelFn kernel_for(int bn, int a_mn, int b_mn) {
     if (bn == 128) return kernel_for<128>(a_mn, b_mn);
     return kernel_for<64>(a_mn, b_mn);
 }
+// FP8 instantiations: BN in {64, 128} x A format (e4m3 forward, e5m2 gradients)
+static KernelFn fp8_kernel_for(int bn, int op) {
+    if (bn == 128) return op == OP_E5M2 ? gemm_fp8_kernel<128, OP_E5M2> : gemm_fp8_kernel<128, OP_E4M3>;
+    return op == OP_E5M2 ? gemm_fp8_kernel<64, OP_E5M2> : gemm_fp8_kernel<64, OP_E4M3>;
+}
 
 static int g_pm = 0, g_pn = 0;                     // ACCO_GEMM_CLUSTER="pm,pn": force the cluster shape (0 = heuristic)
 static unsigned long long* g_dbg = nullptr;        // device buffer for phase time stamps (acco_gemm_set_debug)
@@ -526,6 +595,9 @@ static int init_once() {
             for (int a = 0; a < 2; ++a)
                 for (int b = 0; b < 2; ++b)
                     if (cudaFuncSetAttribute(kernel_for(bn, a, b), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) rc = -4;
+        for (int bn : {64, 128})
+            for (int op : {OP_E4M3, OP_E5M2})
+                if (cudaFuncSetAttribute(fp8_kernel_for(bn, op), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) rc = -4;
         const char* e;
         if ((e = getenv("ACCO_GEMM_CLUSTER")) && e[0] && e[1] == ',') { g_pm = e[0] - '0'; g_pn = e[2] - '0'; }
         if ((e = getenv("ACCO_GEMM_PDL")) && e[0] == '0') g_pdl = 0;
@@ -568,17 +640,20 @@ struct Config {
 // (128 x bn x 64 multiply-adds at 2048 per clock on an H100 SM) and the operand bytes must come in through L2 (~64 B/clk/SM
 // assumed); `epi` charges the epilogue as if it were not overlapped (its TMA stores now drain while the next tile's mainloop runs,
 // so this over-estimates it; the picks are kept as they are).  Split-K needs an adding epilogue: accumulating GEMMs
-// (wgrad), or a zero-filled output.
-static Config choose_config(int M, int N, int K, int a_mn, int b_mn, int reduce, int sms, int bn_req, int splits_req, int pm_req, int pn_req) {
+// (wgrad), or a zero-filled output.  FP8 passes K / 2: its 128-deep k-block moves the bytes of a bf16 one and takes the same tensor-core
+// time (twice the rate), and caps the tile at bn_max = 128.
+static Config choose_config(int M, int N, int K, int a_mn, int b_mn, int reduce, int sms, int bn_req, int splits_req, int pm_req, int pn_req,
+                            int bn_max = BN_MAX) {
     (void)a_mn; (void)b_mn;
     const int num_k = (K + BK - 1) / BK;
     double best = 1e30;
-    Config bc{256, 1, 1, 1};
+    Config bc{bn_max, 1, 1, 1};
     const int cands[3] = {256, 128, 64};
     const int num_mb = (M + BM - 1) / BM;
     for (int ci = 0; ci < 3; ++ci) {
         const int bn = cands[ci];
         if (bn_req > 0 && bn != bn_req) continue;
+        if (bn > bn_max) continue;
         if (bn_req <= 0 && bn > 64 && bn / 2 >= N) continue;                  // a narrower tile already covers N
         const int num_n = (N + bn - 1) / bn;
         for (int pm = 1; pm <= 2; ++pm) {
@@ -650,9 +725,11 @@ struct GatherArgs {
 
 static int launch(const void* a, long long lda, int a_mn, const void* b, long long ldb, int b_mn, void* d, long long ldd, const void* bias, int M,
                   int N, int K, int accumulate, int bn_req, int splits_req, int pm_req, int pn_req, int msub_req, const GatherArgs* ga, int sms,
-                  cudaStream_t st) {
+                  cudaStream_t st, int op = OP_BF16, const float* inv_a = nullptr, const float* inv_b = nullptr) {
     if (M <= 0 || N <= 0 || K <= 0) return -1;
     if ((lda % 8) || (ldb % 8) || (ldd % 8) || (N % 8)) return -1;
+    const int eb = op ? 1 : 2, bke = op ? 2 * BK : BK;                     // operand bytes per element, elements per k-block
+    if (op && (a_mn || b_mn || (lda % 16) || (ldb % 16) || (K % 16) || bn_req > 128 || !inv_a || !inv_b || (ga && ga->n_peers > 0))) return -1;
     if (((uintptr_t)a % 16) || ((uintptr_t)b % 16) || ((uintptr_t)d % 16) || (bias && ((uintptr_t)bias % 16))) return -1;
     if (msub_req > 1) return -1;                                           // one 128-row tile per CTA
     int rc = init_once();
@@ -665,7 +742,7 @@ static int launch(const void* a, long long lda, int a_mn, const void* b, long lo
     if (!gather) {
         if (g_pm > 0 && pm_req <= 0) pm_req = g_pm;
         if (g_pn > 0 && pn_req <= 0) pn_req = g_pn;
-        cfgc = choose_config(M, N, K, a_mn, b_mn, accumulate, sms, bn_req, splits_req, pm_req, pn_req);
+        cfgc = choose_config(M, N, op ? (K + 1) / 2 : K, a_mn, b_mn, accumulate, sms, bn_req, splits_req, pm_req, pn_req, op ? 128 : BN_MAX);
     }
     const int bn = cfgc.bn, pm = cfgc.pm, pn = cfgc.pn;
     int splits = cfgc.splits;
@@ -674,10 +751,10 @@ static int launch(const void* a, long long lda, int a_mn, const void* b, long lo
     if (a_mn && (BM / 64) % pn != 0) return -1;
     Params P;
     if (a_mn) rc = make_map(&P.map_a, a, (uint64_t)M, (uint64_t)K, (uint64_t)lda, 64, BK);
-    else rc = make_map(&P.map_a, a, (uint64_t)K, (uint64_t)M, (uint64_t)lda, BK, (uint32_t)(BM / pn));
+    else rc = make_map_typed(&P.map_a, a, (uint64_t)K, (uint64_t)M, (uint64_t)lda, bke, (uint32_t)(BM / pn), eb);
     if (rc) return rc;
     if (b_mn) rc = make_map(&P.map_b, b, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, 64, BK);
-    else rc = make_map(&P.map_b, b, (uint64_t)K, (uint64_t)N, (uint64_t)ldb, BK, (uint32_t)(bn / pm));
+    else rc = make_map_typed(&P.map_b, b, (uint64_t)K, (uint64_t)N, (uint64_t)ldb, bke, (uint32_t)(bn / pm), eb);
     if (rc) return rc;
     for (int i = 0; i < MAX_PEERS; ++i) {
         if (gather && i < ga->n_peers) {
@@ -694,12 +771,14 @@ static int launch(const void* a, long long lda, int a_mn, const void* b, long lo
     P.out = (__nv_bfloat16*)d;
     P.ldd = ldd;
     P.dbg = g_dbg;
+    P.inv_scale_a = inv_a;
+    P.inv_scale_b = inv_b;
     P.tile_owner = gather ? ga->tile_owner : nullptr;
     P.flags = gather ? ga->flags : nullptr;
     P.epoch = gather ? ga->epoch : nullptr;
     P.done_ctas = gather ? ga->done : nullptr;
     P.M = M; P.N = N; P.K = K;
-    const int num_k = (K + BK - 1) / BK;
+    const int num_k = (K + bke - 1) / bke;
     if (splits < 1) splits = 1;
     if (splits > num_k) splits = num_k;
     P.kb_per_split = (num_k + splits - 1) / splits;
@@ -725,7 +804,7 @@ static int launch(const void* a, long long lda, int a_mn, const void* b, long lo
     const long long units = (long long)((num_mb + pm - 1) / pm) * num_sn * P.splits;
     const int slots = cl > 1 ? max_clusters(cl, sms) : sms;
     if (slots <= 0) return -5;
-    P.band = gather ? num_sn : tile_band(M, K, bn * pn, num_sn);
+    P.band = gather ? num_sn : tile_band(M, op ? (K + 1) / 2 : K, bn * pn, num_sn);
     const int grid = (int)(units < (long long)slots ? units : (long long)slots) * cl;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid);
@@ -748,7 +827,7 @@ static int launch(const void* a, long long lda, int a_mn, const void* b, long lo
     }
     cfg.attrs = attr;
     cfg.numAttrs = na;
-    return (int)cudaLaunchKernelEx(&cfg, kernel_for(bn, a_mn, b_mn), P);
+    return (int)cudaLaunchKernelEx(&cfg, op ? fp8_kernel_for(bn, op) : kernel_for(bn, a_mn, b_mn), P);
 }
 
 }  // namespace acco_gemm
@@ -769,6 +848,15 @@ extern "C" int acco_gemm_tn_gather(const void* x, const void* w_local, void* y, 
                                    const int* tile_owner, uint32_t* flags, uint32_t* epoch, uint32_t* done, int sms, cudaStream_t st) {
     acco_gemm::GatherArgs ga{peers, n_peers, tile_owner, flags, epoch, done};
     return acco_gemm::launch(x, K, 0, w_local, K, 0, y, N, nullptr, M, N, K, 0, 0, 0, 0, 0, 0, n_peers > 0 ? &ga : nullptr, sms, st);
+}
+
+// FP8: D[M,N] (+)= A[M,K] * B[N,K]^T * (inv_a[0] * inv_b[0]) (+ bias).  a, b: one-byte K-major operands (row strides lda, ldb
+// bytes, multiples of 16; K % 16 == 0); a_e5m2: A is e5m2 (gradients), else e4m3; B is e4m3.  inv_a / inv_b: device pointers to 1/s.
+extern "C" int acco_gemm_fp8_run(const void* a, long long lda, const void* b, long long ldb, void* d, long long ldd, const void* bias, int M, int N,
+                                 int K, int accumulate, int a_e5m2, const float* inv_a, const float* inv_b, int bn_req, int splits_req, int sms,
+                                 cudaStream_t st) {
+    return acco_gemm::launch(a, lda, 0, b, ldb, 0, d, ldd, bias, M, N, K, accumulate, bn_req, splits_req, 0, 0, 0, nullptr, sms, st,
+                             a_e5m2 ? acco_gemm::OP_E5M2 : acco_gemm::OP_E4M3, inv_a, inv_b);
 }
 
 extern "C" int acco_gemm_tile_n() { return acco_gemm::BN_MAX; }

@@ -155,6 +155,7 @@ class GPTForCausalLM(nn.Module):
         self.config = config
         self.transformer = _Transformer(config)
         self.lm_head = None if config.tie_word_embeddings else nn.Parameter(torch.empty(config.padded_vocab, config.hidden_size))
+        self.fp8 = False         # FP8 GEMMs for the block linears of training micro-batches (train key `fp8`, ops/fp8.py)
         self.reset_parameters()
 
     @torch.no_grad()
@@ -194,6 +195,7 @@ class GPTForCausalLM(nn.Module):
         T = B * S
         Hh, D, H = cfg.num_attention_heads, cfg.head_dim, cfg.hidden_size
         eps = cfg.layer_norm_epsilon
+        fp8 = self.fp8
         tr = self.transformer
         scale = (1.0 / math.sqrt(D)) if cfg.scale_attn else 1.0
         seg = None
@@ -209,13 +211,13 @@ class GPTForCausalLM(nn.Module):
                 n = ops.layernorm(h, blk.ln_1.weight, blk.ln_1.bias, eps)
             else:
                 n, h = ops.add_layernorm(branch, h, blk.ln_1.weight, blk.ln_1.bias, eps)
-            qkv = ops.linear(n, a.qkv_proj)                                                       # [T, 3H]
+            qkv = ops.linear(n, a.qkv_proj, fp8=fp8)                                                       # [T, 3H]
             att = ops.packed_causal_attention(qkv, B, S, Hh, Hh, D, scale=scale,
                                               window=cfg.window_size if blk.kind == "local" else None, seg=seg)   # [T, H]
-            o = ops.linear(att, a.out_proj.weight, a.out_proj.bias)
+            o = ops.linear(att, a.out_proj.weight, a.out_proj.bias, fp8=fp8)
             n, h = ops.add_layernorm(o, h, blk.ln_2.weight, blk.ln_2.bias, eps)
-            f = ops.linear(n, blk.mlp.c_fc.weight, blk.mlp.c_fc.bias)
-            branch = ops.linear(ops.gelu_new(f), blk.mlp.c_proj.weight, blk.mlp.c_proj.bias)
+            f = ops.linear(n, blk.mlp.c_fc.weight, blk.mlp.c_fc.bias, fp8=fp8)
+            branch = ops.linear(ops.gelu_new(f), blk.mlp.c_proj.weight, blk.mlp.c_proj.bias, fp8=fp8)
         if branch is None:
             n = ops.layernorm(h, tr.ln_f.weight, tr.ln_f.bias, eps)
         else:

@@ -140,6 +140,7 @@ class LlamaForCausalLM(nn.Module):
         self._ag_table: Dict[int, Any] = {}
         self._ag_idx = 0
         self._ag_pending = False
+        self.fp8 = False         # FP8 GEMMs for the block linears of training micro-batches (train key `fp8`, ops/fp8.py)
         self.reset_parameters()
 
     # ------------------------------------------------------------------ init
@@ -204,6 +205,7 @@ class LlamaForCausalLM(nn.Module):
             cos, sin = cos[pos], sin[pos]                                                   # per-token tables [T, D/2]
             seg = ops.segment_starts(position_ids)
         eps = cfg.rms_norm_eps
+        fp8 = self.fp8
 
         h = ops.embedding(input_ids.reshape(T), self.model.embed_tokens)                   # [T, H]
         branch = None          # output of the previous residual branch, not yet added to h
@@ -212,12 +214,12 @@ class LlamaForCausalLM(nn.Module):
                 n = ops.rmsnorm(h, layer.input_layernorm.weight, eps)
             else:
                 n, h = ops.add_rmsnorm(branch, h, layer.input_layernorm.weight, eps)
-            qkv = ops.linear(n, layer.self_attn.qkv_proj, gathered=self._gw(layer.self_attn.qkv_proj))   # [T, (Hq+2Hk)D]
+            qkv = ops.linear(n, layer.self_attn.qkv_proj, gathered=self._gw(layer.self_attn.qkv_proj), fp8=fp8)   # [T, (Hq+2Hk)D]
             att = ops.rope_causal_attention(qkv, cos, sin, B, S, Hq, Hk, D, seg=seg)       # [T, Hq*D]
-            o = ops.linear(att, layer.self_attn.o_proj, gathered=self._gw(layer.self_attn.o_proj))
+            o = ops.linear(att, layer.self_attn.o_proj, gathered=self._gw(layer.self_attn.o_proj), fp8=fp8)
             n, h = ops.add_rmsnorm(o, h, layer.post_attention_layernorm.weight, eps)
-            gu = ops.linear(n, layer.mlp.gate_up_proj, gathered=self._gw(layer.mlp.gate_up_proj))
-            branch = ops.linear(ops.swiglu(gu), layer.mlp.down_proj, gathered=self._gw(layer.mlp.down_proj))
+            gu = ops.linear(n, layer.mlp.gate_up_proj, gathered=self._gw(layer.mlp.gate_up_proj), fp8=fp8)
+            branch = ops.linear(ops.swiglu(gu), layer.mlp.down_proj, gathered=self._gw(layer.mlp.down_proj), fp8=fp8)
         if branch is None:
             n = ops.rmsnorm(h, self.model.norm.weight, eps)
         else:

@@ -81,7 +81,7 @@ def _linear_backward(ctx, dy):
     w = ctx.weight_ref
     acc_tc = (ctx.needs_input_grad[1] and ctx.accumulate and w.grad is not None and tc and w.grad.dtype == torch.bfloat16
               and w.grad.dim() == 2 and w.grad.stride(1) == 1 and w.grad.data_ptr() % 16 == 0)
-    dx = dw = db = None
+    dx = dw = None
     side = _wgrad_stream(dy2.device) if (acc_tc and ctx.needs_input_grad[0]) else None
     if side is not None:
         # fork BEFORE either GEMM is enqueued: wgrad on the side stream, dgrad on the current one, join below
@@ -114,13 +114,18 @@ def _linear_backward(ctx, dy):
             dw = gemm(dy2, x2, a_mn=True, b_mn=True)
         else:
             dw = dy2.t().matmul(x2).to(weight.dtype)
-    if ctx.has_bias and ctx.needs_input_grad[2]:
-        b = ctx.bias_ref
-        if ctx.accumulate and b.grad is not None:
-            b.grad.add_(dy2.sum(0))
-        else:
-            db = dy2.sum(0).to(b.dtype)
-    return dx, dw, db, None
+    return dx, dw, _bias_grad(ctx, dy2), None
+
+
+def _bias_grad(ctx, dy2):
+    """Bias gradient of a linear layer: added to an existing ``.grad`` (accumulating layers), returned otherwise."""
+    if not (ctx.has_bias and ctx.needs_input_grad[2]):
+        return None
+    b = ctx.bias_ref
+    if ctx.accumulate and b.grad is not None:
+        b.grad.add_(dy2.sum(0))
+        return None
+    return dy2.sum(0).to(b.dtype)
 
 
 class GatherLinearFn(torch.autograd.Function):
@@ -146,9 +151,15 @@ class GatherLinearFn(torch.autograd.Function):
 
 
 def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] = None, accumulate_into_grad: bool = True,
-           gathered=None) -> torch.Tensor:
+           gathered=None, fp8: bool = False) -> torch.Tensor:
     """``gathered``: a :class:`~acco_b200.ops.gemm.GatheredWeight` when this is the first use of ``weight`` after a
-    communication round that left its remote row-blocks on their owners (fused all-gather + GEMM)."""
+    communication round that left its remote row-blocks on their owners (fused all-gather + GEMM).
+    ``fp8``: run the GEMMs of a grad-enabled call in FP8 (``ops/fp8.py``) when the shapes allow it (``fp8_supported``); no-grad calls
+    and other shapes keep the bf16 path."""
+    if fp8 and gathered is None and torch.is_grad_enabled() and (weight.requires_grad or x.requires_grad):
+        from .fp8 import Fp8LinearFn, fp8_supported
+        if fp8_supported(x, weight, bias):
+            return Fp8LinearFn.apply(x, weight, bias, accumulate_into_grad)
     if gathered is not None and bias is None and x.is_cuda:
         if torch.is_grad_enabled() and (weight.requires_grad or x.requires_grad):
             return GatherLinearFn.apply(x, weight, gathered, accumulate_into_grad)

@@ -65,6 +65,7 @@ TRAIN_DEFAULTS: Dict[str, Any] = dict(
     fault_inject=None,              # "rank@count" - that rank kills itself (os._exit) once count_grad_tot >= count; fires once per cwd
     packing=False,                  # SFT: pack whole samples into full rows (document-masked attention, per-sample positions)
     max_grad_norm=None,             # global gradient-norm clipping of every round (.inf: log the norm only); logged as grad_norm
+    fp8=False,                      # FP8 GEMMs (e4m3 / e5m2, per-tensor current scaling) for the block linears of native models (ops/fp8.py)
 )
 
 
@@ -152,6 +153,7 @@ class DecoupledTrainer:
             raise ValueError("You must select one of the following method_name: 'acco', 'ddp', 'dpu'")
         self.max_grad_norm = check_max_grad_norm(self.args.max_grad_norm)
         self._grad_norm: Optional[float] = None     # pre-clip norm of the last committed round (max_grad_norm set)
+        self._check_fp8()
 
         self.initialize_com(env)
         self._init_writer()
@@ -292,6 +294,20 @@ class DecoupledTrainer:
         if not isinstance(self.model, (LlamaForCausalLM, GPTForCausalLM)):
             raise ValueError(f"packing=True needs a native model that masks attention by position_ids; {type(self.model).__name__} "
                              "would attend across the samples of a row")
+
+    def _check_fp8(self) -> None:
+        """``fp8``: the native models' block linears run their training GEMMs in FP8 on bf16 weights and gradients."""
+        a = self.args
+        if not a.fp8:
+            return
+        from .models import GPTForCausalLM, LlamaForCausalLM
+        if not isinstance(self.model, (LlamaForCausalLM, GPTForCausalLM)):
+            raise ValueError(f"fp8=True needs a native model (LlamaForCausalLM / GPTForCausalLM); {type(self.model).__name__} has no FP8 path")
+        if not a.use_mixed_precision or str(a.ddp_weights_dtype) == "fp32":
+            raise ValueError("fp8=True quantises bf16 weights and activations: it needs use_mixed_precision=True and ddp_weights_dtype=bf16")
+        if a.fused_ag_gemm:
+            raise ValueError("fp8=True cannot be combined with fused_ag_gemm: the gathering GEMM has no FP8 instantiation")
+        self.model.fp8 = True
 
     def prepare_data(self) -> None:
         """Per-rank sharding (`trainer_base.py:183-200`)."""

@@ -1,0 +1,299 @@
+"""FP8 linear layers on the H100: the quantiser kernels bit for bit against ``quantize_ref``, the FP8 wgmma GEMM against two oracles, the
+FP8 linear autograd against the fp64 contract, whole models against fp32, and the trainer (CUDA graphs, launch counts, loss).
+
+Tolerances.
+* GEMM, fp64 oracle ``y64 = a b^T / (s_a s_b) (+ bias) (+ C)`` on the dequantised operands.  The kernel differs from it by (1) the bf16
+  rounding of the output, at most one bf16 ulp of ``|y64|`` (2^-8 |y64| covers the half-ulp rounding of the result and of the
+  added bf16 ``C``), and (2) the accumulation: Hopper's FP8 tensor cores keep about 14 bits while they sum within one wgmma
+  (DeepSeek-V3 report).  The kernel promotes every 128-deep k-block (four k32 wgmmas) to fp32, so each block loses at most
+  4 * 2^-13 of its absolute sum; summed over blocks that is 2^-11 * S with ``S = |a| |b|^T / (s_a s_b)``.  The fp32 sums of the
+  promoted fragments add K/128 * 2^-24 * S, far below that.  So ``|y - y64| <= 2^-8 |y64| + 2^-11 S + 2^-133`` (the last term is the
+  smallest bf16 subnormal).  An adding epilogue (wgrad) rounds once more per bf16 add into the output, each at the magnitude of the
+  running sum, which is bounded by ``|C| + S``: with ``splits`` partial sums added in bf16 that is ``splits * 2^-9 (|C| + S)`` more.
+* Cross-check: the bf16 wgmma GEMM on the dequantised operands (exact in bf16: e4m3 and e5m2 values are bf16 values, and the scales
+  are powers of two) multiplies the same numbers and accumulates in fp32.  Both round once to bf16, so they agree within one bf16
+  ulp plus the FP8 accumulation term ``2^-11 S`` above.
+* Whole models against fp32: q(x) and q(W) carry a relative rounding error of at most 2^-4 (e4m3) per element and q(g) 2^-3 (e5m2),
+  independent across elements, so a K-term dot product errs by about 2^-4 / sqrt(3) of its magnitude: a few per cent on every GEMM
+  output, less on the loss, which averages over tokens.  The loss must agree within 2 %; every parameter gradient must point the same
+  way (cosine >= 0.95) and have the same norm within 15 %.
+"""
+import logging
+import math
+import os
+
+import pytest
+import torch
+
+pytestmark = pytest.mark.gpu
+
+from acco_b200 import AttrDict, DecoupledTrainer, ops
+from acco_b200.callbacks import TrainerCallback
+from acco_b200.data import synthetic_pretrain_dataset
+from acco_b200.launch import DistEnv
+from acco_b200.models import GPTConfig, GPTForCausalLM, LlamaConfig, LlamaForCausalLM
+from acco_b200.ops.fp8 import E4M3, E5M2, Fp8LinearFn, gemm_fp8, quantize, quantize_ref
+
+DEV = torch.device("cuda")
+LOG = logging.getLogger("acco-test")
+
+# block GEMM shapes (N, K) of the Llama presets: qkv, o, gate|up, down
+PRESETS = {
+    "llama125m": dict(H=768, qkv=2304, I=2048),
+    "llama3-1b": dict(H=2048, qkv=3072, I=8192),
+    "llama3-8b": dict(H=4096, qkv=6144, I=14336),
+}
+
+
+def _rand(shape, seed, scale=1.0):
+    g = torch.Generator(device=DEV).manual_seed(seed)
+    return (torch.randn(shape, device=DEV, generator=g) * scale).to(torch.bfloat16)
+
+
+def _bits(t):
+    return t.view(torch.uint8)
+
+
+# ------------------------------------------------------------------------------------------------------------------ quantiser
+@pytest.mark.parametrize("fmt", [E4M3, E5M2])
+@pytest.mark.parametrize("shape,scale", [((16, 16), 1.0), ((48, 80), 3e-3), ((1040, 784), 40.0), ((8192, 768), 1.0), ((2048, 8192), 0.02),
+                                         ((4096, 2048), 1e4)])
+def test_quantize_kernel_is_bitwise_the_reference(fmt, shape, scale):
+    t = _rand(shape, seed=shape[0] + shape[1], scale=scale)
+    t[3, 5] = 0.0
+    t[0, 1] = -t[0, 1]
+    q, qT, s = quantize(t, fmt, True, True)
+    rq, _, rs = quantize_ref(t.cpu(), fmt, True, False)
+    assert torch.equal(s[:3].cpu(), rs), (s[:3], rs)
+    assert torch.equal(_bits(q).cpu(), _bits(rq))
+    assert torch.equal(_bits(qT).cpu(), _bits(rq).t().contiguous())
+    q1, qT1, _ = quantize(t, fmt, True, False)
+    q2, qT2, _ = quantize(t, fmt, False, True)
+    assert qT1 is None and q2 is None
+    assert torch.equal(_bits(q1), _bits(q)) and torch.equal(_bits(qT2), _bits(qT))
+
+
+@pytest.mark.parametrize("fmt", [E4M3, E5M2])
+def test_quantize_kernel_edges(fmt):
+    z = torch.zeros(32, 64, device=DEV, dtype=torch.bfloat16)
+    q, _, s = quantize(z, fmt)
+    assert s[:3].tolist() == [1.0, 1.0, 0.0] and int(_bits(q).max()) == 0
+    sub = torch.full((32, 64), 2.0 ** -130, device=DEV, dtype=torch.bfloat16)      # bf16 subnormals
+    q, _, s = quantize(sub, fmt)
+    rq, _, rs = quantize_ref(sub.cpu(), fmt)
+    assert torch.equal(s[:3].cpu(), rs) and torch.equal(_bits(q).cpu(), _bits(rq))
+    for bad in (float("nan"), float("inf")):
+        t = _rand((64, 32), seed=1)
+        t[7, 9] = bad
+        _, _, s = quantize(t, fmt)
+        assert math.isnan(float(s[0])) and math.isnan(float(s[1]))
+
+
+# ------------------------------------------------------------------------------------------------------------------ GEMM
+def _operands(M, N, K, a_fmt, seed):
+    a = _rand((M, K), seed)
+    b = _rand((N, K), seed + 1, scale=0.05)
+    qa, _, sa = quantize_ref(a, a_fmt)
+    qb, _, sb = quantize_ref(b, E4M3)
+    return qa, qb, sa.to(DEV), sb.to(DEV)
+
+
+def _check(y, qa, qb, sa, sb, bias=None, c=None, splits=1):
+    a64, b64 = qa.double() * float(sa[1]), qb.double() * float(sb[1])
+    y64 = a64 @ b64.t()
+    S = a64.abs() @ b64.abs().t()
+    if bias is not None:
+        y64 = y64 + bias.double()
+    if c is not None:
+        y64 = y64 + c.double()
+    err = (y.double() - y64).abs()
+    tol = 2.0 ** -8 * y64.abs() + 2.0 ** -11 * S + 2.0 ** -133
+    if c is not None:
+        tol = tol + splits * 2.0 ** -9 * (c.double().abs() + S)
+    assert bool((err <= tol).all()), f"max excess {float((err - tol).max())}"
+    return y64, S
+
+
+def _cross(y, qa, qb, sa, sb, bias=None):
+    """bf16 wgmma GEMM on the dequantised operands (exact in bf16): within one bf16 ulp plus the FP8 accumulation term."""
+    from acco_b200.ops.gemm import gemm
+    a = (qa.float() * sa[1]).to(torch.bfloat16)
+    b = (qb.float() * sb[1]).to(torch.bfloat16)
+    yb = gemm(a, b, bias=bias)
+    S = (a.double().abs() @ b.double().abs().t())
+    ref = torch.maximum(y.double().abs(), yb.double().abs())
+    ulp = torch.exp2(torch.floor(torch.log2(ref.clamp_min(2.0 ** -126)))) * 2.0 ** -7
+    diff = (y.double() - yb.double()).abs()
+    bad = diff > ulp + 2.0 ** -11 * S
+    assert not bool(bad.any()), f"{int(bad.sum())} elements beyond the bound"
+    assert float((diff <= ulp).double().mean()) >= 0.5          # most elements: the two kernels round the same value
+
+
+@pytest.mark.parametrize("bias", [False, True])
+@pytest.mark.parametrize("M,N,K", [(256, 384, 768), (208, 200, 784), (1040, 2056, 2048), (128, 64, 16)])
+def test_gemm_fp8_forward(M, N, K, bias):
+    qa, qb, sa, sb = _operands(M, N, K, E4M3, seed=M + N + K)
+    bv = _rand((N,), seed=5, scale=0.5) if bias else None
+    y = gemm_fp8(qa, qb, sa, sb, bias=bv)
+    assert y.dtype == torch.bfloat16 and y.shape == (M, N)
+    _check(y, qa, qb, sa, sb, bias=bv)
+    _cross(y, qa, qb, sa, sb, bias=bv)
+
+
+@pytest.mark.parametrize("M,N,K", [(4096, 768, 2304), (4096, 2048, 8192), (1024, 4096, 14336), (208, 520, 1040)])
+def test_gemm_fp8_dgrad_e5m2(M, N, K):
+    qa, qb, sa, sb = _operands(M, N, K, E5M2, seed=M + 3 * N)
+    y = gemm_fp8(qa, qb, sa, sb)
+    _check(y, qa, qb, sa, sb)
+    _cross(y, qa, qb, sa, sb)
+
+
+@pytest.mark.parametrize("splits", [1, 4])
+@pytest.mark.parametrize("M,N,K", [(768, 2304, 4096), (2048, 8192, 8192), (336, 528, 1024)])
+def test_gemm_fp8_wgrad_reduce_add(M, N, K, splits):
+    qa, qb, sa, sb = _operands(M, N, K, E5M2, seed=N + K + splits)
+    c = _rand((M, N), seed=9, scale=0.1)
+    out = c.clone()
+    gemm_fp8(qa, qb, sa, sb, out=out, accumulate=True, splits=splits)
+    _check(out, qa, qb, sa, sb, c=c, splits=splits)
+
+
+@pytest.mark.parametrize("preset", sorted(PRESETS))
+def test_gemm_fp8_preset_block_shapes(preset):
+    p = PRESETS[preset]
+    T = 2048
+    for N, K in ((p["qkv"], p["H"]), (p["H"], p["H"]), (2 * p["I"], p["H"]), (p["H"], p["I"])):
+        qa, qb, sa, sb = _operands(T, N, K, E4M3, seed=N + K)
+        _check(gemm_fp8(qa, qb, sa, sb), qa, qb, sa, sb)
+
+
+# ------------------------------------------------------------------------------------------------------------------ autograd
+def test_fp8_linear_autograd_against_the_fp64_contract():
+    T, K, N = 1024, 768, 2304
+    x = _rand((T, K), 1).requires_grad_(True)
+    w = torch.nn.Parameter(_rand((N, K), 2, scale=0.05))
+    b = torch.nn.Parameter(_rand((N,), 3, scale=0.1))
+    w.grad = torch.zeros_like(w)
+    b.grad = torch.zeros_like(b)
+    gs = [_rand((T, N), 10 + i, scale=1e-3) for i in range(2)]
+    for g in gs:
+        y = ops.linear(x, w, b, fp8=True)
+        qx, _, sx = quantize_ref(x.detach(), E4M3)
+        qw, _, sw = quantize_ref(w.detach(), E4M3)
+        qg, _, sg = quantize_ref(g, E5M2)
+        _check(y.detach(), qx, qw, sx, sw, bias=b.detach())
+        x.grad = None
+        prev = w.grad.clone()
+        y.backward(g)
+        _check(x.grad, qg, qw.t().contiguous(), sg, sw)
+        # wgrad added into the existing bf16 gradient (T = 1024 is 8 k-blocks: one K split)
+        _check(w.grad, qg.t().contiguous(), qx.t().contiguous(), sg, sx, c=prev)
+    torch.testing.assert_close(b.grad.float(), sum(g.float().sum(0) for g in gs), rtol=2e-2, atol=1e-3)
+
+
+# ------------------------------------------------------------------------------------------------------------------ models
+def _llama():
+    torch.manual_seed(0)
+    return LlamaForCausalLM(LlamaConfig(vocab_size=512, hidden_size=256, intermediate_size=512, num_hidden_layers=2, num_attention_heads=4,
+                                        num_key_value_heads=2, max_position_embeddings=256))
+
+
+def _neo():
+    torch.manual_seed(0)
+    m = GPTForCausalLM(GPTConfig(vocab_size=512, hidden_size=256, num_hidden_layers=2, num_attention_heads=4, max_position_embeddings=256,
+                                 attention_layers=["global", "local"], window_size=64))
+    with torch.no_grad():
+        for n, p in m.named_parameters():
+            if n.endswith("bias") and ".mlp." in n or n.endswith("out_proj.bias"):
+                p.normal_(0.0, 0.02)                    # non-zero biases: the FP8 epilogue adds them
+    return m
+
+
+def _loss_and_grads(model, dtype, fp8, ids):
+    model = model.to(DEV, dtype)
+    model.fp8 = fp8
+    model.zero_grad(set_to_none=True)
+    out = model(input_ids=ids, labels=ids)
+    out.loss.backward()
+    return float(out.loss), {n: p.grad.float().clone() for n, p in model.named_parameters()}
+
+
+@pytest.mark.parametrize("make", [_llama, _neo], ids=["llama_gqa", "gptneo_window_bias"])
+def test_whole_model_fp8_against_fp32(make):
+    ids = torch.randint(0, 512, (4, 256), device=DEV, generator=torch.Generator(device=DEV).manual_seed(0))
+    ref_loss, ref = _loss_and_grads(make(), torch.float32, False, ids)
+    loss, got = _loss_and_grads(make(), torch.bfloat16, True, ids)
+    assert abs(loss - ref_loss) <= 0.02 * abs(ref_loss)
+    for n, g in got.items():
+        r = ref[n]
+        if float(r.norm()) == 0:
+            continue
+        cos = float((g * r).sum() / (g.norm() * r.norm()))
+        assert cos >= 0.95, (n, cos)
+        assert abs(float(g.norm()) / float(r.norm()) - 1) <= 0.15, n
+
+
+def test_launch_counts_per_micro_batch():
+    model = _llama().to(DEV, torch.bfloat16)
+    model.fp8 = True
+    ids = torch.randint(0, 512, (2, 128), device=DEV)
+    ops.reset_launch_counts()
+    model(input_ids=ids, labels=ids).loss.backward()
+    c = ops.launch_counts()
+    n = 3 * 4 * model.config.num_hidden_layers        # per block linear: x, W, g quantised once each; fwd, dgrad, wgrad GEMMs
+    assert (c.get("fp8_amax"), c.get("fp8_cast"), c.get("gemm_fp8")) == (n, n, n), c
+    ops.reset_launch_counts()
+    with torch.no_grad():
+        model(input_ids=ids)
+    assert "gemm_fp8" not in ops.launch_counts()       # no-grad forwards stay bf16
+
+
+# ------------------------------------------------------------------------------------------------------------------ trainer
+class _Losses(TrainerCallback):
+    def __init__(self):
+        self.losses = []
+
+    def on_log(self, trainer, scalars):
+        self.losses.append(float(scalars["loss"]))
+
+
+def _train(tmp_path, fp8, steps, seed=0, graphs=True, hidden=256, layers=4, S=256, B=8):
+    os.environ.setdefault("ACCO_ALLOW_NCCL_FALLBACK", "1")
+    torch.manual_seed(seed)
+    model = LlamaForCausalLM(LlamaConfig(vocab_size=512, hidden_size=hidden, intermediate_size=2 * hidden, num_hidden_layers=layers,
+                                         num_attention_heads=4, num_key_value_heads=2, max_position_embeddings=S))
+    ds = synthetic_pretrain_dataset(B * steps * 2, S, 512, S, seed=7)
+    args = AttrDict(method_name="ddp", batch_size=B, n_grad_accumulation=1, max_length=S, nb_steps_tot=steps, warmup=10, learning_rate=2e-3,
+                    weight_decay=0.0, scheduler_name="constant", save=False, tensorboard=False, use_mixed_precision=True, seed=seed,
+                    cuda_graphs=graphs, fp8=fp8, log_every=1)
+    cwd = os.getcwd()
+    os.chdir(tmp_path)
+    try:
+        t = DecoupledTrainer(model=model, train_dataset=ds, args=args, log=LOG, env=DistEnv(id_run=f"fp8{fp8}{seed}{graphs}"))
+        cb = _Losses()
+        t.add_callback(cb)
+        t.train()
+    finally:
+        os.chdir(cwd)
+        from acco_b200.launch import shutdown_distributed
+        shutdown_distributed()
+    return cb.losses
+
+
+def test_trainer_fp8_cuda_graphs_match_eager(tmp_path):
+    g = _train(tmp_path, True, 12, graphs=True)
+    e = _train(tmp_path, True, 12, graphs=False)
+    assert len(g) == len(e) == 12
+    for a, b in zip(g, e):
+        assert abs(a - b) <= 1e-2 * abs(b), (g, e)
+
+
+def test_trainer_fp8_loss_tracks_bf16_on_markov_data(tmp_path):
+    bf0 = _train(tmp_path, False, 300, seed=0)
+    bf1 = _train(tmp_path, False, 300, seed=1)
+    f8 = _train(tmp_path, True, 300, seed=0)
+    tail = lambda xs: sum(xs[-50:]) / 50
+    assert tail(f8) < 0.8 * f8[0]                                   # it learns
+    gap = abs(tail(f8) - tail(bf0))
+    allowed = max(abs(tail(bf1) - tail(bf0)), 0.01 * tail(bf0))
+    assert gap <= allowed, (tail(f8), tail(bf0), tail(bf1))

@@ -7,7 +7,7 @@
 
 The summary counts, per listed kernel, the SASS mnemonics that show the Hopper-native path: `HGMMA` = wgmma.mma_async,
 `UTMALDG` / `UTMASTG` = TMA load / store, `SYNCS` = mbarrier operations, `USETMAXREG` = setmaxnreg, `REDG` = per-element atomic
-adds, `LDGMC` = multimem.ld_reduce ...  `tests/test_sass_listings.py` runs the --check so a stale summary cannot be committed."""
+adds, `LDGMC` = multimem.ld_reduce, `QGMMA` = wgmma.mma_async on FP8 operands ...  `tests/test_sass_listings.py` runs the --check so a stale summary cannot be committed."""
 import json
 import os
 import re
@@ -31,6 +31,10 @@ KERNELS = {
     "attn_fwd_wgmma_seg.sass": "_ZN9acco_attn15attn_fwd_kernelILb1EEEvNS_9FwdParamsE",      # document-masked (packed rows)
     "attn_bwd_mma.sass": "_ZN9acco_attn15attn_bwd_kernelILb0EEEvNS_9BwdParamsE",
     "attn_bwd_mma_seg.sass": "_ZN9acco_attn15attn_bwd_kernelILb1EEEvNS_9BwdParamsE",
+    "gemm_fp8_bn128_e4m3.sass": "_ZN9acco_gemm15gemm_fp8_kernelILi128ELi1EEEvNS_6ParamsE",     # train.fp8: forward
+    "gemm_fp8_bn128_e5m2.sass": "_ZN9acco_gemm15gemm_fp8_kernelILi128ELi2EEEvNS_6ParamsE",     # dgrad / wgrad
+    "fp8_amax.sass": "_ZN8acco_fp815fp8_amax_kernelEPK5uint4xPj",
+    "fp8_cast_e4m3.sass": "_ZN8acco_fp815fp8_cast_kernelILi0EEEvPK13__nv_bfloat16PKjiPhS6_Pfii",
 }
 MNEMONICS = ["HGMMA", "UTMALDG", "UTMALDG.2D.MULTICAST", "UTMASTG", "UTMACMDFLUSH", "SYNCS", "USETMAXREG", "REDG", "LDGMC", "HMMA", "MUFU.SQRT",
              "MUFU.EX2", "CCTL"]
@@ -51,6 +55,10 @@ def count(txt: str) -> dict:
         c[m] = sum(1 for o in ops if o == m or o.startswith(m + "."))
     # multimem.st shows up as a STG on the multicast address: count the .STRONG.SYS 128-bit stores as a proxy
     c["STG.E.128.STRONG.SYS"] = sum(1 for o in ops if o.startswith("STG.E") and "128" in o and "SYS" in o)
+    # FP8 wgmma (QGMMA) is listed only where it occurs, so the entries of the bf16 kernels keep their keys
+    q = sum(1 for o in ops if o == "QGMMA" or o.startswith("QGMMA."))
+    if q:
+        c["QGMMA"] = q
     return c
 
 

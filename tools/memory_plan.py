@@ -5,7 +5,8 @@
 
 Persistent buffers are exact (they follow the arena / optimizer layout: two bf16 parameter sets, two bf16 gradient accumulators and
 the fp32 optimizer shard); activations are an estimate of what the native Llama keeps for backward (bf16 tensors saved by the
-fused ops + the padded logits).  Budget: an 80 GB H100, of which 92 % is planned."""
+fused ops + the padded logits).  ``--fp8`` (train key ``fp8``): the block linears keep their GEMM inputs as FP8 copies, 1 byte per
+element instead of 2.  Budget: an 80 GB H100, of which 92 % is planned."""
 import argparse
 import json
 import os
@@ -20,7 +21,7 @@ from acco_b200.parallel.arena import ShardLayout
 GB = 1e9
 
 
-def plan(cfg: LlamaConfig, world: int, batch: int, seq: int, method: str = "acco", align: int = 1024) -> dict:
+def plan(cfg: LlamaConfig, world: int, batch: int, seq: int, method: str = "acco", align: int = 1024, fp8: bool = False) -> dict:
     n = cfg.num_parameters(padded=True)
     lay = ShardLayout(n, world, align)
     two = 2                                                    # bf16
@@ -34,12 +35,14 @@ def plan(cfg: LlamaConfig, world: int, batch: int, seq: int, method: str = "acco
     T = batch * seq
     H, I, L = cfg.hidden_size, cfg.intermediate_size, cfg.num_hidden_layers
     D, Hq, Hk = cfg.head_dim, cfg.num_attention_heads, cfg.num_key_value_heads
+    gemm_in = 1 if fp8 else two                                # FP8: the block GEMMs keep q(x)^T instead of x
     per_layer = T * two * (
         2 * H                      # inputs of the two add+RMSNorm ops (h)
-        + 2 * H                    # normalised activations fed to the qkv / gate|up GEMMs
         + (Hq + 2 * Hk) * D        # rotated qkv (attention backward)
-        + Hq * D                   # attention output (o_proj input) 
         + 2 * I                    # gate|up (SwiGLU backward)
+    ) + T * gemm_in * (
+        2 * H                      # normalised activations fed to the qkv / gate|up GEMMs
+        + Hq * D                   # attention output (o_proj input)
         + I                        # SwiGLU output (down_proj input)
     ) + T * 4 * (2 + Hq)           # rstd x2, attention LSE
     acts = L * per_layer + T * two * H + T * two * cfg.padded_vocab          # final norm input + logits (turned into dlogits in place)
@@ -56,10 +59,11 @@ def main(argv=None):
     ap.add_argument("--batch", type=int, default=4)
     ap.add_argument("--seq", type=int, default=512)
     ap.add_argument("--method", default="acco", choices=["acco", "dpu", "ddp"])
+    ap.add_argument("--fp8", action="store_true", help="train.fp8: FP8 copies of the block GEMM inputs are kept for backward")
     a = ap.parse_args(argv)
     cfg = LlamaConfig.from_dict(PRESETS[a.model][1])
-    out = plan(cfg, a.gpus, a.batch, a.seq, a.method)
-    print(json.dumps({"model": a.model, "gpus": a.gpus, "batch": a.batch, "seq": a.seq, **out}, indent=1))
+    out = plan(cfg, a.gpus, a.batch, a.seq, a.method, fp8=a.fp8)
+    print(json.dumps({"model": a.model, "gpus": a.gpus, "batch": a.batch, "seq": a.seq, "fp8": a.fp8, **out}, indent=1))
     return out
 
 
