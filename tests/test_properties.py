@@ -97,14 +97,18 @@ def test_tentative_plus_real_equals_one_large_batch_step(seed, n1, n2):
 # ----------------------------------------------------------------------------------------------
 # GEMM work decomposition (mirrors `decode_unit` / the unit loops of csrc/gemm_wgmma.cu)
 # ----------------------------------------------------------------------------------------------
-def _gemm_units(M, N, K, bn, splits, pm, pn, slots):
+def _gemm_units(M, N, K, bn, splits, pm, pn, slots, band=None):
     """Python twin of the device-side tile scheduler: yields (cluster, cta, mb, n_blk, kb0, kb1) for every unit every CTA runs.
-    A CTA computes 128-row tiles; a cluster is pm x pn CTAs (cluster rank = pi * pn + pj) owning a super-tile of pm x pn tiles."""
+    A CTA computes 128-row tiles; a cluster is pm x pn CTAs (cluster rank = pi * pn + pj) owning a super-tile of pm x pn tiles.
+    Tiles go in bands of ``band`` super-tile columns (default: one band, row-major): columns fastest inside a band, then rows, then
+    the next band; the last band may be narrower."""
     BM, BK = 128, 64
     num_n, num_k = -(-N // bn), -(-K // BK)
     num_mb = -(-M // BM)
     num_sn = -(-num_n // pn)
-    tiles = -(-num_mb // pm) * num_sn
+    num_smb = -(-num_mb // pm)
+    tiles = num_smb * num_sn
+    band = num_sn if band is None else band
     splits = max(1, min(splits, num_k))
     kbs = -(-num_k // splits)
     splits = -(-num_k // kbs)
@@ -116,7 +120,11 @@ def _gemm_units(M, N, K, bn, splits, pm, pn, slots):
             t = cl
             while t < num_units:
                 s, tile = divmod(t, tiles)
-                smb, sn = divmod(tile, num_sn)
+                bi = tile // (band * num_smb)
+                sn0 = bi * band
+                width = min(band, num_sn - sn0)
+                smb, c = divmod(tile - sn0 * num_smb, width)
+                sn = sn0 + c
                 yield cl, cta, smb * pm + pi, sn * pn + pj, s * kbs, min(num_k, s * kbs + kbs)
                 t += grid_clusters
     return
@@ -124,16 +132,19 @@ def _gemm_units(M, N, K, bn, splits, pm, pn, slots):
 
 @settings(max_examples=150, deadline=None)
 @given(M=st.integers(1, 3000), N=st.integers(8, 1500), K=st.integers(8, 4000), bn=st.sampled_from([64, 128, 256]),
-       splits=st.integers(1, 9), pm=st.sampled_from([1, 2]), pn=st.sampled_from([1, 2]), slots=st.integers(1, 132))
-def test_gemm_tile_scheduler_covers_every_output_k_block_exactly_once(M, N, K, bn, splits, pm, pn, slots):
+       splits=st.integers(1, 9), pm=st.sampled_from([1, 2]), pn=st.sampled_from([1, 2]), slots=st.integers(1, 132),
+       band=st.integers(1, 40))
+def test_gemm_tile_scheduler_covers_every_output_k_block_exactly_once(M, N, K, bn, splits, pm, pn, slots, band):
     """Every real (m-block, n-block, k-block) triple is computed by exactly one CTA; phantom tiles (odd counts under clusters) lie
     entirely outside the matrix (TMA zero-fills their loads, the epilogue stores nothing); all CTAs of a cluster run the same number
-    of k-iterations (they share pipeline stages through multicast), and no split is empty."""
+    of k-iterations (they share pipeline stages through multicast), and no split is empty.  For every band width 1 ... num_sn
+    (``band`` beyond num_sn is row-major order), including a narrower last band."""
     BM = 128
     num_mb, num_n, num_k = -(-M // BM), -(-N // bn), -(-K // 64)
+    band = min(band, -(-num_n // pn))
     seen = {}
     per_cta_iters = {}
-    for cl, cta, mb, n_blk, kb0, kb1 in _gemm_units(M, N, K, bn, splits, pm, pn, slots):
+    for cl, cta, mb, n_blk, kb0, kb1 in _gemm_units(M, N, K, bn, splits, pm, pn, slots, band):
         assert kb1 > kb0                                             # no empty split
         per_cta_iters[(cl, cta)] = per_cta_iters.get((cl, cta), 0) + (kb1 - kb0)
         real = mb < num_mb and n_blk < num_n
@@ -149,3 +160,16 @@ def test_gemm_tile_scheduler_covers_every_output_k_block_exactly_once(M, N, K, b
     for (cl, cta), it in per_cta_iters.items():
         by_cluster.setdefault(cl, set()).add(it)
     assert all(len(v) == 1 for v in by_cluster.values())           # lock-step inside a cluster
+
+
+def test_gemm_band_order_walks_bands_of_columns():
+    """The band decode on the LM-head forward's geometry (197 super-columns of 256, bands of 16, last band 5 wide): inside a band the
+    columns go fastest, then the rows; band b covers columns [16 b, 16 b + 16) of every row before band b + 1 starts."""
+    M, N, K, bn = 8192, 50304, 768, 256
+    order = [(mb, n) for _, _, mb, n, _, _ in _gemm_units(M, N, K, bn, 1, 1, 1, 1, band=16)]
+    assert len(order) == 64 * 197 and len(set(order)) == len(order)
+    assert order[:17] == [(0, c) for c in range(16)] + [(1, 0)]
+    last = order[64 * 192:]
+    assert last[:6] == [(0, 192), (0, 193), (0, 194), (0, 195), (0, 196), (1, 192)] and last[-1] == (63, 196)
+    for i, (mb, n) in enumerate(order[:64 * 192]):
+        assert n // 16 == i // (64 * 16)
