@@ -149,16 +149,21 @@ __global__ void __launch_bounds__(256) swiglu_bwd_kernel(const __nv_bfloat16* __
 }
 
 // ---- GELU (tanh approximation, "gelu_new") --------------------------------------------------------------------------
+// gelu_new(x) = 0.5 x (1 + tanh(u)), u = k0 (x + k1 x^3), evaluated as x * sig(z) with z = 2u (1 + tanh(u) = 2 sig(2u),
+// 1 - tanh(u)^2 = 4 sig(2u) (1 - sig(2u))).  The tanh form cancels in 1 + t for x < -2, where the ~2^-11 relative error of the
+// fast-math tanh (MUFU.TANH) is worth up to thousands of bf16 ulps of the output (256 measured on an H100 below x = -4); the
+// sigmoid form has no such difference.
+constexpr float kGeluZ = 1.5957691216057308f, kGeluK1 = 0.044715f;   // 2 * sqrt(2 / pi), k1
 ACCO_DEVINL float gelu_new_f(float x) {
-    const float k0 = 0.7978845608028654f, k1 = 0.044715f;
-    const float t = tanhf(k0 * (x + k1 * x * x * x));
-    return 0.5f * x * (1.f + t);
+    const float z = kGeluZ * x * (1.f + kGeluK1 * x * x);
+    return x * (1.f / (1.f + __expf(-z)));
 }
 ACCO_DEVINL float gelu_new_grad(float x) {
-    const float k0 = 0.7978845608028654f, k1 = 0.044715f;
-    const float u = k0 * (x + k1 * x * x * x);
-    const float t = tanhf(u);
-    return 0.5f * (1.f + t) + 0.5f * x * (1.f - t * t) * k0 * (1.f + 3.f * k1 * x * x);
+    // gelu' is exactly 1 (x > 0) or 0 (x < 0) in fp32 beyond |x| = 12; clamping keeps x^2 finite (no inf * 0 = NaN)
+    x = fminf(fmaxf(x, -12.f), 12.f);
+    const float x2 = x * x;
+    const float s = 1.f / (1.f + __expf(-kGeluZ * x * (1.f + kGeluK1 * x2)));
+    return s * (1.f + x * (1.f - s) * kGeluZ * (1.f + 3.f * kGeluK1 * x2));
 }
 
 __global__ void __launch_bounds__(256) gelu_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y, long long nvec) {
