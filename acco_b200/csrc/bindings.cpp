@@ -72,6 +72,9 @@ struct RoundParams {   // must mirror acco::RoundParams in rs_adam_ag.cu
     const float* inv_count_in;
     const long long* skip;
     int n_skip;
+    const long long* nodecay;
+    int n_nodecay;
+    long long nodecay_base;
     int watchdog_s;
     int gated;
     long long slice;
@@ -263,10 +266,24 @@ void fill_hyper(RoundParams& P, double lr, double b1, double b2, double eps, dou
     P.commit = (int)commit; P.add_stash = add_stash ? 1 : 0; P.write_stash = write_stash ? 1 : 0;
 }
 
+// No-decay table of a round: sorted, disjoint [lo, hi) ranges of flat parameter indices updated without weight decay, and the flat
+// index of the shard's element 0.  The caller guarantees the order (ShardedAdamW.set_no_decay checks it where the table is built):
+// checking it here would copy the table to the host on every round.
+void set_nodecay(RoundParams& P, const c10::optional<torch::Tensor>& ranges, int64_t base) {
+    if (!ranges.has_value() || !ranges->defined() || ranges->numel() == 0) return;
+    TORCH_CHECK(ranges->is_cuda() && ranges->scalar_type() == torch::kInt64 && ranges->is_contiguous() && ranges->dim() == 2 && ranges->size(1) == 2,
+                "no_decay_ranges must be a contiguous CUDA int64 [n, 2] tensor");
+    TORCH_CHECK(base >= 0, "shard_base must not be negative");
+    P.nodecay = (const long long*)ranges->data_ptr<int64_t>();
+    P.n_nodecay = (int)ranges->size(0);
+    P.nodecay_base = base;
+}
+
 // Local (single GPU / post-NCCL) sharded AdamW: grad_sum [S] (bf16|fp32) -> out [S] (bf16|fp32)
 void adamw_shard(torch::Tensor grad_sum, torch::Tensor master, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, torch::Tensor stash,
                  torch::Tensor out, torch::Tensor inv_count, torch::Tensor scratch /* int32[4]: stash_count,total,epoch,done */,
-                 double lr, double b1, double b2, double eps, double wd, int64_t step, int64_t commit, bool add_stash, bool write_stash) {
+                 double lr, double b1, double b2, double eps, double wd, int64_t step, int64_t commit, bool add_stash, bool write_stash,
+                 c10::optional<torch::Tensor> no_decay_ranges, int64_t shard_base) {
     check_f32(master, "master"); check_f32(exp_avg, "exp_avg"); check_f32(exp_avg_sq, "exp_avg_sq"); check_f32(stash, "stash"); check_f32(inv_count, "inv_count");
     const c10::cuda::CUDAGuard guard(master.device());
     const int64_t S = master.numel();
@@ -285,6 +302,7 @@ void adamw_shard(torch::Tensor grad_sum, torch::Tensor master, torch::Tensor exp
     P.inv_count_in = inv_count.data_ptr<float>();
     P.slice = S; P.rank = 0; P.world = 1; P.local_count = 0;
     fill_hyper(P, lr, b1, b2, eps, wd, step, commit, add_stash, write_stash);
+    set_nodecay(P, no_decay_ranges, shard_base);
     TORCH_CHECK(acco_rs_adam_ag(&P, gb, ob, 0, default_grid(0, S), stream()) == 0, "adamw_shard launch failed");
 }
 
@@ -329,7 +347,7 @@ void rs_adam_ag(std::vector<int64_t> acc_ptrs, std::vector<int64_t> theta_ptrs, 
                 torch::Tensor scratch /* int32[4] */, int64_t slice, int64_t rank, int64_t world, int64_t local_count,
                 double lr, double b1, double b2, double eps, double wd, int64_t step, int64_t commit, bool add_stash, bool write_stash,
                 bool grad_bf16, bool out_bf16, int64_t mode, int64_t grid, c10::optional<torch::Tensor> skip_ranges,
-                c10::optional<torch::Tensor> inv_count) {
+                c10::optional<torch::Tensor> inv_count, c10::optional<torch::Tensor> no_decay_ranges) {
     check_f32(master, "master"); check_f32(exp_avg, "exp_avg"); check_f32(exp_avg_sq, "exp_avg_sq");
     const c10::cuda::CUDAGuard guard(master.device());
     TORCH_CHECK(master.numel() == slice, "slice must match the shard state");
@@ -350,6 +368,7 @@ void rs_adam_ag(std::vector<int64_t> acc_ptrs, std::vector<int64_t> theta_ptrs, 
         if (mode != 0) P.gated = 2;
     }
     fill_hyper(P, lr, b1, b2, eps, wd, step, commit, add_stash, write_stash);
+    set_nodecay(P, no_decay_ranges, rank * slice);
     const int g = grid > 0 ? (int)grid : default_grid((int)mode, slice);
     TORCH_CHECK(acco_rs_adam_ag(&P, grad_bf16, out_bf16, (int)mode, g, stream()) == 0, "rs_adam_ag launch failed");
 }
@@ -603,12 +622,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("swiglu_bwd", &swiglu_bwd);
     m.def("ce_fwd", &ce_fwd);
     m.def("ce_bwd_inplace", &ce_bwd_inplace);
-    m.def("adamw_shard", &adamw_shard);
+    m.def("adamw_shard", &adamw_shard, py::arg("grad_sum"), py::arg("master"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("stash"),
+          py::arg("out"), py::arg("inv_count"), py::arg("scratch"), py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"), py::arg("wd"),
+          py::arg("step"), py::arg("commit"), py::arg("add_stash"), py::arg("write_stash"), py::arg("no_decay_ranges") = py::none(),
+          py::arg("shard_base") = 0);
     m.def("rs_adam_ag", &rs_adam_ag, py::arg("acc_ptrs"), py::arg("theta_ptrs"), py::arg("pad_ptrs"), py::arg("acc_mc"), py::arg("theta_mc"),
           py::arg("master"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("stash"), py::arg("scratch"), py::arg("slice"), py::arg("rank"),
           py::arg("world"), py::arg("local_count"), py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"), py::arg("wd"), py::arg("step"),
           py::arg("commit"), py::arg("add_stash"), py::arg("write_stash"), py::arg("grad_bf16"), py::arg("out_bf16"), py::arg("mode"),
-          py::arg("grid"), py::arg("skip_ranges"), py::arg("inv_count") = py::none());
+          py::arg("grid"), py::arg("skip_ranges"), py::arg("inv_count") = py::none(), py::arg("no_decay_ranges") = py::none());
     m.def("round_norm", &round_norm, py::arg("acc_ptrs"), py::arg("pad_ptrs"), py::arg("acc_mc"), py::arg("stash"), py::arg("scratch"),
           py::arg("out"), py::arg("slice"), py::arg("rank"), py::arg("world"), py::arg("local_count"), py::arg("add_stash"), py::arg("grad_bf16"),
           py::arg("mode"), py::arg("grid"), py::arg("max_norm"));

@@ -21,6 +21,9 @@
 // Optional global gradient-norm clipping (train key `max_grad_norm`): round_norm_kernel streams the same slice first, exchanges
 // the per-rank sums of squares through the signal pad and hands rs_adam_ag_kernel 1/count * clip_coef through `inv_count_in`,
 // so the AdamW pass itself is unchanged.
+// Optional weight-decay exclusion (train key `no_decay_1d`): `nodecay` lists the ranges of the flat parameter vector (norm gains, biases)
+// whose master weights are updated with decay = 1.  Rounds with a table run the kNoDecay instantiations; the gradient path, the
+// barriers and the stash do not change.
 // Cross-GPU ordering: a start barrier (every rank's accumulator is final; also carries the counts)
 // and an end barrier (every rank's pushes have landed) on flag words in a symmetric signal pad,
 // written with st.release.sys and polled with ld.acquire.sys; the epoch lives in device memory so
@@ -56,6 +59,9 @@ struct RoundParams {
     const float* inv_count_in;         // optional device scalar 1/count (world==1 library path); else nullptr
     const long long* skip;             // sorted, disjoint [lo, hi) element ranges that are NOT pushed to peers (they are pulled
     int n_skip;                        //   later by the gather-GEMM, KERNEL B); the owner still updates its own copy
+    const long long* nodecay;          // sorted, disjoint [lo, hi) element ranges of the flat parameter vector that are updated without
+    int n_nodecay;                     //   weight decay (train key `no_decay_1d`: norm gains and biases); any element boundaries
+    long long nodecay_base;            // flat index of this shard's element 0 (rank * slice inside a fused round)
     int watchdog_s;                    // trap if a peer has not reached a barrier after this many seconds (0 = wait forever)
     int gated;                         // 1: the start barrier already ran in round_gate_kernel (tiny, so waiting for a slow peer
                                        //    does not pin registers / SM slots that the overlapping compute needs)
@@ -139,15 +145,39 @@ template <typename T> struct Elem;
 template <> struct Elem<__nv_bfloat16> { static constexpr int kVec = 8; };   // elements per 16 bytes
 template <> struct Elem<float> { static constexpr int kVec = 4; };
 
-// true iff element e lies in one of the sorted, disjoint skip ranges (binary search; ranges are 8-aligned)
-ACCO_DEVINL bool in_skip(const RoundParams& P, long long e) {
-    int lo = 0, hi = P.n_skip;
+// Index of the first of `n` sorted, disjoint [lo, hi) ranges that ends after element e (n if none does): binary search.
+ACCO_DEVINL int first_range_after(const long long* tab, int n, long long e) {
+    int lo = 0, hi = n;
     while (lo < hi) {
         const int mid = (lo + hi) >> 1;
-        if (__ldg(P.skip + 2 * mid + 1) <= e) lo = mid + 1;
+        if (__ldg(tab + 2 * mid + 1) <= e) lo = mid + 1;
         else hi = mid;
     }
-    return lo < P.n_skip && __ldg(P.skip + 2 * lo) <= e;
+    return lo;
+}
+
+// true iff element e lies in one of the skip ranges (they are 8-aligned)
+ACCO_DEVINL bool in_skip(const RoundParams& P, long long e) {
+    const int r = first_range_after(P.skip, P.n_skip, e);
+    return r < P.n_skip && __ldg(P.skip + 2 * r) <= e;
+}
+
+// Bit j set iff element e + j (flat index, j < 8) lies in a no-decay range.  One search per vector: a vector lies wholly inside or
+// wholly outside a range except at the at most 2 * n_nodecay range boundaries, where the ranges it touches are walked.
+ACCO_DEVINL unsigned nodecay_mask(const RoundParams& P, long long e) {
+    int r = first_range_after(P.nodecay, P.n_nodecay, e);
+    if (r == P.n_nodecay) return 0u;
+    long long lo = __ldg(P.nodecay + 2 * r);
+    if (lo >= e + 8) return 0u;
+    if (lo <= e && __ldg(P.nodecay + 2 * r + 1) >= e + 8) return 0xFFu;
+    unsigned mask = 0u;
+    while (lo < e + 8) {
+        const int a = (int)(max(lo, e) - e), b = (int)(min(__ldg(P.nodecay + 2 * r + 1), e + 8) - e);
+        mask |= ((1u << b) - 1u) & ~((1u << a) - 1u);
+        if (++r == P.n_nodecay) break;
+        lo = __ldg(P.nodecay + 2 * r);
+    }
+    return mask;
 }
 
 // Load 8 consecutive gradient elements (sum over ranks) starting at element `e` of the full buffer.
@@ -280,7 +310,9 @@ __global__ void __launch_bounds__(32) round_gate_kernel(const __grid_constant__ 
 // threads x <= 64 registers, one CTA per SM, max shared-memory carve-out).  Not measured; the default instantiations do not use it.
 template <int MODE, bool kSmall = false> constexpr int round_threads() { return (MODE == 2 || kSmall) ? 256 : kAdamThreads; }
 
-template <typename G, typename O, int MODE, bool kSmall = false>
+// kNoDecay: the round has a no-decay table (P.n_nodecay > 0).  The host picks the instantiation, so a round without a table runs the
+// kernel without any lookup, the instruction stream it was measured with.
+template <typename G, typename O, int MODE, bool kSmall = false, bool kNoDecay = false>
 __global__ void __launch_bounds__(round_threads<MODE, kSmall>(), (MODE == 2 || kSmall) ? 4 : 1) rs_adam_ag_kernel(const __grid_constant__ RoundParams P) {
     __shared__ int s_total;
     const int W = P.world;
@@ -359,10 +391,14 @@ __global__ void __launch_bounds__(round_threads<MODE, kSmall>(), (MODE == 2 || k
             const float4* m4 = reinterpret_cast<const float4*>(P.exp_avg + i);
             const float4* v4 = reinterpret_cast<const float4*>(P.exp_avg_sq + i);
             const float4* p4 = reinterpret_cast<const float4*>(P.master + i);
-            const float4 ma = m4[0], mb = m4[1], va = v4[0], vb = v4[1], pa = p4[0], pb = p4[1];
+            const float4 ma = m4[0], mb = m4[1], va = v4[0], vb = v4[1];
             float m[8] = {ma.x, ma.y, ma.z, ma.w, mb.x, mb.y, mb.z, mb.w};
             float vv[8] = {va.x, va.y, va.z, va.w, vb.x, vb.y, vb.z, vb.w};
-            float p[8] = {pa.x, pa.y, pa.z, pa.w, pb.x, pb.y, pb.z, pb.w};
+            float p[8];
+            if constexpr (!kNoDecay) {
+                const float4 pa = p4[0], pb = p4[1];
+                p[0] = pa.x; p[1] = pa.y; p[2] = pa.z; p[3] = pa.w; p[4] = pb.x; p[5] = pb.y; p[6] = pb.z; p[7] = pb.w;
+            }
             float (&gg)[8] = g[u];
             if (P.add_stash) {
                 const float4* s4 = reinterpret_cast<const float4*>(P.stash + i);
@@ -381,9 +417,10 @@ __global__ void __launch_bounds__(round_threads<MODE, kSmall>(), (MODE == 2 || k
                 m[j] = m[j] + (1.f - b1) * (gj - m[j]);                 // lerp, as torch
                 vv[j] = b2 * vv[j] + (1.f - b2) * gj * gj;
                 const float denom = sqrtf(vv[j]) * P.bc2_rsqrt + eps;
-                p[j] = p[j] * decay - step_size * (m[j] / denom);
+                if constexpr (kNoDecay) gg[j] = step_size * (m[j] / denom);
+                else p[j] = p[j] * decay - step_size * (m[j] / denom);
             }
-            if (cp) {
+            if (!kNoDecay && cp) {
                 float4* o = reinterpret_cast<float4*>(P.master + i);
                 o[0] = make_float4(p[0], p[1], p[2], p[3]);
                 o[1] = make_float4(p[4], p[5], p[6], p[7]);
@@ -395,6 +432,20 @@ __global__ void __launch_bounds__(round_threads<MODE, kSmall>(), (MODE == 2 || k
                 om[1] = make_float4(m[4], m[5], m[6], m[7]);
                 ov[0] = make_float4(vv[0], vv[1], vv[2], vv[3]);
                 ov[1] = make_float4(vv[4], vv[5], vv[6], vv[7]);
+            }
+            if constexpr (kNoDecay) {
+                // The lookup and the master load run once the moments are stored, in the registers those held: the instantiations
+                // that overlap compute (<= 64 registers) have none to spare.
+                const unsigned keep = nodecay_mask(P, P.nodecay_base + i);
+                const float4 pa = p4[0], pb = p4[1];
+                p[0] = pa.x; p[1] = pa.y; p[2] = pa.z; p[3] = pa.w; p[4] = pb.x; p[5] = pb.y; p[6] = pb.z; p[7] = pb.w;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) p[j] = p[j] * (((keep >> j) & 1u) ? 1.f : decay) - gg[j];
+                if (cp) {
+                    float4* o = reinterpret_cast<float4*>(P.master + i);
+                    o[0] = make_float4(p[0], p[1], p[2], p[3]);
+                    o[1] = make_float4(p[4], p[5], p[6], p[7]);
+                }
             }
             store_param8<O, MODE>(P, base + i, p, MODE != 0 && P.n_skip > 0 && in_skip(P, base + i));
         }
@@ -531,11 +582,11 @@ __global__ void __launch_bounds__(kNormThreads, MODE == 1 ? 2 : 4) round_norm_ke
 // re-partitioned between L1 and shared memory when it is idle, so a kernel that prefers another carve-out can never be co-resident with
 // them - it waits for the SM to drain (tools/coresidency_check.py checks this).
 // Ask for the same configuration.
-template <typename G, typename O, int MODE>
+template <typename G, typename O, int MODE, bool kNoDecay>
 static void prefer_max_smem_carveout() {
     static bool done = false;
     if (!done) {
-        cudaFuncSetAttribute(rs_adam_ag_kernel<G, O, MODE>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(rs_adam_ag_kernel<G, O, MODE, false, kNoDecay>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         done = true;
     }
 }
@@ -545,27 +596,33 @@ static bool local_small() {
     return on;
 }
 
-template <typename G, typename O>
-static void launch_mode(const RoundParams& P, int mode, int grid, cudaStream_t st) {
-    if (mode == 1) prefer_max_smem_carveout<G, O, 1>();
-    else if (mode == 2) prefer_max_smem_carveout<G, O, 2>();
+template <typename G, typename O, bool kNoDecay>
+static void launch_instance(const RoundParams& P, int mode, int grid, cudaStream_t st) {
+    if (mode == 1) prefer_max_smem_carveout<G, O, 1, kNoDecay>();
+    else if (mode == 2) prefer_max_smem_carveout<G, O, 2, kNoDecay>();
     if (mode == 0 && local_small()) {
         static bool attr = false;
         static int sms = 0;
         if (!attr) {
-            cudaFuncSetAttribute(rs_adam_ag_kernel<G, O, 0, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+            cudaFuncSetAttribute(rs_adam_ag_kernel<G, O, 0, true, kNoDecay>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
             int dev = 0;
             cudaGetDevice(&dev);
             cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
             attr = true;
         }
         if (sms > 0 && grid > sms) grid = sms;           // one 256-thread CTA per SM, like the NVLS rounds
-        rs_adam_ag_kernel<G, O, 0, true><<<grid, round_threads<0, true>(), 0, st>>>(P);
+        rs_adam_ag_kernel<G, O, 0, true, kNoDecay><<<grid, round_threads<0, true>(), 0, st>>>(P);
         return;
     }
-    if (mode == 0) rs_adam_ag_kernel<G, O, 0><<<grid, round_threads<0>(), 0, st>>>(P);
-    else if (mode == 1) rs_adam_ag_kernel<G, O, 1><<<grid, round_threads<1>(), 0, st>>>(P);
-    else rs_adam_ag_kernel<G, O, 2><<<grid, round_threads<2>(), 0, st>>>(P);
+    if (mode == 0) rs_adam_ag_kernel<G, O, 0, false, kNoDecay><<<grid, round_threads<0>(), 0, st>>>(P);
+    else if (mode == 1) rs_adam_ag_kernel<G, O, 1, false, kNoDecay><<<grid, round_threads<1>(), 0, st>>>(P);
+    else rs_adam_ag_kernel<G, O, 2, false, kNoDecay><<<grid, round_threads<2>(), 0, st>>>(P);
+}
+
+template <typename G, typename O>
+static void launch_mode(const RoundParams& P, int mode, int grid, cudaStream_t st) {
+    if (P.n_nodecay > 0) launch_instance<G, O, true>(P, mode, grid, st);
+    else launch_instance<G, O, false>(P, mode, grid, st);
 }
 
 static void launch_gate(const RoundParams& P, cudaStream_t st) {

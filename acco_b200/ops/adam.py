@@ -21,6 +21,16 @@ def _scratch(device) -> torch.Tensor:
     return _SCRATCH[key]
 
 
+def _no_decay_table(hp, device):
+    """``hp``'s no-decay ranges on ``device`` (``ShardedAdamW`` builds the tensor once; a hand-made ``AdamHyper`` gets it here)."""
+    if not hp.no_decay:
+        return None
+    if hp.no_decay_dev is None:
+        from ..optim import check_no_decay_ranges
+        hp.no_decay_dev = torch.tensor(check_no_decay_ranges(hp.no_decay), dtype=torch.int64, device=device).contiguous()
+    return hp.no_decay_dev
+
+
 def fused_adamw_shard(grad_sum, master, exp_avg, exp_avg_sq, stash, out, hp) -> None:
     from ..optim import adamw_shard_update_
     if not use_kernels(grad_sum, master, out, bf16_only=False) or master.numel() % 8 != 0:
@@ -31,7 +41,8 @@ def fused_adamw_shard(grad_sum, master, exp_avg, exp_avg_sq, stash, out, hp) -> 
         inv = torch.full((1,), float(inv), dtype=torch.float32, device=master.device)
     C.adamw_shard(grad_sum, master, exp_avg, exp_avg_sq, stash, out, inv.reshape(1).float(), _scratch(master.device),
                   float(hp.lr), float(hp.beta1), float(hp.beta2), float(hp.eps), float(hp.weight_decay),
-                  int(hp.step), int(hp.commit), bool(hp.add_stash), bool(hp.write_stash))
+                  int(hp.step), int(hp.commit), bool(hp.add_stash), bool(hp.write_stash), _no_decay_table(hp, master.device),
+                  int(hp.shard_base))
     count_launch("adamw_shard")
 
 

@@ -9,13 +9,15 @@ Here the state is four flat fp32 tensors of ``size_slice`` elements (``master, e
 stash``) and an update is *one* pass described by :class:`AdamHyper`:
 
     g      = (reduced_grad_sum [+ stash]) * inv_count
-    master' = master * (1 - lr*wd);  m' = lerp(m, g, 1-b1);  v' = b2*v + (1-b2) g^2
+    master' = master * decay;  m' = lerp(m, g, 1-b1);  v' = b2*v + (1-b2) g^2
+              decay = 1 inside the no-decay ranges (train key ``no_decay_1d``), 1 - lr*wd elsewhere
     master' -= lr / (1 - b1^t) * m' / (sqrt(v') / sqrt(1 - b2^t) + eps)
     out_bf16 = cast(master')                       # always produced (it is what gets all-gathered)
     master, m, v <- master', m', v'                # only if the commit flags say so
 
-which is exactly ``torch.optim.AdamW`` (decoupled weight decay, bias-corrected) - verified in
-``tests/test_optim.py``.  :func:`adamw_shard_update_` below is the plain-PyTorch implementation
+which is exactly ``torch.optim.AdamW`` (decoupled weight decay, bias-corrected; with a no-decay table, AdamW
+with a second parameter group of ``weight_decay=0``) - verified in ``tests/test_optim.py`` and
+``tests/test_no_decay.py``.  :func:`adamw_shard_update_` below is the plain-PyTorch implementation
 (CPU / gloo path and numerics oracle for the sm_90a kernel in ``csrc/rs_adam_ag.cu``).
 
 Gradient clipping (train key ``max_grad_norm``) is a scalar on ``g``, so it never touches the update
@@ -33,13 +35,13 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass
-from typing import Dict, Optional, Tuple
+from typing import Dict, Optional, Sequence, Tuple
 
 import torch
 
 from .parallel.schedule import COMMIT_ALL, COMMIT_PARAM, COMMIT_STATE
 
-__all__ = ["AdamHyper", "ShardedAdamW", "adamw_shard_update_", "clip_scale", "check_max_grad_norm"]
+__all__ = ["AdamHyper", "ShardedAdamW", "adamw_shard_update_", "clip_scale", "check_max_grad_norm", "check_no_decay_ranges"]
 
 
 @dataclass
@@ -54,6 +56,9 @@ class AdamHyper:
     commit: int = COMMIT_ALL
     add_stash: bool = False
     write_stash: bool = False
+    no_decay: Optional[Sequence[Tuple[int, int]]] = None   # sorted, disjoint [lo, hi) ranges of the flat vector updated with decay = 1
+    shard_base: int = 0      # flat index of the shard's element 0 (the ranges are global, the shard is a slice)
+    no_decay_dev: Optional[torch.Tensor] = None            # the same table as a CUDA int64 [n, 2] tensor, for the sm_90a kernel
 
 
 @torch.no_grad()
@@ -76,7 +81,13 @@ def adamw_shard_update_(
     v = exp_avg_sq * hp.beta2 + (1.0 - hp.beta2) * g * g
     bc1 = 1.0 - hp.beta1 ** hp.step
     bc2 = 1.0 - hp.beta2 ** hp.step
-    p = master * (1.0 - hp.lr * hp.weight_decay)
+    decay = 1.0 - hp.lr * hp.weight_decay
+    if hp.no_decay:
+        S = master.numel()
+        decay = torch.full_like(master, decay)
+        for lo, hi in hp.no_decay:
+            decay[max(lo - hp.shard_base, 0):max(min(hi - hp.shard_base, S), 0)] = 1.0
+    p = master * decay
     denom = v.sqrt() / (bc2 ** 0.5) + hp.eps
     p = p - (hp.lr / bc1) * (m / denom)
     out.copy_(p)
@@ -99,6 +110,18 @@ def check_max_grad_norm(value) -> Optional[float]:
     return v
 
 
+def check_no_decay_ranges(ranges) -> Optional[Tuple[Tuple[int, int], ...]]:
+    """A no-decay table as the update uses it: ``None`` when empty, else ``(lo, hi)`` pairs with ``0 <= lo < hi``, sorted and
+    disjoint (the kernel searches it by bisection)."""
+    table = tuple((int(lo), int(hi)) for lo, hi in (ranges or ()))
+    prev = 0
+    for lo, hi in table:
+        if not prev <= lo < hi:
+            raise ValueError(f"no-decay ranges must be sorted, disjoint [lo, hi) pairs with lo < hi, got {list(table)}")
+        prev = hi
+    return table or None
+
+
 def clip_scale(sumsq, inv_count, max_norm: float) -> Tuple[torch.Tensor, torch.Tensor]:
     """``(norm, inv_eff)`` of a round from the global sum of squares of its gradient *sum* (fp32, 1-element tensor or float).
     ``norm = sqrt(sumsq) * inv_count``; ``inv_eff = inv_count * clamp(max_norm / (norm + 1e-6), max=1)``, the coefficient
@@ -114,7 +137,9 @@ class ShardedAdamW:
     """fp32 optimizer state for the slice ``[rank*size_slice, (rank+1)*size_slice)``."""
 
     def __init__(self, shard_init: torch.Tensor, lr: float, betas=(0.9, 0.999), eps: float = 1e-8,
-                 weight_decay: float = 0.01, allocator=None):
+                 weight_decay: float = 0.01, allocator=None, no_decay=None, shard_base: int = 0):
+        """``no_decay``: ranges of the flat parameter vector (global indices, see ``FlatArena.no_decay_ranges``) that are updated
+        without weight decay; ``shard_base``: flat index of this shard's first element."""
         S = shard_init.numel()
         dev = shard_init.device
         alloc = allocator or (lambda n, dt: torch.zeros(n, dtype=dt, device=dev))
@@ -127,6 +152,11 @@ class ShardedAdamW:
         self.base_lr = float(lr)
         self.beta1, self.beta2 = float(betas[0]), float(betas[1])
         self.eps, self.weight_decay = float(eps), float(weight_decay)
+        self.no_decay = check_no_decay_ranges(no_decay)
+        self.shard_base = int(shard_base)
+        self.no_decay_dev = None
+        if self.no_decay and dev.type == "cuda":
+            self.no_decay_dev = torch.tensor(self.no_decay, dtype=torch.int64, device=dev).contiguous()
 
     def hyper(self, lr: float, plan, inv_count) -> AdamHyper:
         """Hyper-parameters of the update for ``plan``.  ``inv_count`` is ``1 / total`` where
@@ -136,6 +166,7 @@ class ShardedAdamW:
             lr=float(lr), beta1=self.beta1, beta2=self.beta2, eps=self.eps, weight_decay=self.weight_decay,
             step=self.step + 1, inv_count=inv_count, commit=plan.commit,
             add_stash=plan.add_stash, write_stash=plan.write_stash,
+            no_decay=self.no_decay, shard_base=self.shard_base, no_decay_dev=self.no_decay_dev,
         )
 
     def after_launch(self, plan) -> None:

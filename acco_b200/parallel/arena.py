@@ -30,7 +30,7 @@ from typing import Callable, Dict, List, Optional, Tuple
 import torch
 import torch.nn as nn
 
-__all__ = ["ShardLayout", "FlatArena", "unique_parameters"]
+__all__ = ["ShardLayout", "FlatArena", "unique_parameters", "no_decay_ranges"]
 
 
 @dataclass(frozen=True)
@@ -82,6 +82,25 @@ def unique_parameters(model: nn.Module, trainable_only: bool = False) -> List[nn
             continue
         out.append(p)
     return out
+
+
+def no_decay_ranges(params: List[nn.Parameter]) -> List[Tuple[int, int]]:
+    """Sorted, disjoint ``[lo, hi)`` element ranges, inside the flat vector that packs ``params`` back to back, of the trainable
+    parameters with ``ndim <= 1`` (norm gains, biases): what train key ``no_decay_1d`` updates without weight decay.  Nothing is
+    aligned, so the bounds are arbitrary element indices, and neighbouring 1-D parameters merge into one range.  The table follows
+    from the model alone, never from the world size: each rank intersects it with its own slice, so a checkpoint carries no table
+    and an elastic resume on another world size rebuilds the same one."""
+    out: List[List[int]] = []
+    off = 0
+    for p in params:
+        n = p.numel()
+        if p.requires_grad and p.ndim <= 1 and n > 0:
+            if out and out[-1][1] == off:
+                out[-1][1] = off + n
+            else:
+                out.append([off, off + n])
+        off += n
+    return [(a, b) for a, b in out]
 
 
 Allocator = Callable[[int, torch.dtype], torch.Tensor]
@@ -190,6 +209,10 @@ class FlatArena:
             if id(p) in by_id:
                 out[name] = by_id[id(p)]
         return out
+
+    def no_decay_ranges(self) -> List[Tuple[int, int]]:
+        """:func:`no_decay_ranges` of this arena's parameters."""
+        return no_decay_ranges(self.params)
 
     def memory_bytes(self) -> int:
         return sum(t.numel() * t.element_size() for t in self.theta + self.acc)

@@ -133,7 +133,7 @@ class SymmBackend(CommBackend):
                           self.scratch, arena.layout.size_slice, self.rank, self.world, int(local_count),
                           float(lr), opt.beta1, opt.beta2, opt.eps, opt.weight_decay, opt.step + 1, int(plan.commit),
                           bool(plan.add_stash), bool(plan.write_stash), self._grad_bf16, self._out_bf16, self.mode, self.grid,
-                          self._skip, inv_eff)
+                          self._skip, inv_eff, opt.no_decay_dev)
         self._ops.count_launch("rs_adam_ag")
         if self.world > 1 and os.environ.get("ACCO_ROUND_GATE", "1") != "0":
             self._ops.count_launch("round_gate")

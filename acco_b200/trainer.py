@@ -66,6 +66,7 @@ TRAIN_DEFAULTS: Dict[str, Any] = dict(
     packing=False,                  # SFT: pack whole samples into full rows (document-masked attention, per-sample positions)
     max_grad_norm=None,             # global gradient-norm clipping of every round (.inf: log the norm only); logged as grad_norm
     fp8=False,                      # FP8 GEMMs (e4m3 / e5m2, per-tensor current scaling) for the block linears of native models (ops/fp8.py)
+    no_decay_1d=False,              # True: trainable parameters with ndim <= 1 (norm gains, biases) are updated without weight decay
 )
 
 
@@ -154,6 +155,9 @@ class DecoupledTrainer:
         self.max_grad_norm = check_max_grad_norm(self.args.max_grad_norm)
         self._grad_norm: Optional[float] = None     # pre-clip norm of the last committed round (max_grad_norm set)
         self._check_fp8()
+        if not isinstance(self.args.no_decay_1d, bool):
+            raise ValueError(f"no_decay_1d must be true or false, got {self.args.no_decay_1d!r}")
+        self.no_decay_1d = self.args.no_decay_1d
 
         self.initialize_com(env)
         self._init_writer()
@@ -401,9 +405,15 @@ class DecoupledTrainer:
     def prepare_opt(self) -> None:
         """fp32 master shard + AdamW state + LR schedule (`trainer_decoupled.py:296-315`)."""
         a = self.args
+        no_decay = self.arena.no_decay_ranges() if self.no_decay_1d else None
+        if self.no_decay_1d and self.rank == 0:
+            excluded = [p for p in self.arena.params if p.requires_grad and p.ndim <= 1]
+            self.log.info(f">>> no_decay_1d: {len(excluded)} parameters ({sum(p.numel() for p in excluded)} elements, "
+                          f"{len(no_decay)} ranges of the flat vector) are updated without weight decay")
         self.sharded_optimizer = ShardedAdamW(
             self.arena.shard(self.arena.theta[0]), lr=float(a.learning_rate),
-            betas=(float(a.adam_beta1), float(a.adam_beta2)), eps=float(a.adam_eps), weight_decay=float(a.weight_decay))
+            betas=(float(a.adam_beta1), float(a.adam_beta2)), eps=float(a.adam_eps), weight_decay=float(a.weight_decay),
+            no_decay=no_decay, shard_base=self.rank * self.size_slice)
         self.params_opt = self.sharded_optimizer.master
         self.backend.attach(self.arena, self.sharded_optimizer, self.max_grad_norm)
         self._setup_fused_ag()
@@ -479,11 +489,21 @@ class DecoupledTrainer:
         from torch.nn.parallel import DistributedDataParallel as DDP
         a = self.args
         self.ddp_model = DDP(self.model) if self.world_size > 1 or dist.is_initialized() else self.model
+        params = list(self.ddp_model.parameters())
+        if self.no_decay_1d:
+            # the two groups of the sharded update: ndim <= 1 without weight decay, the rest with it
+            excluded = [p for p in params if p.requires_grad and p.ndim <= 1]
+            ids = {id(p) for p in excluded}
+            params = [dict(params=[p for p in params if id(p) not in ids]), dict(params=excluded, weight_decay=0.0)]
+            params = [g for g in params if g["params"]]
+            if self.rank == 0:
+                self.log.info(f">>> no_decay_1d: {len(excluded)} parameters ({sum(p.numel() for p in excluded)} elements) "
+                              f"are updated without weight decay")
         self.optimizer = ZeroRedundancyOptimizer(
-            self.ddp_model.parameters(), optimizer_class=torch.optim.AdamW, lr=float(a.learning_rate),
+            params, optimizer_class=torch.optim.AdamW, lr=float(a.learning_rate),
             weight_decay=float(a.weight_decay), betas=(float(a.adam_beta1), float(a.adam_beta2))) \
             if dist.is_initialized() else torch.optim.AdamW(
-            self.model.parameters(), lr=float(a.learning_rate), weight_decay=float(a.weight_decay),
+            params, lr=float(a.learning_rate), weight_decay=float(a.weight_decay),
             betas=(float(a.adam_beta1), float(a.adam_beta2)))
         self.lr_schedule = LRSchedule(float(a.learning_rate), str(a.scheduler_name), int(a.warmup), self.nb_grad_tot, str(a.lr_unit))
         self.sched = RoundScheduler("ddp")

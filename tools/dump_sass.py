@@ -22,8 +22,10 @@ KERNELS = {
     "gemm_wgmma_bn256_tn.sass": "_ZN9acco_gemm11gemm_kernelILi256ELi0ELi0EEEvNS_6ParamsE",
     "gemm_wgmma_bn256_nn.sass": "_ZN9acco_gemm11gemm_kernelILi256ELi0ELi1EEEvNS_6ParamsE",
     "gemm_wgmma_bn128_tt.sass": "_ZN9acco_gemm11gemm_kernelILi128ELi1ELi1EEEvNS_6ParamsE",
-    "rs_adam_ag_multimem_bf16.sass": "_ZN4acco17rs_adam_ag_kernelI13__nv_bfloat16S1_Li2ELb0EEEvNS_11RoundParamsE",
-    "rs_adam_ag_p2p_bf16.sass": "_ZN4acco17rs_adam_ag_kernelI13__nv_bfloat16S1_Li1ELb0EEEvNS_11RoundParamsE",
+    "rs_adam_ag_multimem_bf16.sass": "_ZN4acco17rs_adam_ag_kernelI13__nv_bfloat16S1_Li2ELb0ELb0EEEvNS_11RoundParamsE",
+    "rs_adam_ag_p2p_bf16.sass": "_ZN4acco17rs_adam_ag_kernelI13__nv_bfloat16S1_Li1ELb0ELb0EEEvNS_11RoundParamsE",
+    "rs_adam_ag_multimem_bf16_nodecay.sass": "_ZN4acco17rs_adam_ag_kernelI13__nv_bfloat16S1_Li2ELb0ELb1EEEvNS_11RoundParamsE",   # no_decay_1d
+    "rs_adam_ag_local_bf16_nodecay.sass": "_ZN4acco17rs_adam_ag_kernelI13__nv_bfloat16S1_Li0ELb0ELb1EEEvNS_11RoundParamsE",
     "round_gate.sass": "_ZN4acco17round_gate_kernelENS_11RoundParamsE",
     "round_norm_multimem_bf16.sass": "_ZN4acco17round_norm_kernelI13__nv_bfloat16Li2EEEvNS_11RoundParamsEPff",   # max_grad_norm
     "round_norm_local_bf16.sass": "_ZN4acco17round_norm_kernelI13__nv_bfloat16Li0EEEvNS_11RoundParamsEPff",

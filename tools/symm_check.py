@@ -9,6 +9,7 @@ BOTH backends, and after every round checks: identical global counts; fp32 maste
 stash agree with the NCCL+fused-local-AdamW path within bf16-reduction tolerance; the gathered
 parameters are bit-identical on all ranks; the consumed accumulator is zero.  Then it times the
 round (CUDA events, max over ranks) and reports achieved NVLink bytes/s and the HBM floor.
+``--no-decay`` runs the same checks with a no-decay table (train key ``no_decay_1d``) whose ranges straddle every rank boundary.
 """
 import argparse
 import json
@@ -36,6 +37,28 @@ class Flat(nn.Module):
         self.w = nn.Parameter(torch.empty(n))
 
 
+def straddling_ranges(layout):
+    """A no-decay table for the checks: a range across every rank boundary (5 elements on one side, 3 on the other), single
+    elements and short ranges at odd offsets inside every slice, the first element and the last 13 of the vector."""
+    S, n = layout.size_slice, layout.numel
+    r = [(0, 1), (n - 13, n)]
+    for k in range(layout.world):
+        b = k * S
+        if k:
+            r.append((b - 5, b + 3))
+        r += [(b + 17, b + 18), (b + 1001, b + 1024), (b + S // 2 + 3, b + S // 2 + 12)]
+    from acco_b200.parallel.symm import merge_ranges
+    return [(lo, min(hi, n)) for lo, hi in merge_ranges(r) if lo < n]
+
+
+NO_DECAY = False
+
+
+def make_opt(shard, layout, rank):
+    no_decay = straddling_ranges(layout) if NO_DECAY else None
+    return ShardedAdamW(shard, lr=1e-3, betas=(0.9, 0.95), weight_decay=0.1, no_decay=no_decay, shard_base=rank * layout.size_slice)
+
+
 def build(kind, n, env, dev, mode_env=None):
     if mode_env:
         os.environ["ACCO_SYMM_MODE"] = mode_env
@@ -50,7 +73,7 @@ def build(kind, n, env, dev, mode_env=None):
     else:
         be = TorchDistBackend(env.rank, env.world_size, dev, fused_adam=fused_adamw_shard)
     ar = FlatArena(m, env.world_size, env.rank, torch.bfloat16, dev, align=1024, allocator=be.allocator())
-    opt = ShardedAdamW(ar.shard(ar.theta[0]), lr=1e-3, betas=(0.9, 0.95), weight_decay=0.1)
+    opt = make_opt(ar.shard(ar.theta[0]), ar.layout, env.rank)
     be.attach(ar, opt)
     return be, ar, opt
 
@@ -69,11 +92,14 @@ def main():
     ap.add_argument("--bench-iters", type=int, default=10)
     ap.add_argument("--out", default=None)
     ap.add_argument("--grids", default="", help="comma list of CTA counts to sweep for the fused kernel (0 = default)")
+    ap.add_argument("--no-decay", action="store_true", help="run every round with a no-decay table that straddles the rank boundaries")
     a = ap.parse_args()
+    global NO_DECAY
+    NO_DECAY = a.no_decay
     env = init_distributed(discover_env())
     dev = torch.device("cuda", env.local_rank)
     W, rank = env.world_size, env.rank
-    report = {"world": W, "numel": a.numel, "modes": {}}
+    report = {"world": W, "numel": a.numel, "no_decay": a.no_decay, "modes": {}}
     ref_be, ref_ar, ref_opt = build("nccl", a.numel, env, dev)
     modes = ["p2p", "multimem"]
     for mode in modes:
@@ -92,7 +118,7 @@ def main():
         # which the validation plans make every round write), so master / m / v / theta must then agree to fp32 round-off on BOTH
         # transports - no "Adam amplifies a 1-ulp difference" escape hatch.  The reduced gradient itself is checked separately,
         # element-wise, against the exact fp32 sum of the ranks' bf16 gradients.
-        oracle = ShardedAdamW(ar.shard(ar.theta[0]).clone(), lr=1e-3, betas=(0.9, 0.95), weight_decay=0.1)
+        oracle = make_opt(ar.shard(ar.theta[0]).clone(), ar.layout, rank)
         oracle_stash_count = 0
         prev_stash = torch.zeros_like(opt.stash)
         for r in range(a.rounds):
