@@ -23,9 +23,9 @@ int acco_rope_qkv(void* qkv, const float* cos_t, const float* sin_t, int T, int 
 int acco_swiglu_fwd(const void* gu, void* out, long long T, int I, int sms, cudaStream_t st);
 int acco_swiglu_bwd(const void* dout, const void* gu, void* dgu, long long T, int I, int sms, cudaStream_t st);
 int acco_ce_fwd(const void* logits, const long long* labels, float* lse, float* row_loss, float* loss, float* inv_n, long long T,
-                int V, int Vp, long long ignore_index, cudaStream_t st);
+                int V, int Vp, long long ignore_index, float label_smoothing, cudaStream_t st);
 int acco_ce_bwd(void* logits, const long long* labels, const float* lse, const float* scale, long long T, int V, int Vp,
-                long long ignore_index, cudaStream_t st);
+                long long ignore_index, float label_smoothing, cudaStream_t st);
 int acco_gelu_fwd(const void* x, void* y, long long n, int sms, cudaStream_t st);
 int acco_gelu_bwd(const void* dy, const void* x, void* dx, long long n, int sms, cudaStream_t st);
 int acco_debug_occupy(unsigned long long ns, int ctas, float* sink, cudaStream_t st);
@@ -223,8 +223,13 @@ torch::Tensor swiglu_bwd(torch::Tensor dout, torch::Tensor gu) {
 }
 
 // ---------------------------------------------------------------- cross entropy
-std::vector<torch::Tensor> ce_fwd(torch::Tensor logits, torch::Tensor labels, int64_t V, int64_t ignore_index) {
+void check_label_smoothing(double eps) {
+    TORCH_CHECK(std::isfinite(eps) && eps >= 0.0 && eps <= 1.0, "label_smoothing must be finite and in [0, 1], got ", eps);
+}
+
+std::vector<torch::Tensor> ce_fwd(torch::Tensor logits, torch::Tensor labels, int64_t V, int64_t ignore_index, double label_smoothing) {
     check_bf16(logits, "logits");
+    check_label_smoothing(label_smoothing);
     TORCH_CHECK(labels.is_cuda() && labels.scalar_type() == torch::kInt64 && labels.is_contiguous(), "labels must be contiguous CUDA int64");
     const c10::cuda::CUDAGuard guard(logits.device());
     const int64_t T = logits.size(0), Vp = logits.size(1);
@@ -235,17 +240,20 @@ std::vector<torch::Tensor> ce_fwd(torch::Tensor logits, torch::Tensor labels, in
     auto loss = torch::empty({}, f32);
     auto inv_n = torch::empty({1}, f32);
     TORCH_CHECK(acco_ce_fwd(logits.data_ptr(), (const long long*)labels.data_ptr<int64_t>(), lse.data_ptr<float>(), row_loss.data_ptr<float>(),
-                            loss.data_ptr<float>(), inv_n.data_ptr<float>(), T, (int)V, (int)Vp, ignore_index, stream()) == 0,
+                            loss.data_ptr<float>(), inv_n.data_ptr<float>(), T, (int)V, (int)Vp, ignore_index, (float)label_smoothing,
+                            stream()) == 0,
                 "ce_fwd: padded vocab must be a multiple of 8 and >= V");
     return {loss, inv_n, lse};
 }
 
-void ce_bwd_inplace(torch::Tensor logits, torch::Tensor labels, torch::Tensor lse, torch::Tensor scale, int64_t V, int64_t ignore_index) {
+void ce_bwd_inplace(torch::Tensor logits, torch::Tensor labels, torch::Tensor lse, torch::Tensor scale, int64_t V, int64_t ignore_index,
+                    double label_smoothing) {
     check_bf16(logits, "logits"); check_f32(lse, "lse"); check_f32(scale, "scale");
+    check_label_smoothing(label_smoothing);
     const c10::cuda::CUDAGuard guard(logits.device());
     const int64_t T = logits.size(0), Vp = logits.size(1);
     TORCH_CHECK(acco_ce_bwd(logits.data_ptr(), (const long long*)labels.data_ptr<int64_t>(), lse.data_ptr<float>(), scale.data_ptr<float>(), T,
-                            (int)V, (int)Vp, ignore_index, stream()) == 0, "ce_bwd: bad shapes");
+                            (int)V, (int)Vp, ignore_index, (float)label_smoothing, stream()) == 0, "ce_bwd: bad shapes");
 }
 
 // ---------------------------------------------------------------- fused round kernel
@@ -620,8 +628,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("rope_pack_bwd", &rope_pack_bwd);
     m.def("swiglu_fwd", &swiglu_fwd);
     m.def("swiglu_bwd", &swiglu_bwd);
-    m.def("ce_fwd", &ce_fwd);
-    m.def("ce_bwd_inplace", &ce_bwd_inplace);
+    m.def("ce_fwd", &ce_fwd, py::arg("logits"), py::arg("labels"), py::arg("V"), py::arg("ignore_index"), py::arg("label_smoothing") = 0.0);
+    m.def("ce_bwd_inplace", &ce_bwd_inplace, py::arg("logits"), py::arg("labels"), py::arg("lse"), py::arg("scale"), py::arg("V"),
+          py::arg("ignore_index"), py::arg("label_smoothing") = 0.0);
     m.def("adamw_shard", &adamw_shard, py::arg("grad_sum"), py::arg("master"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("stash"),
           py::arg("out"), py::arg("inv_count"), py::arg("scratch"), py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"), py::arg("wd"),
           py::arg("step"), py::arg("commit"), py::arg("add_stash"), py::arg("write_stash"), py::arg("no_decay_ranges") = py::none(),

@@ -7,15 +7,23 @@
 //   ce_reduce : deterministic tree over rows -> loss (mean) and inv_n = 1 / #valid rows
 //   ce_bwd : in place  logits <- (softmax - onehot) * scale   (scale = dloss * inv_n, device scalar);
 //            ignored rows and padded columns are written as 0.
+//
+// Label smoothing (kSmooth, eps > 0; HF LabelSmoother / F.cross_entropy(label_smoothing=eps) over the V valid columns):
+//   row_loss = lse - (1 - eps) x[label] - (eps / V) sum_{c<V} x_c,   d = (softmax - (1 - eps) onehot - eps / V) * scale.
+// The forward adds the row sum of x to the same streaming pass and one more block reduction; `one_m_eps` = 1 - eps and
+// `eps_v` = eps / V are fp32 values computed on the host.  eps = 0 launches the kSmooth = false instantiations, which ignore
+// both arguments and compile to the same code as before smoothing existed.
 #include "common.cuh"
 
 namespace acco {
 
 constexpr int kCEThreads = 512;
 
+template <bool kSmooth>
 __global__ void __launch_bounds__(kCEThreads) ce_fwd_kernel(const __nv_bfloat16* __restrict__ logits,
                                                             const long long* __restrict__ labels, float* __restrict__ lse_out,
-                                                            float* __restrict__ row_loss, int V, int Vp, long long ignore_index) {
+                                                            float* __restrict__ row_loss, int V, int Vp, long long ignore_index,
+                                                            float one_m_eps, float eps_v) {
     __shared__ float red[32];
     const long long row = blockIdx.x;
     const __nv_bfloat16* x = logits + row * (size_t)Vp;
@@ -29,6 +37,7 @@ __global__ void __launch_bounds__(kCEThreads) ce_fwd_kernel(const __nv_bfloat16*
     }
     const int nvec_full = V >> 3;          // vectors entirely inside the valid range
     float m = -INFINITY, s = 0.f;
+    float sx = 0.f;                        // kSmooth: running sum of the valid logits
     for (int v = threadIdx.x; v < nvec_full; v += kCEThreads) {
         float f[8];
         unpack8(ld_stream(x + 8 * v), f);
@@ -41,6 +50,12 @@ __global__ void __launch_bounds__(kCEThreads) ce_fwd_kernel(const __nv_bfloat16*
         for (int j = 0; j < 8; ++j) acc += __expf(f[j] - nm);
         s = s * __expf(m - nm) + acc;
         m = nm;
+        if constexpr (kSmooth) {
+            float ax = f[0];
+#pragma unroll
+            for (int j = 1; j < 8; ++j) ax += f[j];
+            sx += ax;
+        }
     }
     // ragged tail (V not a multiple of 8): scalar, handled by the first few threads
     for (int c = (nvec_full << 3) + threadIdx.x; c < V; c += kCEThreads) {
@@ -48,14 +63,24 @@ __global__ void __launch_bounds__(kCEThreads) ce_fwd_kernel(const __nv_bfloat16*
         const float nm = fmaxf(m, f);
         s = s * __expf(m - nm) + __expf(f - nm);
         m = nm;
+        if constexpr (kSmooth) sx += f;
     }
     const float gm = block_max(m, red);
     const float part = (m == -INFINITY) ? 0.f : s * __expf(m - gm);
     const float gs = block_sum(part, red);
-    if (threadIdx.x == 0) {
-        const float lse = gm + __logf(gs);
-        lse_out[row] = lse;
-        row_loss[row] = lse - __bfloat162float(x[label]);
+    if constexpr (kSmooth) {
+        const float gsx = block_sum(sx, red);
+        if (threadIdx.x == 0) {
+            const float lse = gm + __logf(gs);
+            lse_out[row] = lse;
+            row_loss[row] = lse - one_m_eps * __bfloat162float(x[label]) - eps_v * gsx;
+        }
+    } else {
+        if (threadIdx.x == 0) {
+            const float lse = gm + __logf(gs);
+            lse_out[row] = lse;
+            row_loss[row] = lse - __bfloat162float(x[label]);
+        }
     }
 }
 
@@ -79,9 +104,10 @@ __global__ void __launch_bounds__(1024) ce_reduce_kernel(const float* __restrict
     }
 }
 
+template <bool kSmooth>
 __global__ void __launch_bounds__(kCEThreads) ce_bwd_kernel(__nv_bfloat16* __restrict__ logits, const long long* __restrict__ labels,
                                                             const float* __restrict__ lse_in, const float* __restrict__ scale_ptr,
-                                                            int V, int Vp, long long ignore_index) {
+                                                            int V, int Vp, long long ignore_index, float one_m_eps, float eps_v) {
     const long long row = blockIdx.x;
     __nv_bfloat16* x = logits + row * (size_t)Vp;
     const long long label = labels[row];
@@ -102,9 +128,15 @@ __global__ void __launch_bounds__(kCEThreads) ce_bwd_kernel(__nv_bfloat16* __res
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             const int c = c0 + j;
-            float p = (c < V) ? __expf(f[j] - lse) : 0.f;
-            if (c == label) p -= 1.f;
-            f[j] = p * scale;
+            if constexpr (kSmooth) {
+                float p = (c < V) ? __expf(f[j] - lse) - eps_v : 0.f;
+                if (c == label) p -= one_m_eps;
+                f[j] = p * scale;
+            } else {
+                float p = (c < V) ? __expf(f[j] - lse) : 0.f;
+                if (c == label) p -= 1.f;
+                f[j] = p * scale;
+            }
         }
         st_stream(x + 8 * v, pack8(f));
     }
@@ -112,18 +144,30 @@ __global__ void __launch_bounds__(kCEThreads) ce_bwd_kernel(__nv_bfloat16* __res
 
 }  // namespace acco
 
+// `label_smoothing` in [0, 1] (checked by the binding); 0 runs the unsmoothed instantiation.
 extern "C" int acco_ce_fwd(const void* logits, const long long* labels, float* lse, float* row_loss, float* loss, float* inv_n,
-                           long long T, int V, int Vp, long long ignore_index, cudaStream_t st) {
+                           long long T, int V, int Vp, long long ignore_index, float label_smoothing, cudaStream_t st) {
     if (Vp % 8 != 0 || V > Vp) return -1;
-    acco::ce_fwd_kernel<<<(unsigned)T, acco::kCEThreads, 0, st>>>((const __nv_bfloat16*)logits, labels, lse, row_loss, V, Vp,
-                                                                  ignore_index);
+    const float one_m_eps = 1.f - label_smoothing, eps_v = label_smoothing / (float)V;
+    if (label_smoothing != 0.f)
+        acco::ce_fwd_kernel<true><<<(unsigned)T, acco::kCEThreads, 0, st>>>((const __nv_bfloat16*)logits, labels, lse, row_loss, V, Vp,
+                                                                            ignore_index, one_m_eps, eps_v);
+    else
+        acco::ce_fwd_kernel<false><<<(unsigned)T, acco::kCEThreads, 0, st>>>((const __nv_bfloat16*)logits, labels, lse, row_loss, V, Vp,
+                                                                             ignore_index, one_m_eps, eps_v);
     acco::ce_reduce_kernel<<<1, 1024, 0, st>>>(row_loss, labels, loss, inv_n, T, ignore_index);
     return 0;
 }
 
 extern "C" int acco_ce_bwd(void* logits, const long long* labels, const float* lse, const float* scale, long long T, int V, int Vp,
-                           long long ignore_index, cudaStream_t st) {
+                           long long ignore_index, float label_smoothing, cudaStream_t st) {
     if (Vp % 8 != 0 || V > Vp) return -1;
-    acco::ce_bwd_kernel<<<(unsigned)T, acco::kCEThreads, 0, st>>>((__nv_bfloat16*)logits, labels, lse, scale, V, Vp, ignore_index);
+    const float one_m_eps = 1.f - label_smoothing, eps_v = label_smoothing / (float)V;
+    if (label_smoothing != 0.f)
+        acco::ce_bwd_kernel<true><<<(unsigned)T, acco::kCEThreads, 0, st>>>((__nv_bfloat16*)logits, labels, lse, scale, V, Vp, ignore_index,
+                                                                            one_m_eps, eps_v);
+    else
+        acco::ce_bwd_kernel<false><<<(unsigned)T, acco::kCEThreads, 0, st>>>((__nv_bfloat16*)logits, labels, lse, scale, V, Vp,
+                                                                             ignore_index, one_m_eps, eps_v);
     return 0;
 }

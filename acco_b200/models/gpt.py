@@ -156,6 +156,7 @@ class GPTForCausalLM(nn.Module):
         self.transformer = _Transformer(config)
         self.lm_head = None if config.tie_word_embeddings else nn.Parameter(torch.empty(config.padded_vocab, config.hidden_size))
         self.fp8 = False         # FP8 GEMMs for the block linears of training micro-batches (train key `fp8`, ops/fp8.py)
+        self.label_smoothing = 0.0   # label smoothing of the loss when labels are given (train key `label_smoothing_factor`)
         self.reset_parameters()
 
     @torch.no_grad()
@@ -227,7 +228,7 @@ class GPTForCausalLM(nn.Module):
             return CausalLMOutput(loss=None, logits=logits.view(B, S, -1)[..., : cfg.vocab_size])
         shifted = torch.full_like(labels, -100)
         shifted[:, :-1] = labels[:, 1:]
-        loss = ops.softmax_cross_entropy(logits, shifted.reshape(T), cfg.vocab_size, -100)
+        loss = ops.softmax_cross_entropy(logits, shifted.reshape(T), cfg.vocab_size, -100, label_smoothing=self.label_smoothing)
         return CausalLMOutput(loss=loss, logits=None)
 
     # ------------------------------------------------------------------ HF-compatible checkpoints

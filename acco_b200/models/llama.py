@@ -141,6 +141,7 @@ class LlamaForCausalLM(nn.Module):
         self._ag_idx = 0
         self._ag_pending = False
         self.fp8 = False         # FP8 GEMMs for the block linears of training micro-batches (train key `fp8`, ops/fp8.py)
+        self.label_smoothing = 0.0   # label smoothing of the loss when labels are given (train key `label_smoothing_factor`)
         self.reset_parameters()
 
     # ------------------------------------------------------------------ init
@@ -230,7 +231,7 @@ class LlamaForCausalLM(nn.Module):
         # HF shift: position t predicts token t+1; the last position has no target
         shifted = torch.full_like(labels, -100)
         shifted[:, :-1] = labels[:, 1:]
-        loss = ops.softmax_cross_entropy(logits, shifted.reshape(T), cfg.vocab_size, -100)
+        loss = ops.softmax_cross_entropy(logits, shifted.reshape(T), cfg.vocab_size, -100, label_smoothing=self.label_smoothing)
         return CausalLMOutput(loss=loss, logits=None)
 
     # ------------------------------------------------------------------ HF-compatible checkpoints

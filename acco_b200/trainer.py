@@ -24,6 +24,7 @@ from __future__ import annotations
 
 import contextlib
 import logging
+import math
 import os
 import threading
 import time
@@ -155,11 +156,15 @@ class DecoupledTrainer:
         self.max_grad_norm = check_max_grad_norm(self.args.max_grad_norm)
         self._grad_norm: Optional[float] = None     # pre-clip norm of the last committed round (max_grad_norm set)
         self._check_fp8()
+        self._fused_smoothing = self._check_label_smoothing()
         if not isinstance(self.args.no_decay_1d, bool):
             raise ValueError(f"no_decay_1d must be true or false, got {self.args.no_decay_1d!r}")
         self.no_decay_1d = self.args.no_decay_1d
 
         self.initialize_com(env)
+        if self._fused_smoothing and self.rank == 0:
+            self.log.info(f">>> label_smoothing_factor={self._fused_smoothing}: smoothed inside the fused cross-entropy kernel "
+                          f"of {type(self.model).__name__} (CUDA graphs stay available)")
         self._init_writer()
         self.prepare_data()
         self._tokenize_if_needed()
@@ -312,6 +317,20 @@ class DecoupledTrainer:
         if a.fused_ag_gemm:
             raise ValueError("fp8=True cannot be combined with fused_ag_gemm: the gathering GEMM has no FP8 instantiation")
         self.model.fp8 = True
+
+    def _check_label_smoothing(self) -> float:
+        """``label_smoothing_factor`` on a native model is applied by its fused cross-entropy kernel (``model.label_smoothing``):
+        the micro-batch keeps the ``model(..., labels=...)`` path, with no fp32 copy of the logits and CUDA graphs available.
+        Every other model keeps :class:`LabelSmoother` on its logits.  Returns the factor the native model smooths with (0 if none)."""
+        eps = self.label_smoothing_factor
+        from .models import GPTForCausalLM, LlamaForCausalLM
+        if not eps or not isinstance(self.model, (LlamaForCausalLM, GPTForCausalLM)):
+            return 0.0
+        if isinstance(eps, bool) or not isinstance(eps, (int, float)) or not math.isfinite(eps) or not 0.0 <= eps <= 1.0:
+            raise ValueError(f"label_smoothing_factor must be a finite number in [0, 1], got {eps!r}")
+        self.model.label_smoothing = float(eps)
+        self.label_smoother = None
+        return float(eps)
 
     def prepare_data(self) -> None:
         """Per-rank sharding (`trainer_base.py:183-200`)."""
@@ -515,6 +534,13 @@ class DecoupledTrainer:
             return self.compute_loss(model, dict(inputs))
         if "labels" in inputs:
             out = model(**inputs)
+        elif self._fused_smoothing:
+            # a batch without labels is scored on its own tokens unsmoothed, as on the LabelSmoother route (it smooths labels only)
+            self.model.label_smoothing = 0.0
+            try:
+                out = model(**inputs, labels=inputs["input_ids"])
+            finally:
+                self.model.label_smoothing = self._fused_smoothing
         else:
             out = model(**inputs, labels=inputs["input_ids"])
         return out["loss"] if isinstance(out, dict) else out[0]
@@ -536,7 +562,8 @@ class DecoupledTrainer:
         return self._prepare_input(inputs)
 
     def compute_loss(self, model, inputs, return_outputs: bool = False):
-        """Loss with optional label smoothing (`trainer_base.py:262-282`)."""
+        """Loss with optional label smoothing (`trainer_base.py:262-282`): through :class:`LabelSmoother`, or, for a native model,
+        inside the model's fused cross-entropy (``model.label_smoothing``, set at construction)."""
         labels = inputs.pop("labels") if (self.label_smoother is not None and "labels" in inputs) else None
         outputs = model(**inputs)
         if labels is not None:
