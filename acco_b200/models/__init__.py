@@ -8,11 +8,12 @@ import json
 import os
 from typing import Any, Mapping
 
+from .base import NativeCausalLM, NativeConfig
 from .gpt import GPTConfig, GPTForCausalLM
 from .llama import LlamaConfig, LlamaForCausalLM
 from .output import CausalLMOutput
 
-__all__ = ["LlamaConfig", "LlamaForCausalLM", "GPTConfig", "GPTForCausalLM", "CausalLMOutput",
+__all__ = ["NativeConfig", "NativeCausalLM", "LlamaConfig", "LlamaForCausalLM", "GPTConfig", "GPTForCausalLM", "CausalLMOutput",
            "build_model", "PRESETS", "preset", "from_pretrained", "load_hf_state_dict"]
 
 PRESETS = {

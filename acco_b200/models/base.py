@@ -1,0 +1,127 @@
+"""What the native Llama and GPT-Neo models share: config helpers, the training switches, initialisation, the loss tail and
+the HF checkpoint format.
+
+Each model describes its checkpoint once, as a table of ``(HF key, view of the live parameter)`` pairs (``_hf_tensors``);
+``state_dict()`` and ``load_state_dict()`` both walk that table, so saving and loading cannot drift apart."""
+from __future__ import annotations
+
+from collections import OrderedDict
+from dataclasses import asdict
+from typing import Any, Dict, List, Optional, Tuple
+
+import torch
+import torch.nn as nn
+
+from .. import ops
+from .output import CausalLMOutput
+
+__all__ = ["NativeConfig", "NativeCausalLM"]
+
+
+class NativeConfig:
+    """Mixin for the config dataclasses (``vocab_size``, ``hidden_size``, ``num_attention_heads``, ``pad_vocab_multiple``)."""
+
+    @property
+    def head_dim(self) -> int:
+        return self.hidden_size // self.num_attention_heads
+
+    @property
+    def padded_vocab(self) -> int:
+        m = max(int(self.pad_vocab_multiple), 1)
+        return ((self.vocab_size + m - 1) // m) * m
+
+    def to_dict(self) -> Dict[str, Any]:
+        return asdict(self)
+
+    @classmethod
+    def from_dict(cls, d: Dict[str, Any]):
+        """Build from a mapping, ignoring keys that are not fields (HF ``config.json`` carries many)."""
+        keys = cls.__dataclass_fields__.keys()
+        return cls(**{k: v for k, v in dict(d).items() if k in keys})
+
+
+class NativeCausalLM(nn.Module):
+    """Base of the native causal LMs.  A subclass registers its parameters, including ``lm_head`` (``None`` when the head is
+    tied to the input embedding), then calls :meth:`reset_parameters`.  It provides ``embed_weight``, ``_init_fill``,
+    ``_hf_tensors`` and ``_hf_ignored_suffixes``.  This class registers no parameter, buffer or submodule."""
+
+    _hf_ignored_suffixes: Tuple[str, ...] = ()      # checkpoint keys ending so are never reported as unexpected
+
+    def __init__(self, config):
+        super().__init__()
+        self.config = config
+        self.fp8 = False             # FP8 GEMMs for the block linears of training micro-batches (train key `fp8`, ops/fp8.py)
+        self.label_smoothing = 0.0   # label smoothing of the loss when labels are given (train key `label_smoothing_factor`)
+
+    @property
+    def embed_weight(self) -> torch.Tensor:
+        raise NotImplementedError
+
+    @property
+    def head_weight(self) -> torch.Tensor:
+        return self.embed_weight if self.lm_head is None else self.lm_head
+
+    # ------------------------------------------------------------------ init
+    def _init_fill(self, name: str) -> Optional[float]:
+        """The constant parameter ``name`` starts at, or None to draw it from N(0, initializer_range)."""
+        raise NotImplementedError
+
+    @torch.no_grad()
+    def reset_parameters(self) -> None:
+        std = self.config.initializer_range
+        for name, p in self.named_parameters():
+            fill = self._init_fill(name)
+            if fill is None:
+                p.normal_(0.0, std)
+            else:
+                p.fill_(fill)
+        # alignment padding rows of the vocabulary are exactly zero and stay zero
+        V = self.config.vocab_size
+        self.embed_weight[V:].zero_()
+        if self.lm_head is not None:
+            self.lm_head[V:].zero_()
+
+    # ------------------------------------------------------------------ loss
+    def _lm_output(self, logits: torch.Tensor, labels: Optional[torch.Tensor], B: int, S: int) -> CausalLMOutput:
+        """Logits ``[B*S, Vp]`` -> the logits cut to ``vocab_size`` without labels, else the mean cross-entropy loss."""
+        V = self.config.vocab_size
+        if labels is None:
+            return CausalLMOutput(loss=None, logits=logits.view(B, S, -1)[..., :V])
+        # HF shift: position t predicts token t+1; the last position has no target
+        shifted = torch.full_like(labels, -100)
+        shifted[:, :-1] = labels[:, 1:]
+        loss = ops.softmax_cross_entropy(logits, shifted.reshape(B * S), V, -100, label_smoothing=self.label_smoothing)
+        return CausalLMOutput(loss=loss, logits=None)
+
+    # ------------------------------------------------------------------ HF-compatible checkpoints
+    def _hf_tensors(self) -> List[Tuple[str, torch.Tensor]]:
+        """``(HF key, view of the live parameter)`` in checkpoint order, with HF shapes (fused weights split, vocabulary padding
+        removed) and ``lm_head.weight`` last."""
+        raise NotImplementedError
+
+    def state_dict(self, *args, destination=None, prefix: str = "", keep_vars: bool = False, **kw):
+        """HF key names and shapes.  The tensors are views of the live parameters (hence of the flat arena), like the
+        reference's checkpoints (`trainer_decoupled.py:568-573`)."""
+        sd = destination if destination is not None else OrderedDict()
+        for key, t in self._hf_tensors():
+            sd[prefix + key] = t if keep_vars else t.detach()
+        return sd
+
+    @torch.no_grad()
+    def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):
+        """Copy an HF-keyed state dict into the parameters.  A tied head takes its weights from the embedding, so it neither
+        needs nor reports ``lm_head.weight``."""
+        sd = dict(state_dict)
+        used, missing = set(), []
+        for key, dst in self._hf_tensors():
+            if key == "lm_head.weight" and self.lm_head is None:
+                used.add(key)
+            elif key in sd:
+                used.add(key)
+                dst.copy_(sd[key].to(dst.dtype))
+            else:
+                missing.append(key)
+        unexpected = [k for k in sd if k not in used and not k.endswith(self._hf_ignored_suffixes)]
+        if strict and (missing or unexpected):
+            raise RuntimeError(f"load_state_dict: missing={missing[:5]} unexpected={unexpected[:5]}")
+        return torch.nn.modules.module._IncompatibleKeys(missing, unexpected)

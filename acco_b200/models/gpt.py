@@ -18,21 +18,21 @@ HF GPT-Neo key names (``transformer.h.N.attn.attention.q_proj.weight`` ...) and 
 from __future__ import annotations
 
 import math
-from collections import OrderedDict
-from dataclasses import dataclass, asdict
-from typing import Any, Dict, List, Optional
+from dataclasses import dataclass
+from typing import Any, Dict, List, Optional, Tuple
 
 import torch
 import torch.nn as nn
 
 from .. import ops
+from .base import NativeCausalLM, NativeConfig
 from .output import CausalLMOutput
 
 __all__ = ["GPTConfig", "GPTForCausalLM"]
 
 
 @dataclass
-class GPTConfig:
+class GPTConfig(NativeConfig):
     vocab_size: int = 50257
     hidden_size: int = 768
     num_hidden_layers: int = 12
@@ -60,18 +60,6 @@ class GPTConfig:
                 raise ValueError("attention_layers must be 'global', 'alternating' or a list")
         assert len(self.attention_layers) == self.num_hidden_layers
 
-    @property
-    def head_dim(self) -> int:
-        return self.hidden_size // self.num_attention_heads
-
-    @property
-    def padded_vocab(self) -> int:
-        m = max(int(self.pad_vocab_multiple), 1)
-        return ((self.vocab_size + m - 1) // m) * m
-
-    def to_dict(self) -> Dict[str, Any]:
-        return asdict(self)
-
     @classmethod
     def from_dict(cls, d: Dict[str, Any]) -> "GPTConfig":
         d = dict(d)
@@ -85,8 +73,7 @@ class GPTConfig:
             for kinds, rep in d["attention_types"]:
                 layers.extend(list(kinds) * int(rep))
             d["attention_layers"] = layers
-        keys = cls.__dataclass_fields__.keys()
-        return cls(**{k: v for k, v in d.items() if k in keys})
+        return super().from_dict(d)
 
     def flops_per_token(self, seq_len: int) -> float:
         H, I, L = self.hidden_size, self.intermediate_size, self.num_hidden_layers
@@ -149,35 +136,23 @@ class _Transformer(nn.Module):
         self.ln_f = _LN(cfg.hidden_size)
 
 
-class GPTForCausalLM(nn.Module):
+class GPTForCausalLM(NativeCausalLM):
+    _hf_ignored_suffixes = (".attn.attention.bias", "masked_bias")      # HF's causal-mask buffers
+
     def __init__(self, config: GPTConfig):
-        super().__init__()
-        self.config = config
+        super().__init__(config)
         self.transformer = _Transformer(config)
         self.lm_head = None if config.tie_word_embeddings else nn.Parameter(torch.empty(config.padded_vocab, config.hidden_size))
-        self.fp8 = False         # FP8 GEMMs for the block linears of training micro-batches (train key `fp8`, ops/fp8.py)
-        self.label_smoothing = 0.0   # label smoothing of the loss when labels are given (train key `label_smoothing_factor`)
         self.reset_parameters()
 
-    @torch.no_grad()
-    def reset_parameters(self) -> None:
-        std = self.config.initializer_range
-        V = self.config.vocab_size
-        for name, p in self.named_parameters():
-            if name.endswith("bias"):
-                p.zero_()
-            elif ".ln_" in name or name.endswith("ln_f.weight"):
-                p.fill_(1.0)
-            else:
-                p.normal_(0.0, std)
-        # alignment padding rows of the vocabulary are exactly zero and stay zero
-        self.transformer.wte[V:].zero_()
-        if self.lm_head is not None:
-            self.lm_head[V:].zero_()
+    def _init_fill(self, name: str) -> Optional[float]:
+        if name.endswith("bias"):
+            return 0.0
+        return 1.0 if ".ln_" in name else None
 
     @property
-    def head_weight(self) -> torch.Tensor:
-        return self.transformer.wte if self.lm_head is None else self.lm_head
+    def embed_weight(self) -> torch.Tensor:
+        return self.transformer.wte
 
     def num_parameters(self, padded: bool = False) -> int:
         n = sum(p.numel() for p in self.parameters())
@@ -224,74 +199,23 @@ class GPTForCausalLM(nn.Module):
         else:
             n, h = ops.add_layernorm(branch, h, tr.ln_f.weight, tr.ln_f.bias, eps)
         logits = ops.linear(n, self.head_weight)                                                  # [T, Vp]
-        if labels is None:
-            return CausalLMOutput(loss=None, logits=logits.view(B, S, -1)[..., : cfg.vocab_size])
-        shifted = torch.full_like(labels, -100)
-        shifted[:, :-1] = labels[:, 1:]
-        loss = ops.softmax_cross_entropy(logits, shifted.reshape(T), cfg.vocab_size, -100, label_smoothing=self.label_smoothing)
-        return CausalLMOutput(loss=loss, logits=None)
+        return self._lm_output(logits, labels, B, S)
 
-    # ------------------------------------------------------------------ HF-compatible checkpoints
-    def state_dict(self, *args, destination=None, prefix: str = "", keep_vars: bool = False, **kw):
-        """HF ``GPTNeoForCausalLM`` key names and shapes (fused QKV split, vocab padding removed); the tensors are views of the
-        live parameters (hence of the flat arena)."""
-        cfg = self.config
-        H, V = cfg.hidden_size, cfg.vocab_size
-        get = (lambda p: p) if keep_vars else (lambda p: p.detach())
-        sd = destination if destination is not None else OrderedDict()
+    def _hf_tensors(self) -> List[Tuple[str, torch.Tensor]]:
+        """HF ``GPTNeoForCausalLM`` keys: the fused QKV weight is split back into HF's three projections."""
+        H, V = self.config.hidden_size, self.config.vocab_size
         tr = self.transformer
-        sd[prefix + "transformer.wte.weight"] = get(tr.wte)[:V]
-        sd[prefix + "transformer.wpe.weight"] = get(tr.wpe)
+        t = [("transformer.wte.weight", tr.wte[:V]), ("transformer.wpe.weight", tr.wpe)]
         for i, blk in enumerate(tr.h):
-            b = f"{prefix}transformer.h.{i}."
-            a = blk.attn.attention
-            qkv = get(a.qkv_proj)
-            sd[b + "ln_1.weight"], sd[b + "ln_1.bias"] = get(blk.ln_1.weight), get(blk.ln_1.bias)
-            sd[b + "attn.attention.q_proj.weight"] = qkv[:H]
-            sd[b + "attn.attention.k_proj.weight"] = qkv[H:2 * H]
-            sd[b + "attn.attention.v_proj.weight"] = qkv[2 * H:]
-            sd[b + "attn.attention.out_proj.weight"], sd[b + "attn.attention.out_proj.bias"] = get(a.out_proj.weight), get(a.out_proj.bias)
-            sd[b + "ln_2.weight"], sd[b + "ln_2.bias"] = get(blk.ln_2.weight), get(blk.ln_2.bias)
-            sd[b + "mlp.c_fc.weight"], sd[b + "mlp.c_fc.bias"] = get(blk.mlp.c_fc.weight), get(blk.mlp.c_fc.bias)
-            sd[b + "mlp.c_proj.weight"], sd[b + "mlp.c_proj.bias"] = get(blk.mlp.c_proj.weight), get(blk.mlp.c_proj.bias)
-        sd[prefix + "transformer.ln_f.weight"], sd[prefix + "transformer.ln_f.bias"] = get(tr.ln_f.weight), get(tr.ln_f.bias)
-        sd[prefix + "lm_head.weight"] = get(self.head_weight)[:V]
-        return sd
-
-    @torch.no_grad()
-    def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):
-        cfg = self.config
-        H, V = cfg.hidden_size, cfg.vocab_size
-        sd = {k: v for k, v in dict(state_dict).items() if not k.endswith(".attn.attention.bias") and not k.endswith("masked_bias")}
-        used, missing = set(), []
-
-        def put(dst: torch.Tensor, name: str):
-            if name in sd:
-                used.add(name)
-                dst.copy_(sd[name].to(dst.dtype))
-            else:
-                missing.append(name)
-
-        tr = self.transformer
-        put(tr.wte[:V], "transformer.wte.weight")
-        put(tr.wpe, "transformer.wpe.weight")
-        for i, blk in enumerate(tr.h):
-            b = f"transformer.h.{i}."
-            a = blk.attn.attention
-            put(blk.ln_1.weight, b + "ln_1.weight"), put(blk.ln_1.bias, b + "ln_1.bias")
-            put(a.qkv_proj[:H], b + "attn.attention.q_proj.weight")
-            put(a.qkv_proj[H:2 * H], b + "attn.attention.k_proj.weight")
-            put(a.qkv_proj[2 * H:], b + "attn.attention.v_proj.weight")
-            put(a.out_proj.weight, b + "attn.attention.out_proj.weight"), put(a.out_proj.bias, b + "attn.attention.out_proj.bias")
-            put(blk.ln_2.weight, b + "ln_2.weight"), put(blk.ln_2.bias, b + "ln_2.bias")
-            put(blk.mlp.c_fc.weight, b + "mlp.c_fc.weight"), put(blk.mlp.c_fc.bias, b + "mlp.c_fc.bias")
-            put(blk.mlp.c_proj.weight, b + "mlp.c_proj.weight"), put(blk.mlp.c_proj.bias, b + "mlp.c_proj.bias")
-        put(tr.ln_f.weight, "transformer.ln_f.weight"), put(tr.ln_f.bias, "transformer.ln_f.bias")
-        if self.lm_head is not None:
-            put(self.lm_head[:V], "lm_head.weight")
-        elif "lm_head.weight" in sd:
-            used.add("lm_head.weight")
-        unexpected = [k for k in sd if k not in used]
-        if strict and (missing or unexpected):
-            raise RuntimeError(f"load_state_dict: missing={missing[:5]} unexpected={unexpected[:5]}")
-        return torch.nn.modules.module._IncompatibleKeys(missing, unexpected)
+            b, a, mlp = f"transformer.h.{i}.", blk.attn.attention, blk.mlp
+            t += [(b + "ln_1.weight", blk.ln_1.weight), (b + "ln_1.bias", blk.ln_1.bias),
+                  (b + "attn.attention.q_proj.weight", a.qkv_proj[:H]),
+                  (b + "attn.attention.k_proj.weight", a.qkv_proj[H:2 * H]),
+                  (b + "attn.attention.v_proj.weight", a.qkv_proj[2 * H:]),
+                  (b + "attn.attention.out_proj.weight", a.out_proj.weight), (b + "attn.attention.out_proj.bias", a.out_proj.bias),
+                  (b + "ln_2.weight", blk.ln_2.weight), (b + "ln_2.bias", blk.ln_2.bias),
+                  (b + "mlp.c_fc.weight", mlp.c_fc.weight), (b + "mlp.c_fc.bias", mlp.c_fc.bias),
+                  (b + "mlp.c_proj.weight", mlp.c_proj.weight), (b + "mlp.c_proj.bias", mlp.c_proj.bias)]
+        t += [("transformer.ln_f.weight", tr.ln_f.weight), ("transformer.ln_f.bias", tr.ln_f.bias),
+              ("lm_head.weight", self.head_weight[:V])]
+        return t

@@ -16,21 +16,21 @@ but is laid out for the GPU kernel path:
 """
 from __future__ import annotations
 
-from collections import OrderedDict
-from dataclasses import dataclass, asdict
-from typing import Any, Dict, Optional
+from dataclasses import dataclass
+from typing import Any, Dict, List, Optional, Tuple
 
 import torch
 import torch.nn as nn
 
 from .. import ops
+from .base import NativeCausalLM, NativeConfig
 from .output import CausalLMOutput
 
 __all__ = ["LlamaConfig", "LlamaForCausalLM"]
 
 
 @dataclass
-class LlamaConfig:
+class LlamaConfig(NativeConfig):
     vocab_size: int = 50257
     hidden_size: int = 768
     intermediate_size: int = 2048
@@ -51,23 +51,6 @@ class LlamaConfig:
             self.num_key_value_heads = self.num_attention_heads
         assert self.hidden_size % self.num_attention_heads == 0
         assert self.num_attention_heads % self.num_key_value_heads == 0
-
-    @property
-    def head_dim(self) -> int:
-        return self.hidden_size // self.num_attention_heads
-
-    @property
-    def padded_vocab(self) -> int:
-        m = max(int(self.pad_vocab_multiple), 1)
-        return ((self.vocab_size + m - 1) // m) * m
-
-    def to_dict(self) -> Dict[str, Any]:
-        return asdict(self)
-
-    @classmethod
-    def from_dict(cls, d: Dict[str, Any]) -> "LlamaConfig":
-        keys = cls.__dataclass_fields__.keys()
-        return cls(**{k: v for k, v in dict(d).items() if k in keys})
 
     def num_parameters(self, padded: bool = False) -> int:
         H, I, L = self.hidden_size, self.intermediate_size, self.num_hidden_layers
@@ -126,10 +109,11 @@ class _Body(nn.Module):
         self.norm = _Norm(cfg.hidden_size)
 
 
-class LlamaForCausalLM(nn.Module):
+class LlamaForCausalLM(NativeCausalLM):
+    _hf_ignored_suffixes = ("rotary_emb.inv_freq",)
+
     def __init__(self, config: LlamaConfig):
-        super().__init__()
-        self.config = config
+        super().__init__(config)
         self.model = _Body(config)
         if config.tie_word_embeddings:
             self.lm_head = None
@@ -140,28 +124,14 @@ class LlamaForCausalLM(nn.Module):
         self._ag_table: Dict[int, Any] = {}
         self._ag_idx = 0
         self._ag_pending = False
-        self.fp8 = False         # FP8 GEMMs for the block linears of training micro-batches (train key `fp8`, ops/fp8.py)
-        self.label_smoothing = 0.0   # label smoothing of the loss when labels are given (train key `label_smoothing_factor`)
         self.reset_parameters()
 
-    # ------------------------------------------------------------------ init
-    @torch.no_grad()
-    def reset_parameters(self) -> None:
-        std = self.config.initializer_range
-        V = self.config.vocab_size
-        for name, p in self.named_parameters():
-            if name.endswith("layernorm.weight") or name.endswith("norm.weight"):
-                p.fill_(1.0)
-            else:
-                p.normal_(0.0, std)
-        # alignment padding rows of the vocabulary are exactly zero and stay zero
-        self.model.embed_tokens[V:].zero_()
-        if self.lm_head is not None:
-            self.lm_head[V:].zero_()
+    def _init_fill(self, name: str) -> Optional[float]:
+        return 1.0 if name.endswith("norm.weight") else None
 
     @property
-    def head_weight(self) -> torch.Tensor:
-        return self.model.embed_tokens if self.lm_head is None else self.lm_head
+    def embed_weight(self) -> torch.Tensor:
+        return self.model.embed_tokens
 
     def num_parameters(self) -> int:
         return sum(p.numel() for p in self.parameters())
@@ -226,79 +196,24 @@ class LlamaForCausalLM(nn.Module):
         else:
             n, h = ops.add_rmsnorm(branch, h, self.model.norm.weight, eps)
         logits = ops.linear(n, self.head_weight, gathered=self._gw(self.head_weight) if self.lm_head is not None else None)   # [T, Vp]
-        if labels is None:
-            return CausalLMOutput(loss=None, logits=logits.view(B, S, -1)[..., : cfg.vocab_size])
-        # HF shift: position t predicts token t+1; the last position has no target
-        shifted = torch.full_like(labels, -100)
-        shifted[:, :-1] = labels[:, 1:]
-        loss = ops.softmax_cross_entropy(logits, shifted.reshape(T), cfg.vocab_size, -100, label_smoothing=self.label_smoothing)
-        return CausalLMOutput(loss=loss, logits=None)
+        return self._lm_output(logits, labels, B, S)
 
-    # ------------------------------------------------------------------ HF-compatible checkpoints
-    def state_dict(self, *args, destination=None, prefix: str = "", keep_vars: bool = False, **kw):
-        """HF ``LlamaForCausalLM`` key names and shapes (fused weights split, vocab padding removed).
-        The tensors are views of the live parameters (hence of the flat arena), like the
-        reference's checkpoints (`trainer_decoupled.py:568-573`)."""
+    def _hf_tensors(self) -> List[Tuple[str, torch.Tensor]]:
+        """HF ``LlamaForCausalLM`` keys: the fused QKV and gate|up weights are split back into HF's projections."""
         cfg = self.config
         D, Hq, Hk, V, I = cfg.head_dim, cfg.num_attention_heads, cfg.num_key_value_heads, cfg.vocab_size, cfg.intermediate_size
-        get = (lambda p: p) if keep_vars else (lambda p: p.detach())
-        sd = destination if destination is not None else OrderedDict()
-        sd[prefix + "model.embed_tokens.weight"] = get(self.model.embed_tokens)[:V]
-        for i, layer in enumerate(self.model.layers):
-            base = f"{prefix}model.layers.{i}."
-            qkv = get(layer.self_attn.qkv_proj)
-            sd[base + "self_attn.q_proj.weight"] = qkv[: Hq * D]
-            sd[base + "self_attn.k_proj.weight"] = qkv[Hq * D: (Hq + Hk) * D]
-            sd[base + "self_attn.v_proj.weight"] = qkv[(Hq + Hk) * D:]
-            sd[base + "self_attn.o_proj.weight"] = get(layer.self_attn.o_proj)
-            gu = get(layer.mlp.gate_up_proj)
-            sd[base + "mlp.gate_proj.weight"] = gu[:I]
-            sd[base + "mlp.up_proj.weight"] = gu[I:]
-            sd[base + "mlp.down_proj.weight"] = get(layer.mlp.down_proj)
-            sd[base + "input_layernorm.weight"] = get(layer.input_layernorm.weight)
-            sd[base + "post_attention_layernorm.weight"] = get(layer.post_attention_layernorm.weight)
-        sd[prefix + "model.norm.weight"] = get(self.model.norm.weight)
-        sd[prefix + "lm_head.weight"] = get(self.head_weight)[:V]
-        return sd
-
-    @torch.no_grad()
-    def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):
-        cfg = self.config
-        D, Hq, Hk, V, I = cfg.head_dim, cfg.num_attention_heads, cfg.num_key_value_heads, cfg.vocab_size, cfg.intermediate_size
-        sd = dict(state_dict)
-        used = set()
-
-        def take(name):
-            used.add(name)
-            return sd[name]
-
-        missing = []
-
-        def put(dst: torch.Tensor, name: str):
-            if name in sd:
-                dst.copy_(take(name).to(dst.dtype))
-            else:
-                missing.append(name)
-
-        put(self.model.embed_tokens[:V], "model.embed_tokens.weight")
+        t = [("model.embed_tokens.weight", self.model.embed_tokens[:V])]
         for i, layer in enumerate(self.model.layers):
             b = f"model.layers.{i}."
             qkv, gu = layer.self_attn.qkv_proj, layer.mlp.gate_up_proj
-            put(qkv[: Hq * D], b + "self_attn.q_proj.weight")
-            put(qkv[Hq * D: (Hq + Hk) * D], b + "self_attn.k_proj.weight")
-            put(qkv[(Hq + Hk) * D:], b + "self_attn.v_proj.weight")
-            put(layer.self_attn.o_proj, b + "self_attn.o_proj.weight")
-            put(gu[:I], b + "mlp.gate_proj.weight")
-            put(gu[I:], b + "mlp.up_proj.weight")
-            put(layer.mlp.down_proj, b + "mlp.down_proj.weight")
-            put(layer.input_layernorm.weight, b + "input_layernorm.weight")
-            put(layer.post_attention_layernorm.weight, b + "post_attention_layernorm.weight")
-        put(self.model.norm.weight, "model.norm.weight")
-        if self.lm_head is not None:
-            put(self.lm_head[:V], "lm_head.weight")
-        elif "lm_head.weight" in sd:
-            used.add("lm_head.weight")
-        unexpected = [k for k in sd if k not in used and not k.endswith("rotary_emb.inv_freq")]
-        if strict and (missing or unexpected):
-            raise RuntimeError(f"load_state_dict: missing={missing[:5]} unexpected={unexpected[:5]}")
-        return torch.nn.modules.module._IncompatibleKeys(missing, unexpected)
+            t += [(b + "self_attn.q_proj.weight", qkv[: Hq * D]),
+                  (b + "self_attn.k_proj.weight", qkv[Hq * D: (Hq + Hk) * D]),
+                  (b + "self_attn.v_proj.weight", qkv[(Hq + Hk) * D:]),
+                  (b + "self_attn.o_proj.weight", layer.self_attn.o_proj),
+                  (b + "mlp.gate_proj.weight", gu[:I]),
+                  (b + "mlp.up_proj.weight", gu[I:]),
+                  (b + "mlp.down_proj.weight", layer.mlp.down_proj),
+                  (b + "input_layernorm.weight", layer.input_layernorm.weight),
+                  (b + "post_attention_layernorm.weight", layer.post_attention_layernorm.weight)]
+        t += [("model.norm.weight", self.model.norm.weight), ("lm_head.weight", self.head_weight[:V])]
+        return t

@@ -299,8 +299,8 @@ class DecoupledTrainer:
             raise ValueError("packing=True needs const_len_batch=False: const-len pre-training rows are already full")
         if a.group_by_length:
             raise ValueError("packing=True cannot be combined with group_by_length: packed rows all have max_length tokens")
-        from .models import GPTForCausalLM, LlamaForCausalLM
-        if not isinstance(self.model, (LlamaForCausalLM, GPTForCausalLM)):
+        from .models import NativeCausalLM
+        if not isinstance(self.model, NativeCausalLM):
             raise ValueError(f"packing=True needs a native model that masks attention by position_ids; {type(self.model).__name__} "
                              "would attend across the samples of a row")
 
@@ -309,8 +309,8 @@ class DecoupledTrainer:
         a = self.args
         if not a.fp8:
             return
-        from .models import GPTForCausalLM, LlamaForCausalLM
-        if not isinstance(self.model, (LlamaForCausalLM, GPTForCausalLM)):
+        from .models import NativeCausalLM
+        if not isinstance(self.model, NativeCausalLM):
             raise ValueError(f"fp8=True needs a native model (LlamaForCausalLM / GPTForCausalLM); {type(self.model).__name__} has no FP8 path")
         if not a.use_mixed_precision or str(a.ddp_weights_dtype) == "fp32":
             raise ValueError("fp8=True quantises bf16 weights and activations: it needs use_mixed_precision=True and ddp_weights_dtype=bf16")
@@ -323,8 +323,8 @@ class DecoupledTrainer:
         the micro-batch keeps the ``model(..., labels=...)`` path, with no fp32 copy of the logits and CUDA graphs available.
         Every other model keeps :class:`LabelSmoother` on its logits.  Returns the factor the native model smooths with (0 if none)."""
         eps = self.label_smoothing_factor
-        from .models import GPTForCausalLM, LlamaForCausalLM
-        if not eps or not isinstance(self.model, (LlamaForCausalLM, GPTForCausalLM)):
+        from .models import NativeCausalLM
+        if not eps or not isinstance(self.model, NativeCausalLM):
             return 0.0
         if isinstance(eps, bool) or not isinstance(eps, (int, float)) or not math.isfinite(eps) or not 0.0 <= eps <= 1.0:
             raise ValueError(f"label_smoothing_factor must be a finite number in [0, 1], got {eps!r}")

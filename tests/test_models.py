@@ -1,3 +1,7 @@
+import json
+import os
+import re
+
 import pytest
 import torch
 
@@ -9,6 +13,82 @@ def tiny_llama(**kw):
                num_key_value_heads=2, max_position_embeddings=64, pad_vocab_multiple=16)
     cfg.update(kw)
     return LlamaForCausalLM(LlamaConfig(**cfg))
+
+
+# parameter and checkpoint layout of tiny native models ({llama, gpt_neo} x {tied, untied}): the flat arena, optimizer shards and
+# elastic resume follow named_parameters(); checkpoint files follow state_dict()
+with open(os.path.join(os.path.dirname(__file__), "golden", "native_checkpoint_layout.json")) as _f:
+    LAYOUT = json.load(_f)
+# HF buffers a checkpoint may carry that have no parameter here
+HF_BUFFERS = {"llama": ["model.layers.0.self_attn.rotary_emb.inv_freq"],
+              "gpt_neo": ["transformer.h.0.attn.attention.bias", "transformer.h.0.attn.attention.masked_bias"]}
+
+
+def native(case, seed=0):
+    cls, cfg = {"llama": (LlamaForCausalLM, LlamaConfig), "gpt_neo": (GPTForCausalLM, GPTConfig)}[case.rsplit("_", 1)[0]]
+    torch.manual_seed(seed)
+    return cls(cfg(**LAYOUT[case]["config"])).float()
+
+
+@pytest.mark.parametrize("case", list(LAYOUT))
+def test_native_layout_matches_golden(case):
+    m = native(case)
+    assert [[n, list(p.shape)] for n, p in m.named_parameters()] == LAYOUT[case]["named_parameters"]
+    assert [[k, list(v.shape)] for k, v in m.state_dict().items()] == LAYOUT[case]["state_dict"]
+
+
+@pytest.mark.parametrize("case", list(LAYOUT))
+def test_native_checkpoint_roundtrip(case):
+    src, dst = native(case, seed=1), native(case, seed=0)
+    assert dst.load_state_dict({k: v.clone() for k, v in src.state_dict().items()}) == ([], [])
+    for (name, p), q in zip(dst.named_parameters(), src.parameters()):
+        assert torch.equal(p, q), name                        # vocabulary padding rows included: zero in both
+    # saved tensors are views of the live parameters, under DDP's prefix too
+    sd = dst.state_dict(prefix="module.", keep_vars=True)
+    assert list(sd) == ["module." + k for k, _ in LAYOUT[case]["state_dict"]] and all(v.requires_grad for v in sd.values())
+    with torch.no_grad():
+        dst.head_weight[0, 0] = 5.0
+    assert dst.state_dict()["lm_head.weight"][0, 0] == 5.0
+
+
+@pytest.mark.parametrize("case", list(LAYOUT))
+def test_native_load_strict(case):
+    m = native(case)
+    sd = {k: v.clone() for k, v in m.state_dict().items()}
+    with pytest.raises(RuntimeError, match=re.escape("unexpected=['bogus.weight']")):
+        m.load_state_dict({**sd, "bogus.weight": torch.zeros(1)})
+    first = next(iter(sd))
+    less = {k: v for k, v in sd.items() if k != first}
+    with pytest.raises(RuntimeError, match=re.escape(f"missing=['{first}']")):
+        m.load_state_dict(less)
+    assert m.load_state_dict({**less, "bogus.weight": torch.zeros(1)}, strict=False) == ([first], ["bogus.weight"])
+
+
+@pytest.mark.parametrize("case", list(LAYOUT))
+def test_native_load_ignores_own_hf_buffers(case):
+    family = case.rsplit("_", 1)[0]
+    other = HF_BUFFERS["gpt_neo" if family == "llama" else "llama"]
+    m = native(case)
+    sd = {k: v.clone() for k, v in m.state_dict().items()}
+    assert m.load_state_dict({**sd, **{k: torch.zeros(1) for k in HF_BUFFERS[family]}}) == ([], [])
+    assert m.load_state_dict({**sd, **{k: torch.zeros(1) for k in other}}, strict=False) == ([], other)
+
+
+@pytest.mark.parametrize("case", list(LAYOUT))
+def test_native_load_lm_head(case):
+    """A tied head is the embedding: it neither needs ``lm_head.weight`` nor reports it, and ignores its values."""
+    tied = case.endswith("_tied")
+    m = native(case)
+    sd = {k: v.clone() for k, v in native(case, seed=1).state_dict().items()}
+    sd.pop("lm_head.weight")
+    assert m.load_state_dict(sd, strict=False) == ([] if tied else ["lm_head.weight"], [])
+    if not tied:
+        with pytest.raises(RuntimeError, match=re.escape("missing=['lm_head.weight']")):
+            m.load_state_dict(sd)
+    embed = next(iter(sd))
+    assert m.load_state_dict({**sd, "lm_head.weight": torch.zeros_like(sd[embed])}) == ([], [])
+    head = m.state_dict()["lm_head.weight"]
+    assert torch.equal(head, sd[embed]) if tied else not head.any()
 
 
 def test_llama_param_count_presets():
