@@ -287,6 +287,21 @@ void set_nodecay(RoundParams& P, const c10::optional<torch::Tensor>& ranges, int
     P.nodecay_base = base;
 }
 
+// The round kernel moves every shard tensor in 16-byte vectors and takes its scalars and counters from device memory.
+// The address is taken from the storage: data_ptr() is null for an empty view, wherever it lies.
+void check_round_vec(const torch::Tensor& t, const torch::Tensor& master, const char* name) {
+    TORCH_CHECK(t.device() == master.device(), name, " must be on the device of master (", master.device(), "), got ", t.device());
+    const uintptr_t addr = (uintptr_t)t.storage().data() + (uintptr_t)t.storage_offset() * (uintptr_t)t.element_size();
+    TORCH_CHECK(addr % 16 == 0, name, " must be 16-byte aligned");
+}
+void check_same_device(const torch::Tensor& t, const torch::Tensor& master, const char* name) {
+    TORCH_CHECK(t.device() == master.device(), name, " must be on the device of master (", master.device(), "), got ", t.device());
+}
+void check_moments(const torch::Tensor& exp_avg, const torch::Tensor& exp_avg_sq, int64_t S) {
+    TORCH_CHECK(exp_avg.numel() == S && exp_avg_sq.numel() == S, "exp_avg and exp_avg_sq must hold the shard's ", S, " elements, got ",
+                exp_avg.numel(), " and ", exp_avg_sq.numel());
+}
+
 // Local (single GPU / post-NCCL) sharded AdamW: grad_sum [S] (bf16|fp32) -> out [S] (bf16|fp32)
 void adamw_shard(torch::Tensor grad_sum, torch::Tensor master, torch::Tensor exp_avg, torch::Tensor exp_avg_sq, torch::Tensor stash,
                  torch::Tensor out, torch::Tensor inv_count, torch::Tensor scratch /* int32[4]: stash_count,total,epoch,done */,
@@ -297,6 +312,11 @@ void adamw_shard(torch::Tensor grad_sum, torch::Tensor master, torch::Tensor exp
     const int64_t S = master.numel();
     TORCH_CHECK(S % 8 == 0, "shard size must be a multiple of 8 (use slice alignment >= 8)");
     TORCH_CHECK(grad_sum.numel() >= S && out.numel() >= S && grad_sum.is_contiguous() && out.is_contiguous(), "bad grad/out");
+    check_moments(exp_avg, exp_avg_sq, S);
+    TORCH_CHECK(stash.numel() == S, "stash must hold the shard's ", S, " elements, got ", stash.numel());
+    check_round_vec(grad_sum, master, "grad_sum"); check_round_vec(master, master, "master"); check_round_vec(exp_avg, master, "exp_avg");
+    check_round_vec(exp_avg_sq, master, "exp_avg_sq"); check_round_vec(stash, master, "stash"); check_round_vec(out, master, "out");
+    check_same_device(inv_count, master, "inv_count"); check_same_device(scratch, master, "scratch");
     TORCH_CHECK(scratch.scalar_type() == torch::kInt32 && scratch.numel() >= 4, "scratch must be int32[4]");
     const bool gb = grad_sum.scalar_type() == torch::kBFloat16, ob = out.scalar_type() == torch::kBFloat16;
     TORCH_CHECK(gb || grad_sum.scalar_type() == torch::kFloat32, "grad dtype");
@@ -326,6 +346,7 @@ RoundParams round_params(const std::vector<int64_t>& acc_ptrs, const std::vector
     TORCH_CHECK(slice % 8 == 0 && stash.numel() == slice, "slice must be a multiple of 8 and match the shard state");
     TORCH_CHECK(mode != 2 || acc_mc != 0, "multicast mode needs multicast pointers");
     TORCH_CHECK(scratch.scalar_type() == torch::kInt32 && scratch.numel() >= 4, "scratch must be int32[4]");
+    for (int64_t p : acc_ptrs) TORCH_CHECK(p % 16 == 0, "acc_ptrs must be 16-byte aligned addresses");
     RoundParams P{};
     for (size_t i = 0; i < acc_ptrs.size() && i < (size_t)kMaxWorld; ++i) P.acc_peer[i] = (const void*)acc_ptrs[i];
     for (size_t i = 0; i < theta_ptrs.size() && i < (size_t)kMaxWorld; ++i) P.theta_peer[i] = (void*)theta_ptrs[i];
@@ -359,6 +380,10 @@ void rs_adam_ag(std::vector<int64_t> acc_ptrs, std::vector<int64_t> theta_ptrs, 
     check_f32(master, "master"); check_f32(exp_avg, "exp_avg"); check_f32(exp_avg_sq, "exp_avg_sq");
     const c10::cuda::CUDAGuard guard(master.device());
     TORCH_CHECK(master.numel() == slice, "slice must match the shard state");
+    check_moments(exp_avg, exp_avg_sq, slice);
+    check_round_vec(master, master, "master"); check_round_vec(exp_avg, master, "exp_avg"); check_round_vec(exp_avg_sq, master, "exp_avg_sq");
+    check_round_vec(stash, master, "stash"); check_same_device(scratch, master, "scratch");
+    for (int64_t p : theta_ptrs) TORCH_CHECK(p % 16 == 0, "theta_ptrs must be 16-byte aligned addresses");
     TORCH_CHECK((int64_t)theta_ptrs.size() >= (mode == 0 ? 1 : world), "peer pointer tables too short");
     TORCH_CHECK(mode != 2 || theta_mc != 0, "multicast mode needs multicast pointers");
     RoundParams P = round_params(acc_ptrs, theta_ptrs, pad_ptrs, acc_mc, theta_mc, stash, scratch, slice, rank, world, local_count, mode);
@@ -371,6 +396,7 @@ void rs_adam_ag(std::vector<int64_t> acc_ptrs, std::vector<int64_t> theta_ptrs, 
     }
     if (inv_count.has_value() && inv_count->defined()) {
         check_f32(*inv_count, "inv_count");
+        check_same_device(*inv_count, master, "inv_count");
         TORCH_CHECK(inv_count->numel() >= 2, "inv_count must be the scratch of round_norm (inv_eff at index 1)");
         P.inv_count_in = inv_count->data_ptr<float>() + 1;
         if (mode != 0) P.gated = 2;
