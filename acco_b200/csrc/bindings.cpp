@@ -521,8 +521,9 @@ std::vector<torch::Tensor> fp8_quantize(torch::Tensor t, bool e5m2, bool rowmajo
 
 // out[M,N] (+)= a[M,K] * b[N,K]^T / (s_a s_b) (+ bias).  a: e4m3 or e5m2, b: e4m3, both K-major with 16-byte aligned rows; scale_a / scale_b:
 // the scale tensors of fp8_quantize (1/s read on the device).  accumulate: out += (bf16 reduce-add epilogue, split-K allowed).
+// max_ctas > 0 caps the persistent grid, as in gemm.
 torch::Tensor gemm_fp8(torch::Tensor a, torch::Tensor b, torch::Tensor scale_a, torch::Tensor scale_b, c10::optional<torch::Tensor> out,
-                       c10::optional<torch::Tensor> bias, bool accumulate, int64_t bn, int64_t splits) {
+                       c10::optional<torch::Tensor> bias, bool accumulate, int64_t bn, int64_t splits, int64_t max_ctas) {
     auto ok2d = [](const torch::Tensor& t) {
         return t.is_cuda() && t.dim() == 2 && t.stride(1) == 1 && t.stride(0) % 16 == 0 && t.stride(0) >= t.size(1) && (uintptr_t)t.data_ptr() % 16 == 0;
     };
@@ -550,9 +551,11 @@ torch::Tensor gemm_fp8(torch::Tensor a, torch::Tensor b, torch::Tensor scale_a, 
                     (uintptr_t)bias->data_ptr() % 16 == 0, "gemm_fp8: bias must be a contiguous, 16-byte aligned CUDA bf16 [N] vector");
         bias_p = bias->data_ptr();
     }
+    int sms = sm_count();
+    if (max_ctas > 0 && max_ctas < sms) sms = (int)max_ctas;
     const int rc = acco_gemm_fp8_run(a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), y.data_ptr(), y.stride(0), bias_p, (int)M, (int)N, (int)K,
                                      accumulate ? 1 : 0, a.scalar_type() == torch::kFloat8_e5m2 ? 1 : 0, scale_a.data_ptr<float>() + 1,
-                                     scale_b.data_ptr<float>() + 1, (int)bn, (int)splits, sm_count(), stream());
+                                     scale_b.data_ptr<float>() + 1, (int)bn, (int)splits, sms, stream());
     TORCH_CHECK(rc == 0, "gemm_fp8 launch failed, code ", rc, " (M=", M, " N=", N, " K=", K, ")");
     return y;
 }

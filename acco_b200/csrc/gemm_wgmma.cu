@@ -157,6 +157,44 @@ __device__ __forceinline__ void mma_k32(float (&acc)[BN / 2], uint64_t da, uint6
     else wgmma_m64n64k32_f8<OP == OP_E5M2>(acc, da, db, scale_d);
 }
 
+// |v| = m 2^e with m in [1, 2), for a finite non-zero fp32 (subnormals included: read from the bits, not flushed)
+__device__ __forceinline__ void split_exponent(uint32_t u, int& e, float& m) {
+    u &= 0x7FFFFFFFu;
+    uint32_t frac = u & 0x7FFFFFu;
+    if ((u >> 23) == 0) {
+        const int lead = 31 - __clz(frac);
+        e = -149 + lead;
+        frac = (frac << (23 - lead)) & 0x7FFFFFu;
+    } else {
+        e = (int)(u >> 23) - 127;
+    }
+    m = __uint_as_float(0x3F800000u | frac);
+}
+
+// FP8 output scale 1 / (s_a s_b) = inv_a * inv_b, applied as (acc * pre) * post.  The quantiser emits inverses from 2^-127 (a subnormal,
+// which this fast-math build would read as 0) to 2^120, so their product spans 2^-254 .. 2^240.  post is that product at its exponent
+// clamped to the normal range, pre = 2^(the rest): pre = 1 whenever the product is a normal fp32 (the epilogue is then one fma per
+// element), otherwise pre rescales the fp32 sum first, exactly (a power of two; whenever the result is a normal number, so is acc * pre).
+// Launch-uniform: every thread derives the same pair from the same two words.
+__device__ __forceinline__ void fp8_out_scale(float inv_a, float inv_b, float& pre, float& post) {
+    const uint32_t ua = __float_as_uint(inv_a), ub = __float_as_uint(inv_b);
+    pre = 1.f;
+    if ((ua & 0x7FFFFFFFu) == 0 || (ub & 0x7FFFFFFFu) == 0 || (ua & 0x7F800000u) == 0x7F800000u || (ub & 0x7F800000u) == 0x7F800000u) {
+        post = inv_a * inv_b;                              // 0, Inf or NaN (a NaN / Inf tensor's scale): propagate
+        return;
+    }
+    int ea, eb;
+    float ma, mb;
+    split_exponent(ua, ea, ma);
+    split_exponent(ub, eb, mb);
+    float m = ma * mb;                                     // [1, 4); exact for powers of two
+    int e = ea + eb;
+    if (m >= 2.f) { m *= 0.5f; ++e; }
+    const int ec = min(max(e, -126), 127), d = e - ec;    // d in [-172, 127]
+    post = __uint_as_float(((ua ^ ub) & 0x80000000u) | (__float_as_uint(m) + ((uint32_t)ec << 23)));
+    pre = d < -126 ? 0.f : __uint_as_float((uint32_t)(d + 127) << 23);   // below 2^-126 the output is far below bf16's normal range
+}
+
 template <int BN, int A_MN, int B_MN, int OP>
 __device__ __forceinline__ void gemm_body(const Params& P) {
     static_assert(OP == OP_BF16 || (A_MN == 0 && B_MN == 0), "FP8 wgmma has no transpose: both operands K-major");
@@ -322,8 +360,8 @@ __device__ __forceinline__ void gemm_body(const Params& P) {
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
         float part[OP ? BN / 2 : 1];                       // FP8: the current k-block's fragment
-        float out_scale = 1.f;
-        if constexpr (OP != OP_BF16) out_scale = P.inv_scale_a[0] * P.inv_scale_b[0];   // powers of two: exact
+        float out_scale = 1.f, pre_scale = 1.f;
+        if constexpr (OP != OP_BF16) fp8_out_scale(P.inv_scale_a[0], P.inv_scale_b[0], pre_scale, out_scale);
         int stage = 0;
         uint32_t phase = 0;
         for (int t = unit0; t < num_units; t += unit_stride) {
@@ -381,6 +419,9 @@ __device__ __forceinline__ void gemm_body(const Params& P) {
                 wgmma_wait<0>();
                 reg_fence(acc);
                 release(prev);
+            } else if (pre_scale != 1.f) {                 // an output scale outside fp32's normal range (fp8_out_scale)
+#pragma unroll
+                for (int i = 0; i < BN / 2; ++i) acc[i] *= pre_scale;
             }
             // ---------------- epilogue: fragment (row 16 warp + lane/4 (+8), columns 8 j + 2 (lane % 4) (+1)) -> staging -> TMA
             const int m0 = u.mb * BM + cw * 64;

@@ -62,10 +62,13 @@ def quantize(t: torch.Tensor, fmt, rowmajor: bool = True, transposed: bool = Fal
 
 
 def gemm_fp8_ref(a, b, scale_a, scale_b, out=None, bias=None, accumulate=False, dtype=torch.bfloat16):
-    """``out[M,N] (+)= a[M,K] b[N,K]^T / (s_a s_b) (+ bias)`` in fp32, rounded once to ``dtype`` (``out``'s when given)."""
-    y = (a.float() @ b.float().t()) * (scale_a[1] * scale_b[1])
+    """``out[M,N] (+)= a[M,K] b[N,K]^T / (s_a s_b) (+ bias)`` in fp32, rounded once to ``dtype`` (``out``'s when given).  The scale
+    product is formed in fp64, as the kernel's epilogue forms it exactly: ``1/s`` runs from ``2^-127`` to ``2^120``, so the product of
+    two can leave fp32's range although the output is an ordinary number."""
+    y = (a.float() @ b.float().t()).double() * (scale_a[1].double() * scale_b[1].double())
     if bias is not None:
-        y = y + bias.float()
+        y = y + bias.double()
+    y = y.float()
     if accumulate:
         y = y + out.float()
     if out is not None:
@@ -74,12 +77,13 @@ def gemm_fp8_ref(a, b, scale_a, scale_b, out=None, bias=None, accumulate=False, 
     return y.to(dtype)
 
 
-def gemm_fp8(a, b, scale_a, scale_b, out=None, bias=None, accumulate=False, bn: int = 0, splits: int = 0):
+def gemm_fp8(a, b, scale_a, scale_b, out=None, bias=None, accumulate=False, bn: int = 0, splits: int = 0, max_ctas: int = 0):
     """FP8 wgmma GEMM (``csrc/gemm_wgmma.cu``, ``gemm_fp8_kernel``): ``a`` e4m3 or e5m2, ``b`` e4m3, both K-major one-byte ``[rows, K]``;
-    bf16 out; ``accumulate`` adds into ``out`` (split-K allowed).  ``bn`` / ``splits``: 0 = heuristic."""
+    bf16 out; ``accumulate`` adds into ``out`` (split-K allowed).  ``bn`` / ``splits``: 0 = heuristic; ``max_ctas`` > 0 caps the
+    persistent grid (as in :func:`ops.gemm.gemm`)."""
     if not use_kernels(a, b, bf16_only=False):
         return gemm_fp8_ref(a, b, scale_a, scale_b, out, bias, accumulate)
-    y = load_ext(required=True).gemm_fp8(a, b, scale_a, scale_b, out, bias, bool(accumulate), int(bn), int(splits))
+    y = load_ext(required=True).gemm_fp8(a, b, scale_a, scale_b, out, bias, bool(accumulate), int(bn), int(splits), int(max_ctas))
     count_launch("gemm_fp8")
     return y
 

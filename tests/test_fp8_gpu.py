@@ -2,17 +2,15 @@
 FP8 linear autograd against the fp64 contract, whole models against fp32, and the trainer (CUDA graphs, launch counts, loss).
 
 Tolerances.
-* GEMM, fp64 oracle ``y64 = a b^T / (s_a s_b) (+ bias) (+ C)`` on the dequantised operands.  The kernel differs from it by (1) the bf16
-  rounding of the output, at most one bf16 ulp of ``|y64|`` (2^-8 |y64| covers the half-ulp rounding of the result and of the
-  added bf16 ``C``), and (2) the accumulation: Hopper's FP8 tensor cores keep about 14 bits while they sum within one wgmma
-  (DeepSeek-V3 report).  The kernel promotes every 128-deep k-block (four k32 wgmmas) to fp32, so each block loses at most
-  4 * 2^-13 of its absolute sum; summed over blocks that is 2^-11 * S with ``S = |a| |b|^T / (s_a s_b)``.  The fp32 sums of the
-  promoted fragments add K/128 * 2^-24 * S, far below that.  So ``|y - y64| <= 2^-8 |y64| + 2^-11 S + 2^-133`` (the last term is the
-  smallest bf16 subnormal).  An adding epilogue (wgrad) rounds once more per bf16 add into the output, each at the magnitude of the
-  running sum, which is bounded by ``|C| + S``: with ``splits`` partial sums added in bf16 that is ``splits * 2^-9 (|C| + S)`` more.
+* GEMM: the per-element bound of ``test_fp8_oracle.py`` (``bound``), against the fp64 result ``y64 = a b^T / (s_a s_b) (+ bias)
+  (+ C)`` on the dequantised operands, where it is derived with the accumulator width (``ACC_BITS``) as a named constant.  It is
+  looser than the bound this file used to carry: one bf16 ulp ``2^-7 |y64|`` instead of ``2^-8 |y64|`` (so that an exact emulation of
+  the kernel stays within half of it), and on split-K paths a term for two bf16 roundings per split, which makes it a valid worst case
+  there.  The checks that pin the arithmetic down are elsewhere: the exact tier (bit for bit), the scale edges and the two sharp
+  statistics (share of elements off ``bf16_rn(y64)``, relative rms error) run in ``test_fp8_oracle_gpu.py``.
 * Cross-check: the bf16 wgmma GEMM on the dequantised operands (exact in bf16: e4m3 and e5m2 values are bf16 values, and the scales
   are powers of two) multiplies the same numbers and accumulates in fp32.  Both round once to bf16, so they agree within one bf16
-  ulp plus the FP8 accumulation term ``2^-11 S`` above.
+  ulp plus the FP8 accumulation term ``4 * 2^(1 - ACC_BITS) S`` of that bound.
 * Whole models against fp32: q(x) and q(W) carry a relative rounding error of at most 2^-4 (e4m3) per element and q(g) 2^-3 (e5m2),
   independent across elements, so a K-term dot product errs by about 2^-4 / sqrt(3) of its magnitude: a few per cent on every GEMM
   output, less on the loss, which averages over tokens.  The loss must agree within 2 %; every parameter gradient must point the same
@@ -33,6 +31,7 @@ from acco_b200.data import synthetic_pretrain_dataset
 from acco_b200.launch import DistEnv
 from acco_b200.models import GPTConfig, GPTForCausalLM, LlamaConfig, LlamaForCausalLM
 from acco_b200.ops.fp8 import E4M3, E5M2, Fp8LinearFn, gemm_fp8, quantize, quantize_ref
+from test_fp8_oracle import ACC_BITS, bound as fp8_bound, split_geometry as fp8_split_geometry  # noqa: E402
 
 DEV = torch.device("cuda")
 LOG = logging.getLogger("acco-test")
@@ -99,17 +98,19 @@ def _operands(M, N, K, a_fmt, seed):
 
 
 def _check(y, qa, qb, sa, sb, bias=None, c=None, splits=1):
+    """``y`` within ``test_fp8_oracle.bound``; ``splits``: the K splits requested (the host's effective count is used)."""
     a64, b64 = qa.double() * float(sa[1]), qb.double() * float(sb[1])
     y64 = a64 @ b64.t()
     S = a64.abs() @ b64.abs().t()
+    mag = S.clone()
     if bias is not None:
         y64 = y64 + bias.double()
+        mag = mag + bias.double().abs()
     if c is not None:
         y64 = y64 + c.double()
+        mag = mag + c.double().abs()
     err = (y.double() - y64).abs()
-    tol = 2.0 ** -8 * y64.abs() + 2.0 ** -11 * S + 2.0 ** -133
-    if c is not None:
-        tol = tol + splits * 2.0 ** -9 * (c.double().abs() + S)
+    tol = fp8_bound(y64, S, mag, qa.shape[1], fp8_split_geometry(qa.shape[1], splits)[1])
     assert bool((err <= tol).all()), f"max excess {float((err - tol).max())}"
     return y64, S
 
@@ -124,7 +125,7 @@ def _cross(y, qa, qb, sa, sb, bias=None):
     ref = torch.maximum(y.double().abs(), yb.double().abs())
     ulp = torch.exp2(torch.floor(torch.log2(ref.clamp_min(2.0 ** -126)))) * 2.0 ** -7
     diff = (y.double() - yb.double()).abs()
-    bad = diff > ulp + 2.0 ** -11 * S
+    bad = diff > ulp + 2.0 ** (3 - ACC_BITS) * S
     assert not bool(bad.any()), f"{int(bad.sum())} elements beyond the bound"
     assert float((diff <= ulp).double().mean()) >= 0.5          # most elements: the two kernels round the same value
 
