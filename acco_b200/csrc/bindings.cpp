@@ -26,6 +26,7 @@ int acco_ce_fwd(const void* logits, const long long* labels, float* lse, float* 
                 int V, int Vp, long long ignore_index, float label_smoothing, cudaStream_t st);
 int acco_ce_bwd(void* logits, const long long* labels, const float* lse, const float* scale, long long T, int V, int Vp,
                 long long ignore_index, float label_smoothing, cudaStream_t st);
+int acco_embedding_bwd(void* grad, const long long* sorted, const long long* perm, const void* dy, int T, int H, int sms, cudaStream_t st);
 int acco_gelu_fwd(const void* x, void* y, long long n, int sms, cudaStream_t st);
 int acco_gelu_bwd(const void* dy, const void* x, void* dx, long long n, int sms, cudaStream_t st);
 int acco_debug_occupy(unsigned long long ns, int ctas, float* sink, cudaStream_t st);
@@ -220,6 +221,23 @@ torch::Tensor swiglu_bwd(torch::Tensor dout, torch::Tensor gu) {
     auto dgu = torch::empty_like(gu);
     TORCH_CHECK(acco_swiglu_bwd(dout.data_ptr(), gu.data_ptr(), dgu.data_ptr(), T, (int)I, sm_count(), stream()) == 0, "swiglu: I must be a multiple of 8");
     return dgu;
+}
+
+// ---------------------------------------------------------------- embedding backward
+// grad [R, H] += the rows of dy [T, H] scattered by the ids, in place: `sorted` is the stably sorted ids (int64 [T]) and `perm`
+// the dy row of each sorted position.  Each row an id hits is read and written once, from an fp32 sum in a fixed order.
+void embedding_bwd(torch::Tensor grad, torch::Tensor sorted, torch::Tensor perm, torch::Tensor dy) {
+    check_bf16(grad, "grad"); check_bf16(dy, "dy");
+    for (auto* t : {&sorted, &perm})
+        TORCH_CHECK(t->is_cuda() && t->scalar_type() == torch::kInt64 && t->is_contiguous() && t->numel() == dy.size(0),
+                    "sorted ids / permutation must be contiguous CUDA int64 with one entry per dy row");
+    TORCH_CHECK(grad.dim() == 2 && dy.dim() == 2 && grad.size(1) == dy.size(1), "grad and dy must be [R, H] and [T, H]");
+    TORCH_CHECK(grad.device() == dy.device() && sorted.device() == dy.device() && perm.device() == dy.device(), "tensors on different devices");
+    TORCH_CHECK((uintptr_t)grad.data_ptr() % 16 == 0 && (uintptr_t)dy.data_ptr() % 16 == 0, "grad and dy must be 16-byte aligned");
+    const c10::cuda::CUDAGuard guard(dy.device());
+    TORCH_CHECK(acco_embedding_bwd(grad.data_ptr(), (const long long*)sorted.data_ptr<int64_t>(), (const long long*)perm.data_ptr<int64_t>(),
+                                   dy.data_ptr(), (int)dy.size(0), (int)dy.size(1), sm_count(), stream()) == 0,
+                "embedding_bwd: hidden size must be a multiple of 8");
 }
 
 // ---------------------------------------------------------------- cross entropy
@@ -657,6 +675,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("rope_pack_bwd", &rope_pack_bwd);
     m.def("swiglu_fwd", &swiglu_fwd);
     m.def("swiglu_bwd", &swiglu_bwd);
+    m.def("embedding_bwd", &embedding_bwd);
     m.def("ce_fwd", &ce_fwd, py::arg("logits"), py::arg("labels"), py::arg("V"), py::arg("ignore_index"), py::arg("label_smoothing") = 0.0);
     m.def("ce_bwd_inplace", &ce_bwd_inplace, py::arg("logits"), py::arg("labels"), py::arg("lse"), py::arg("scale"), py::arg("V"),
           py::arg("ignore_index"), py::arg("label_smoothing") = 0.0);

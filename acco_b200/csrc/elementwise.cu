@@ -1,5 +1,5 @@
-// RoPE (in place on the fused QKV buffer), SwiGLU and GELU-new forward/backward.  Pure streaming kernels:
-// 16-byte vector accesses, one pass, grid sized by the caller's element count.
+// RoPE (in place on the fused QKV buffer), SwiGLU and GELU-new forward/backward, and the embedding backward.  Pure streaming
+// kernels: 16-byte vector accesses, one pass, grid sized by the caller's element count.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -187,6 +187,62 @@ __global__ void __launch_bounds__(256) gelu_bwd_kernel(const __nv_bfloat16* __re
     }
 }
 
+// ---- embedding backward ---------------------------------------------------------------------------------------------
+// grad[r] = bf16_rn(grad[r] + sum_{i: ids[i] = r} dy[i]) with the sum in fp32 and ONE write per row, in a fixed order.
+// The ids come sorted (`sorted`, stable, with the permutation `perm` back to dy rows), so each distinct row is one run.
+// A CTA owns a 256-column slice of a run: its 8 warps take the run's occurrences round-robin (up to 4 loads in flight
+// per lane), then warp 0 adds the 8 partial sums in warp order to the row.  Rows no id hits are never read or written.
+constexpr int kEmbWarps = 8, kEmbCols = 8 * kWarp, kEmbUnroll = 4;
+__global__ void __launch_bounds__(kEmbWarps * kWarp) embedding_bwd_kernel(__nv_bfloat16* __restrict__ grad,
+                                                                       const long long* __restrict__ sorted,
+                                                                       const long long* __restrict__ perm,
+                                                                       const __nv_bfloat16* __restrict__ dy, int T, int H) {
+    __shared__ float part[kEmbWarps][kEmbCols];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int col = blockIdx.y * kEmbCols + 8 * lane;
+    const bool live = col < H;
+    for (int i = blockIdx.x; i < T; i += gridDim.x) {
+        const long long r = sorted[i];
+        if (i > 0 && sorted[i - 1] == r) continue;      // not the start of a run (uniform across the CTA)
+        float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        for (int j = i + w; j < T && sorted[j] == r; j += kEmbWarps * kEmbUnroll) {
+            bf16x8 v[kEmbUnroll];
+            bool ok[kEmbUnroll];
+#pragma unroll
+            for (int u = 0; u < kEmbUnroll; ++u) {
+                const int ju = j + u * kEmbWarps;
+                ok[u] = live && ju < T && sorted[ju] == r;
+                if (ok[u]) v[u] = ld_stream(dy + (size_t)perm[ju] * H + col);
+            }
+#pragma unroll
+            for (int u = 0; u < kEmbUnroll; ++u) {
+                if (!ok[u]) break;
+                float f[8];
+                unpack8(v[u], f);
+#pragma unroll
+                for (int k = 0; k < 8; ++k) acc[k] += f[k];
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < 8; ++k) part[w][8 * lane + k] = acc[k];
+        __syncthreads();
+        if (w == 0 && live) {
+            __nv_bfloat16* row = grad + (size_t)r * H + col;
+            float s[8];
+            unpack8(ld_vec(row), s);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+                float t = part[0][8 * lane + k];
+#pragma unroll
+                for (int q = 1; q < kEmbWarps; ++q) t += part[q][8 * lane + k];
+                s[k] += t;
+            }
+            st_vec(row, pack8(s));
+        }
+        __syncthreads();
+    }
+}
+
 static int grid_for(long long work_items, int threads, int sms) {
     long long want = (work_items + threads - 1) / threads;
     long long cap = (long long)sms * (2048 / threads) * 4;  // a few waves; kernels are grid-stride
@@ -215,6 +271,16 @@ extern "C" int acco_rope_pack_bwd(const void* dq, const void* dk, const void* dv
     const long long work = (long long)B * S * 32;   // one warp per token
     acco::rope_pack_bwd_kernel<<<acco::grid_for(work, 256, sms), 256, 0, st>>>(src, (__nv_bfloat16*)dqkv, cos_t, sin_t, B, S, Hq, Hk, D);
     return 0;
+}
+
+extern "C" int acco_embedding_bwd(void* grad, const long long* sorted, const long long* perm, const void* dy, int T, int H, int sms,
+                                  cudaStream_t st) {
+    if (H % 8 != 0) return -1;
+    if (T == 0) return 0;
+    const dim3 grid(T < 4 * sms ? T : 4 * sms, (H + acco::kEmbCols - 1) / acco::kEmbCols);
+    acco::embedding_bwd_kernel<<<grid, acco::kEmbWarps * acco::kWarp, 0, st>>>((__nv_bfloat16*)grad, sorted, perm,
+                                                                              (const __nv_bfloat16*)dy, T, H);
+    return (int)cudaGetLastError();
 }
 
 extern "C" int acco_swiglu_fwd(const void* gu, void* out, long long T, int I, int sms, cudaStream_t st) {

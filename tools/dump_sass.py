@@ -37,6 +37,7 @@ KERNELS = {
     "gemm_fp8_bn128_e5m2.sass": "_ZN9acco_gemm15gemm_fp8_kernelILi128ELi2EEEvNS_6ParamsE",     # dgrad / wgrad
     "fp8_amax.sass": "_ZN8acco_fp815fp8_amax_kernelEPK5uint4xPj",
     "fp8_cast_e4m3.sass": "_ZN8acco_fp815fp8_cast_kernelILi0EEEvPK13__nv_bfloat16PKjiPhS6_Pfii",
+    "embedding_bwd.sass": "_ZN4acco20embedding_bwd_kernelEP13__nv_bfloat16PKxS3_PKS0_ii",        # one write per row: no REDG
 }
 MNEMONICS = ["HGMMA", "UTMALDG", "UTMALDG.2D.MULTICAST", "UTMASTG", "UTMACMDFLUSH", "SYNCS", "USETMAXREG", "REDG", "LDGMC", "HMMA", "MUFU.SQRT",
              "MUFU.EX2", "CCTL"]
