@@ -26,7 +26,10 @@ int acco_ce_fwd(const void* logits, const long long* labels, float* lse, float* 
                 int V, int Vp, long long ignore_index, float label_smoothing, cudaStream_t st);
 int acco_ce_bwd(void* logits, const long long* labels, const float* lse, const float* scale, long long T, int V, int Vp,
                 long long ignore_index, float label_smoothing, cudaStream_t st);
+int acco_norm_bwd_acc_f32(const void* dy, const void* dh_extra, const void* h, const void* w, const float* mean, const float* rstd, void* dh,
+                          float* partial, float* dw_accum, float* db_accum, int T, int H, int grid, cudaStream_t st);
 int acco_embedding_bwd(void* grad, const long long* sorted, const long long* perm, const void* dy, int T, int H, int sms, cudaStream_t st);
+int acco_embedding_bwd_f32(float* grad, const long long* sorted, const long long* perm, const void* dy, int T, int H, int sms, cudaStream_t st);
 int acco_gelu_fwd(const void* x, void* y, long long n, int sms, cudaStream_t st);
 int acco_gelu_bwd(const void* dy, const void* x, void* dx, long long n, int sms, cudaStream_t st);
 int acco_debug_occupy(unsigned long long ns, int ctas, float* sink, cudaStream_t st);
@@ -41,6 +44,10 @@ void acco_gemm_set_debug(unsigned long long* buf);
 void acco_gemm_choose(int M, int N, int K, int a_mn, int b_mn, int accumulate, int sms, int* out5);
 int acco_gemm_fp8_run(const void* a, long long lda, const void* b, long long ldb, void* d, long long ldd, const void* bias, int M, int N, int K,
                       int accumulate, int a_e5m2, const float* inv_a, const float* inv_b, int bn_req, int splits_req, int sms, cudaStream_t st);
+int acco_gemm_wgrad_f32(const void* a, long long lda, const void* b, long long ldb, float* d, long long ldd, int M, int N, int K, int bn_req,
+                        int splits_req, int sms, cudaStream_t st);
+int acco_gemm_fp8_acc_f32(const void* a, long long lda, const void* b, long long ldb, float* d, long long ldd, int M, int N, int K, int a_e5m2,
+                          const float* inv_a, const float* inv_b, int bn_req, int splits_req, int sms, cudaStream_t st);
 int acco_fp8_amax_ctas(long long n, int sms);
 int acco_fp8_quantize(const void* t, int R, int C, int e5m2, void* q, void* qT, float* scale_out, int ctas, cudaStream_t st);
 int acco_gemm_tile_n();
@@ -161,6 +168,32 @@ std::vector<torch::Tensor> norm_bwd(torch::Tensor dy, c10::optional<torch::Tenso
     return {dh, dwdb};
 }
 
+// As norm_bwd with the dw (| db) sums added to fp32 gradients (fp32 gradient accumulators under bf16 weights): wgrad, and bgrad for
+// LayerNorm, are required.  Returns dh.
+torch::Tensor norm_bwd_acc_f32(torch::Tensor dy, c10::optional<torch::Tensor> dh_extra, torch::Tensor h, torch::Tensor w,
+                               c10::optional<torch::Tensor> mean, torch::Tensor rstd, torch::Tensor wgrad, c10::optional<torch::Tensor> bgrad) {
+    check_bf16(dy, "dy"); check_bf16(h, "h"); check_bf16(w, "weight"); check_f32(rstd, "rstd"); check_f32(wgrad, "weight.grad");
+    const bool has_e = dh_extra.has_value() && dh_extra->defined(), layer = mean.has_value() && mean->defined();
+    if (has_e) check_bf16(*dh_extra, "dh_extra");
+    const c10::cuda::CUDAGuard guard(dy.device());
+    const int T = dy.size(0), H = dy.size(1), np = layer ? 2 : 1;
+    TORCH_CHECK(wgrad.numel() == H, "weight.grad has the wrong size");
+    if (layer) {
+        check_f32(*mean, "mean");
+        TORCH_CHECK(bgrad.has_value() && bgrad->defined(), "norm_bwd_acc_f32: LayerNorm needs bias.grad");
+        check_f32(*bgrad, "bias.grad");
+        TORCH_CHECK(bgrad->numel() == H, "bias.grad has the wrong size");
+    }
+    auto dh = torch::empty_like(dy);
+    const int grid = acco_norm_grid(T, H, sm_count(), 1);
+    auto partial = torch::empty({grid, np * H}, dy.options().dtype(torch::kFloat32));
+    TORCH_CHECK(acco_norm_bwd_acc_f32(dy.data_ptr(), has_e ? dh_extra->data_ptr() : nullptr, h.data_ptr(), w.data_ptr(),
+                                      layer ? mean->data_ptr<float>() : nullptr, rstd.data_ptr<float>(), dh.data_ptr(), partial.data_ptr<float>(),
+                                      wgrad.data_ptr<float>(), layer ? bgrad->data_ptr<float>() : nullptr, T, H, grid, stream()) == 0,
+                "norm_bwd_acc_f32: unsupported hidden size ", H);
+    return dh;
+}
+
 // ---------------------------------------------------------------- gelu (GPT family)
 torch::Tensor gelu_fwd(torch::Tensor x) {
     check_bf16(x, "x");
@@ -238,6 +271,21 @@ void embedding_bwd(torch::Tensor grad, torch::Tensor sorted, torch::Tensor perm,
     TORCH_CHECK(acco_embedding_bwd(grad.data_ptr(), (const long long*)sorted.data_ptr<int64_t>(), (const long long*)perm.data_ptr<int64_t>(),
                                    dy.data_ptr(), (int)dy.size(0), (int)dy.size(1), sm_count(), stream()) == 0,
                 "embedding_bwd: hidden size must be a multiple of 8");
+}
+
+// As embedding_bwd into fp32 rows: grad [R, H] fp32 (an fp32 gradient accumulator) += the bf16 rows of dy, one fp32 sum per row hit.
+void embedding_bwd_f32(torch::Tensor grad, torch::Tensor sorted, torch::Tensor perm, torch::Tensor dy) {
+    check_f32(grad, "grad"); check_bf16(dy, "dy");
+    for (auto* t : {&sorted, &perm})
+        TORCH_CHECK(t->is_cuda() && t->scalar_type() == torch::kInt64 && t->is_contiguous() && t->numel() == dy.size(0),
+                    "sorted ids / permutation must be contiguous CUDA int64 with one entry per dy row");
+    TORCH_CHECK(grad.dim() == 2 && dy.dim() == 2 && grad.size(1) == dy.size(1), "grad and dy must be [R, H] and [T, H]");
+    TORCH_CHECK(grad.device() == dy.device() && sorted.device() == dy.device() && perm.device() == dy.device(), "tensors on different devices");
+    TORCH_CHECK((uintptr_t)grad.data_ptr() % 16 == 0 && (uintptr_t)dy.data_ptr() % 16 == 0, "grad and dy must be 16-byte aligned");
+    const c10::cuda::CUDAGuard guard(dy.device());
+    TORCH_CHECK(acco_embedding_bwd_f32(grad.data_ptr<float>(), (const long long*)sorted.data_ptr<int64_t>(), (const long long*)perm.data_ptr<int64_t>(),
+                                       dy.data_ptr(), (int)dy.size(0), (int)dy.size(1), sm_count(), stream()) == 0,
+                "embedding_bwd_f32: hidden size must be a multiple of 8");
 }
 
 // ---------------------------------------------------------------- cross entropy
@@ -518,6 +566,28 @@ torch::Tensor gemm(torch::Tensor a, torch::Tensor b, c10::optional<torch::Tensor
     return y;
 }
 
+// wgrad into an fp32 gradient:  out[M,N] += A * B^T with a [K,M] and b [K,N] (both MN-major bf16, rows may be strided as in gemm) and
+// out a [M,N] fp32 matrix (unit inner stride, rows 16-byte aligned).  One K split adds exactly; split-K adds fp32 partials through TMA.
+void gemm_wgrad_f32(torch::Tensor a, torch::Tensor b, torch::Tensor out, int64_t bn, int64_t splits, int64_t max_ctas) {
+    auto ok2d = [](const torch::Tensor& t) {
+        return t.is_cuda() && t.scalar_type() == torch::kBFloat16 && t.dim() == 2 && t.stride(1) == 1 && t.stride(0) % 8 == 0 && t.stride(0) >= t.size(1) &&
+               (uintptr_t)t.data_ptr() % 16 == 0;
+    };
+    TORCH_CHECK(ok2d(a) && ok2d(b), "gemm_wgrad_f32: operands must be 2-D CUDA bf16, unit inner stride, 16-byte aligned rows");
+    const c10::cuda::CUDAGuard guard(a.device());
+    const int64_t M = a.size(1), K = a.size(0), N = b.size(1);
+    TORCH_CHECK(b.size(0) == K, "gemm_wgrad_f32: contraction sizes differ (", K, " vs ", b.size(0), ")");
+    TORCH_CHECK(N % 8 == 0, "gemm_wgrad_f32: N must be a multiple of 8");
+    TORCH_CHECK(out.is_cuda() && out.scalar_type() == torch::kFloat32 && out.dim() == 2 && out.size(0) == M && out.size(1) == N && out.stride(1) == 1 &&
+                out.stride(0) % 8 == 0 && out.stride(0) >= N && (uintptr_t)out.data_ptr() % 16 == 0,
+                "gemm_wgrad_f32: out must be a [M,N] CUDA fp32 matrix with 16-byte aligned rows");
+    int sms = sm_count();
+    if (max_ctas > 0 && max_ctas < sms) sms = (int)max_ctas;
+    const int rc = acco_gemm_wgrad_f32(a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), out.data_ptr<float>(), out.stride(0), (int)M, (int)N,
+                                       (int)K, (int)bn, (int)splits, sms, stream());
+    TORCH_CHECK(rc == 0, "gemm_wgrad_f32 launch failed, code ", rc, " (M=", M, " N=", N, " K=", K, ")");
+}
+
 // ---------------------------------------------------------------- FP8 (per-tensor current scaling)
 // t [R, C] bf16 -> {q [R, C] or None, qT [C, R] or None, scale fp32 [3 + ctas] = {s, 1/s, amax, per-CTA maxima...}}; e4m3 or (e5m2) e5m2.
 std::vector<torch::Tensor> fp8_quantize(torch::Tensor t, bool e5m2, bool rowmajor, bool transposed) {
@@ -576,6 +646,32 @@ torch::Tensor gemm_fp8(torch::Tensor a, torch::Tensor b, torch::Tensor scale_a, 
                                      scale_b.data_ptr<float>() + 1, (int)bn, (int)splits, sms, stream());
     TORCH_CHECK(rc == 0, "gemm_fp8 launch failed, code ", rc, " (M=", M, " N=", N, " K=", K, ")");
     return y;
+}
+
+// As gemm_fp8 with accumulate, into an fp32 out [M,N] (an fp32 gradient accumulator): out += a * b^T / (s_a s_b); no bias.
+void gemm_fp8_acc_f32(torch::Tensor a, torch::Tensor b, torch::Tensor scale_a, torch::Tensor scale_b, torch::Tensor out, int64_t bn, int64_t splits,
+                      int64_t max_ctas) {
+    auto ok2d = [](const torch::Tensor& t) {
+        return t.is_cuda() && t.dim() == 2 && t.stride(1) == 1 && t.stride(0) % 16 == 0 && t.stride(0) >= t.size(1) && (uintptr_t)t.data_ptr() % 16 == 0;
+    };
+    TORCH_CHECK(ok2d(a) && ok2d(b), "gemm_fp8_acc_f32: operands must be 2-D CUDA, unit inner stride, 16-byte aligned rows");
+    TORCH_CHECK(a.scalar_type() == torch::kFloat8_e4m3fn || a.scalar_type() == torch::kFloat8_e5m2, "gemm_fp8_acc_f32: a must be e4m3 or e5m2");
+    TORCH_CHECK(b.scalar_type() == torch::kFloat8_e4m3fn, "gemm_fp8_acc_f32: b must be e4m3");
+    check_f32(scale_a, "scale_a"); check_f32(scale_b, "scale_b");
+    TORCH_CHECK(scale_a.numel() >= 2 && scale_b.numel() >= 2, "gemm_fp8_acc_f32: scales must be {s, 1/s, ...}");
+    const c10::cuda::CUDAGuard guard(a.device());
+    const int64_t M = a.size(0), K = a.size(1), N = b.size(0);
+    TORCH_CHECK(b.size(1) == K, "gemm_fp8_acc_f32: contraction sizes differ (", K, " vs ", b.size(1), ")");
+    TORCH_CHECK(K % 16 == 0 && N % 8 == 0, "gemm_fp8_acc_f32: K must be a multiple of 16 and N of 8");
+    TORCH_CHECK(out.is_cuda() && out.scalar_type() == torch::kFloat32 && out.dim() == 2 && out.size(0) == M && out.size(1) == N && out.stride(1) == 1 &&
+                out.stride(0) % 8 == 0 && out.stride(0) >= N && (uintptr_t)out.data_ptr() % 16 == 0,
+                "gemm_fp8_acc_f32: out must be a [M,N] CUDA fp32 matrix with 16-byte aligned rows");
+    int sms = sm_count();
+    if (max_ctas > 0 && max_ctas < sms) sms = (int)max_ctas;
+    const int rc = acco_gemm_fp8_acc_f32(a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), out.data_ptr<float>(), out.stride(0), (int)M, (int)N,
+                                         (int)K, a.scalar_type() == torch::kFloat8_e5m2 ? 1 : 0, scale_a.data_ptr<float>() + 1,
+                                         scale_b.data_ptr<float>() + 1, (int)bn, (int)splits, sms, stream());
+    TORCH_CHECK(rc == 0, "gemm_fp8_acc_f32 launch failed, code ", rc, " (M=", M, " N=", N, " K=", K, ")");
 }
 
 // heuristic's pick for a shape: {bn, splits, pm, pn, rows per CTA / 128}
@@ -669,6 +765,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     TORCH_CHECK(acco_round_params_size() == (int)sizeof(RoundParams), "RoundParams layout mismatch between bindings.cpp and rs_adam_ag.cu");
     m.def("norm_fwd", &norm_fwd);
     m.def("norm_bwd", &norm_bwd);
+    m.def("norm_bwd_acc_f32", &norm_bwd_acc_f32);
     m.def("gelu_fwd", &gelu_fwd);
     m.def("gelu_bwd", &gelu_bwd);
     m.def("rope_qkv_inplace", &rope_qkv_inplace);
@@ -676,6 +773,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("swiglu_fwd", &swiglu_fwd);
     m.def("swiglu_bwd", &swiglu_bwd);
     m.def("embedding_bwd", &embedding_bwd);
+    m.def("embedding_bwd_f32", &embedding_bwd_f32);
     m.def("ce_fwd", &ce_fwd, py::arg("logits"), py::arg("labels"), py::arg("V"), py::arg("ignore_index"), py::arg("label_smoothing") = 0.0);
     m.def("ce_bwd_inplace", &ce_bwd_inplace, py::arg("logits"), py::arg("labels"), py::arg("lse"), py::arg("scale"), py::arg("V"),
           py::arg("ignore_index"), py::arg("label_smoothing") = 0.0);
@@ -693,9 +791,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("mode"), py::arg("grid"), py::arg("max_norm"));
     m.def("gemm_tn", &gemm_tn);
     m.def("gemm", &gemm);
+    m.def("gemm_wgrad_f32", &gemm_wgrad_f32, py::arg("a"), py::arg("b"), py::arg("out"), py::arg("bn") = 0, py::arg("splits") = 0,
+          py::arg("max_ctas") = 0);
     m.def("gemm_choose", &gemm_choose);
     m.def("fp8_quantize", &fp8_quantize);
     m.def("gemm_fp8", &gemm_fp8);
+    m.def("gemm_fp8_acc_f32", &gemm_fp8_acc_f32, py::arg("a"), py::arg("b"), py::arg("scale_a"), py::arg("scale_b"), py::arg("out"), py::arg("bn") = 0,
+          py::arg("splits") = 0, py::arg("max_ctas") = 0);
     m.def("gemm_map_encodes", &gemm_map_encodes);
     m.def("gemm_max_clusters", &gemm_max_clusters);
     m.def("gemm_set_debug", &gemm_set_debug);

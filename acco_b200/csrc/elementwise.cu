@@ -192,11 +192,22 @@ __global__ void __launch_bounds__(256) gelu_bwd_kernel(const __nv_bfloat16* __re
 // The ids come sorted (`sorted`, stable, with the permutation `perm` back to dy rows), so each distinct row is one run.
 // A CTA owns a 256-column slice of a run: its 8 warps take the run's occurrences round-robin (up to 4 loads in flight
 // per lane), then warp 0 adds the 8 partial sums in warp order to the row.  Rows no id hits are never read or written.
+// G = float: the same with an fp32 row (an fp32 gradient accumulator), grad[r] += that sum, no rounding to bf16.
 constexpr int kEmbWarps = 8, kEmbCols = 8 * kWarp, kEmbUnroll = 4;
-__global__ void __launch_bounds__(kEmbWarps * kWarp) embedding_bwd_kernel(__nv_bfloat16* __restrict__ grad,
-                                                                       const long long* __restrict__ sorted,
-                                                                       const long long* __restrict__ perm,
-                                                                       const __nv_bfloat16* __restrict__ dy, int T, int H) {
+ACCO_DEVINL void load_row8(const __nv_bfloat16* row, float (&s)[8]) { unpack8(ld_vec(row), s); }
+ACCO_DEVINL void store_row8(__nv_bfloat16* row, const float (&s)[8]) { st_vec(row, pack8(s)); }
+ACCO_DEVINL void load_row8(const float* row, float (&s)[8]) {
+    const float4 a = reinterpret_cast<const float4*>(row)[0], b = reinterpret_cast<const float4*>(row)[1];
+    s[0] = a.x; s[1] = a.y; s[2] = a.z; s[3] = a.w; s[4] = b.x; s[5] = b.y; s[6] = b.z; s[7] = b.w;
+}
+ACCO_DEVINL void store_row8(float* row, const float (&s)[8]) {
+    reinterpret_cast<float4*>(row)[0] = make_float4(s[0], s[1], s[2], s[3]);
+    reinterpret_cast<float4*>(row)[1] = make_float4(s[4], s[5], s[6], s[7]);
+}
+
+template <typename G>
+ACCO_DEVINL void embedding_bwd_body(G* __restrict__ grad, const long long* __restrict__ sorted, const long long* __restrict__ perm,
+                                    const __nv_bfloat16* __restrict__ dy, int T, int H) {
     __shared__ float part[kEmbWarps][kEmbCols];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     const int col = blockIdx.y * kEmbCols + 8 * lane;
@@ -227,9 +238,9 @@ __global__ void __launch_bounds__(kEmbWarps * kWarp) embedding_bwd_kernel(__nv_b
         for (int k = 0; k < 8; ++k) part[w][8 * lane + k] = acc[k];
         __syncthreads();
         if (w == 0 && live) {
-            __nv_bfloat16* row = grad + (size_t)r * H + col;
+            G* row = grad + (size_t)r * H + col;
             float s[8];
-            unpack8(ld_vec(row), s);
+            load_row8(row, s);
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
                 float t = part[0][8 * lane + k];
@@ -237,10 +248,20 @@ __global__ void __launch_bounds__(kEmbWarps * kWarp) embedding_bwd_kernel(__nv_b
                 for (int q = 1; q < kEmbWarps; ++q) t += part[q][8 * lane + k];
                 s[k] += t;
             }
-            st_vec(row, pack8(s));
+            store_row8(row, s);
         }
         __syncthreads();
     }
+}
+__global__ void __launch_bounds__(kEmbWarps * kWarp) embedding_bwd_kernel(__nv_bfloat16* __restrict__ grad, const long long* __restrict__ sorted,
+                                                                       const long long* __restrict__ perm,
+                                                                       const __nv_bfloat16* __restrict__ dy, int T, int H) {
+    embedding_bwd_body(grad, sorted, perm, dy, T, H);
+}
+__global__ void __launch_bounds__(kEmbWarps * kWarp) embedding_bwd_kernel(float* __restrict__ grad, const long long* __restrict__ sorted,
+                                                                       const long long* __restrict__ perm,
+                                                                       const __nv_bfloat16* __restrict__ dy, int T, int H) {
+    embedding_bwd_body(grad, sorted, perm, dy, T, H);
 }
 
 static int grid_for(long long work_items, int threads, int sms) {
@@ -273,14 +294,24 @@ extern "C" int acco_rope_pack_bwd(const void* dq, const void* dk, const void* dv
     return 0;
 }
 
-extern "C" int acco_embedding_bwd(void* grad, const long long* sorted, const long long* perm, const void* dy, int T, int H, int sms,
-                                  cudaStream_t st) {
+template <typename G>
+static int embedding_bwd(G* grad, const long long* sorted, const long long* perm, const void* dy, int T, int H, int sms, cudaStream_t st) {
     if (H % 8 != 0) return -1;
     if (T == 0) return 0;
     const dim3 grid(T < 4 * sms ? T : 4 * sms, (H + acco::kEmbCols - 1) / acco::kEmbCols);
-    acco::embedding_bwd_kernel<<<grid, acco::kEmbWarps * acco::kWarp, 0, st>>>((__nv_bfloat16*)grad, sorted, perm,
-                                                                              (const __nv_bfloat16*)dy, T, H);
+    acco::embedding_bwd_kernel<<<grid, acco::kEmbWarps * acco::kWarp, 0, st>>>(grad, sorted, perm, (const __nv_bfloat16*)dy, T, H);
     return (int)cudaGetLastError();
+}
+
+extern "C" int acco_embedding_bwd(void* grad, const long long* sorted, const long long* perm, const void* dy, int T, int H, int sms,
+                                  cudaStream_t st) {
+    return embedding_bwd((__nv_bfloat16*)grad, sorted, perm, dy, T, H, sms, st);
+}
+
+// grad: fp32 [R, H] rows (an fp32 gradient accumulator); dy stays bf16
+extern "C" int acco_embedding_bwd_f32(float* grad, const long long* sorted, const long long* perm, const void* dy, int T, int H, int sms,
+                                      cudaStream_t st) {
+    return embedding_bwd(grad, sorted, perm, dy, T, H, sms, st);
 }
 
 extern "C" int acco_swiglu_fwd(const void* gu, void* out, long long T, int I, int sms, cudaStream_t st) {

@@ -5,7 +5,7 @@
 //   forward   Y  = X  * W^T      A = X  (K-major)    B = W  (K-major)                      ("TN")
 //   dgrad     dX = dY * W        A = dY (K-major)    B = W  stored [K, N] -> MN-major      ("NN")
 //   wgrad     dW += dY^T * X     A = dY stored [K, M] -> MN-major,  B = X stored [K, N] -> MN-major, split-K,
-//                                epilogue = add into the bf16 gradient arena (beta = 1)
+//                                epilogue = add into the bf16 gradient arena (beta = 1), or into an fp32 one (gemm_f32acc_kernel)
 //
 // and its weight operand can be ALL-GATHERED ON THE FLY: W is a weight matrix living in the flat parameter arena.  After an ACCO
 // round the fresh values of a row-block of W exist only on the rank that owns that slice of the arena (the round kernel can skip
@@ -195,7 +195,19 @@ __device__ __forceinline__ void fp8_out_scale(float inv_a, float inv_b, float& p
     pre = d < -126 ? 0.f : __uint_as_float((uint32_t)(d + 127) << 23);   // below 2^-126 the output is far below bf16's normal range
 }
 
-template <int BN, int A_MN, int B_MN, int OP>
+__device__ __forceinline__ float2 ld_shared_f32x2(uint32_t addr) {
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_shared_f32x2(uint32_t addr, float a, float b) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
+}
+
+// F32D: D is fp32 (an fp32 gradient accumulator under bf16 weights).  The epilogue then stages 64 x 32 fp32 sub-tiles - a 128-byte
+// swizzled row holds 32 floats - through the same 8 KiB buffers, and the TMA unit reads C / writes and reduce-adds D in fp32: with one
+// K split D += tile is exact up to the one fp32 add per element, with split-K each split's partial is added in fp32.
+template <int BN, int A_MN, int B_MN, int OP, bool F32D = false>
 __device__ __forceinline__ void gemm_body(const Params& P) {
     static_assert(OP == OP_BF16 || (A_MN == 0 && B_MN == 0), "FP8 wgmma has no transpose: both operands K-major");
     constexpr int BKE = OP ? 2 * BK : BK;                  // elements per k-block (128 bytes per row in both formats)
@@ -341,7 +353,8 @@ __device__ __forceinline__ void gemm_body(const Params& P) {
         // epilogue: BN / 64 sub-tiles of 64 x 64 through this warpgroup's two staging buffers (sub-tile s uses buffer s % 2); thread 0
         // of the warpgroup issues the TMA traffic.  Before a buffer is rewritten, the store that last read it must be done reading:
         // the bulk group two commits back (one back with a single sub-tile per tile).
-        constexpr int NSUB = BN / 64;
+        constexpr int SUBW = F32D ? 32 : 64;               // output columns per staged sub-tile (128 B rows)
+        constexpr int NSUB = BN / SUBW;
         constexpr int NPRE = NSUB < 2 ? NSUB : 2;          // C sub-tiles prefetched during the mainloop (beta = 1, one split)
         uint8_t* epi = epi_smem + cw * 2 * EPI_BUF_BYTES;
         uint64_t* cbar = c_bar + cw * 2;
@@ -354,7 +367,7 @@ __device__ __forceinline__ void gemm_body(const Params& P) {
         };
         auto load_c_sub = [&](const Unit& u, int s) {
             mbar_expect_tx(&cbar[s & 1], (uint32_t)EPI_BUF_BYTES);
-            tma_load_2d(&P.map_d, &cbar[s & 1], epi + (s & 1) * EPI_BUF_BYTES, u.n_blk * BN + s * 64, u.mb * BM + cw * 64);
+            tma_load_2d(&P.map_d, &cbar[s & 1], epi + (s & 1) * EPI_BUF_BYTES, u.n_blk * BN + s * SUBW, u.mb * BM + cw * 64);
         };
         float acc[BN / 2];
 #pragma unroll
@@ -425,8 +438,10 @@ __device__ __forceinline__ void gemm_body(const Params& P) {
             }
             // ---------------- epilogue: fragment (row 16 warp + lane/4 (+8), columns 8 j + 2 (lane % 4) (+1)) -> staging -> TMA
             const int m0 = u.mb * BM + cw * 64;
-            // my rows r = 16 warp + lane / 4 (+8) of the 64-row half; r % 8 = lane / 4 sets the swizzle of both
-            const uint32_t row_addr = smem_u32(epi) + (uint32_t)((warp * 16 + (lane >> 2)) * 128 + 4 * (lane & 3));
+            // my rows r = 16 warp + lane / 4 (+8) of the 64-row half; r % 8 = lane / 4 sets the swizzle of both.  My two columns of
+            // a fragment group are 4 bf16 bytes at 4 (lane % 4) of its 16-byte chunk, or 8 fp32 bytes at 8 (lane % 2) of chunk lane % 4 / 2
+            // of its two chunks.
+            const uint32_t row_addr = smem_u32(epi) + (uint32_t)((warp * 16 + (lane >> 2)) * 128 + (F32D ? 8 * (lane & 1) : 4 * (lane & 3)));
             const int colb = u.n_blk * BN + 2 * (lane & 3);
             const bool bias_on = P.bias != nullptr && u.kb0 == 0;
 #pragma unroll
@@ -445,15 +460,16 @@ __device__ __forceinline__ void gemm_body(const Params& P) {
                     named_barrier(bar_id, 128);
                 }
 #pragma unroll
-                for (int jj = 0; jj < 8; ++jj) {
-                    const int j = s * 8 + jj;
+                for (int jj = 0; jj < SUBW / 8; ++jj) {
+                    const int j = s * (SUBW / 8) + jj;
                     const int col = colb + 8 * j;
                     float b0 = 0.f, b1 = 0.f;
                     if (bias_on && col < P.N) {                    // N % 8 == 0: col < N implies col + 1 < N
                         const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(P.bias + col));
                         b0 = f.x; b1 = f.y;
                     }
-                    const uint32_t chunk_addr = buf_addr + (uint32_t)((jj ^ (lane >> 2)) << 4);
+                    const int chunk = F32D ? 2 * jj + ((lane & 3) >> 1) : jj;
+                    const uint32_t chunk_addr = buf_addr + (uint32_t)((chunk ^ (lane >> 2)) << 4);
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
                         const uint32_t dst = chunk_addr + h * 8 * 128;
@@ -465,21 +481,29 @@ __device__ __forceinline__ void gemm_body(const Params& P) {
                             v0 = acc[4 * j + 2 * h] + b0;
                             v1 = acc[4 * j + 2 * h + 1] + b1;
                         }
-                        if (load_c) {
-                            // beta = 1 with a single K split: exact fp32 accumulate (one rounding), nobody else touches this tile
-                            const uint32_t cv = ld_shared_u32(dst);
-                            const float2 c = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&cv));
-                            v0 += c.x; v1 += c.y;
+                        if constexpr (F32D) {
+                            if (load_c) {
+                                const float2 c = ld_shared_f32x2(dst);
+                                v0 += c.x; v1 += c.y;
+                            }
+                            st_shared_f32x2(dst, v0, v1);
+                        } else {
+                            if (load_c) {
+                                // beta = 1 with a single K split: exact fp32 accumulate (one rounding), nobody else touches this tile
+                                const uint32_t cv = ld_shared_u32(dst);
+                                const float2 c = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&cv));
+                                v0 += c.x; v1 += c.y;
+                            }
+                            st_shared_u32(dst, pack_bf16x2(v0, v1));
                         }
-                        st_shared_u32(dst, pack_bf16x2(v0, v1));
                     }
                 }
                 fence_async_smem();                        // my st.shared -> visible to the TMA engine
                 named_barrier(bar_id, 128);
                 if (tid == 0) {
                     // ragged rows / columns fall outside map_d's extents and are dropped by the TMA unit
-                    if (P.atomic) tma_reduce_add_2d(&P.map_d, buf, u.n_blk * BN + s * 64, m0);
-                    else tma_store_2d(&P.map_d, buf, u.n_blk * BN + s * 64, m0);
+                    if (P.atomic) tma_reduce_add_2d(&P.map_d, buf, u.n_blk * BN + s * SUBW, m0);
+                    else tma_store_2d(&P.map_d, buf, u.n_blk * BN + s * SUBW, m0);
                     bulk_commit();
                 }
             }
@@ -512,6 +536,16 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_kernel(const __grid_constant_
 template <int BN, int OP>
 __global__ void __launch_bounds__(THREADS, 1) gemm_fp8_kernel(const __grid_constant__ Params P) {
     gemm_body<BN, 0, 0, OP>(P);
+}
+
+// Accumulating GEMMs into an fp32 D (F32D): the wgrad layout (both operands MN-major) at every tile width, and the FP8 GEMM
+template <int BN>
+__global__ void __launch_bounds__(THREADS, 1) gemm_f32acc_kernel(const __grid_constant__ Params P) {
+    gemm_body<BN, 1, 1, OP_BF16, true>(P);
+}
+template <int BN, int OP>
+__global__ void __launch_bounds__(THREADS, 1) gemm_fp8_f32acc_kernel(const __grid_constant__ Params P) {
+    gemm_body<BN, 0, 0, OP, true>(P);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -625,6 +659,14 @@ static KernelFn fp8_kernel_for(int bn, int op) {
     return op == OP_E5M2 ? gemm_fp8_kernel<64, OP_E5M2> : gemm_fp8_kernel<64, OP_E4M3>;
 }
 
+static KernelFn f32acc_kernel_for(int bn) {
+    return bn == 256 ? gemm_f32acc_kernel<256> : bn == 128 ? gemm_f32acc_kernel<128> : gemm_f32acc_kernel<64>;
+}
+static KernelFn fp8_f32acc_kernel_for(int bn, int op) {
+    if (bn == 128) return op == OP_E5M2 ? gemm_fp8_f32acc_kernel<128, OP_E5M2> : gemm_fp8_f32acc_kernel<128, OP_E4M3>;
+    return op == OP_E5M2 ? gemm_fp8_f32acc_kernel<64, OP_E5M2> : gemm_fp8_f32acc_kernel<64, OP_E4M3>;
+}
+
 static int g_pm = 0, g_pn = 0;                     // ACCO_GEMM_CLUSTER="pm,pn": force the cluster shape (0 = heuristic)
 static unsigned long long* g_dbg = nullptr;        // device buffer for phase time stamps (acco_gemm_set_debug)
 static int g_pdl = 1;                              // ACCO_GEMM_PDL=0: no programmatic dependent launch
@@ -638,7 +680,11 @@ static int init_once() {
                     if (cudaFuncSetAttribute(kernel_for(bn, a, b), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) rc = -4;
         for (int bn : {64, 128})
             for (int op : {OP_E4M3, OP_E5M2})
-                if (cudaFuncSetAttribute(fp8_kernel_for(bn, op), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) rc = -4;
+                if (cudaFuncSetAttribute(fp8_kernel_for(bn, op), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess ||
+                    cudaFuncSetAttribute(fp8_f32acc_kernel_for(bn, op), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess)
+                    rc = -4;
+        for (int bn : {64, 128, 256})
+            if (cudaFuncSetAttribute(f32acc_kernel_for(bn), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) rc = -4;
         const char* e;
         if ((e = getenv("ACCO_GEMM_CLUSTER")) && e[0] && e[1] == ',') { g_pm = e[0] - '0'; g_pn = e[2] - '0'; }
         if ((e = getenv("ACCO_GEMM_PDL")) && e[0] == '0') g_pdl = 0;
@@ -766,8 +812,10 @@ struct GatherArgs {
 
 static int launch(const void* a, long long lda, int a_mn, const void* b, long long ldb, int b_mn, void* d, long long ldd, const void* bias, int M,
                   int N, int K, int accumulate, int bn_req, int splits_req, int pm_req, int pn_req, int msub_req, const GatherArgs* ga, int sms,
-                  cudaStream_t st, int op = OP_BF16, const float* inv_a = nullptr, const float* inv_b = nullptr) {
+                  cudaStream_t st, int op = OP_BF16, const float* inv_a = nullptr, const float* inv_b = nullptr, int f32d = 0) {
     if (M <= 0 || N <= 0 || K <= 0) return -1;
+    // fp32 D: accumulate only, no bias, and (bf16) the wgrad operand layout - the instantiations that exist
+    if (f32d && (!accumulate || bias || (ga && ga->n_peers > 0) || (!op && !(a_mn && b_mn)))) return -1;
     if ((lda % 8) || (ldb % 8) || (ldd % 8) || (N % 8)) return -1;
     const int eb = op ? 1 : 2, bke = op ? 2 * BK : BK;                     // operand bytes per element, elements per k-block
     if (op && (a_mn || b_mn || (lda % 16) || (ldb % 16) || (K % 16) || bn_req > 128 || !inv_a || !inv_b || (ga && ga->n_peers > 0))) return -1;
@@ -806,7 +854,8 @@ static int launch(const void* a, long long lda, int a_mn, const void* b, long lo
         }
     }
     // the output map spans exactly the (M, N) view of D: the TMA stores of ragged tiles cannot reach the elements around it
-    rc = make_map(&P.map_d, d, (uint64_t)N, (uint64_t)M, (uint64_t)ldd, 64, 64);
+    rc = f32d ? make_map_typed(&P.map_d, d, (uint64_t)N, (uint64_t)M, (uint64_t)ldd, 32, 64, 4)
+              : make_map(&P.map_d, d, (uint64_t)N, (uint64_t)M, (uint64_t)ldd, 64, 64);
     if (rc) return rc;
     P.bias = (const __nv_bfloat16*)bias;
     P.out = (__nv_bfloat16*)d;
@@ -868,7 +917,8 @@ static int launch(const void* a, long long lda, int a_mn, const void* b, long lo
     }
     cfg.attrs = attr;
     cfg.numAttrs = na;
-    return (int)cudaLaunchKernelEx(&cfg, op ? fp8_kernel_for(bn, op) : kernel_for(bn, a_mn, b_mn), P);
+    const KernelFn fn = f32d ? (op ? fp8_f32acc_kernel_for(bn, op) : f32acc_kernel_for(bn)) : (op ? fp8_kernel_for(bn, op) : kernel_for(bn, a_mn, b_mn));
+    return (int)cudaLaunchKernelEx(&cfg, fn, P);
 }
 
 }  // namespace acco_gemm
@@ -898,6 +948,21 @@ extern "C" int acco_gemm_fp8_run(const void* a, long long lda, const void* b, lo
                                  cudaStream_t st) {
     return acco_gemm::launch(a, lda, 0, b, ldb, 0, d, ldd, bias, M, N, K, accumulate, bn_req, splits_req, 0, 0, 0, nullptr, sms, st,
                              a_e5m2 ? acco_gemm::OP_E5M2 : acco_gemm::OP_E4M3, inv_a, inv_b);
+}
+
+// wgrad into an fp32 gradient: D[M,N] (fp32, row stride ldd) += A * B^T with A stored [K, M] and B stored [K, N] (both MN-major,
+// bf16).  One K split adds the tile to D exactly (one fp32 add per element); split-K adds each split's fp32 partial through the TMA unit.
+extern "C" int acco_gemm_wgrad_f32(const void* a, long long lda, const void* b, long long ldb, float* d, long long ldd, int M, int N, int K,
+                                   int bn_req, int splits_req, int sms, cudaStream_t st) {
+    return acco_gemm::launch(a, lda, 1, b, ldb, 1, d, ldd, nullptr, M, N, K, 1, bn_req, splits_req, 0, 0, 0, nullptr, sms, st, acco_gemm::OP_BF16,
+                             nullptr, nullptr, 1);
+}
+
+// FP8 into an fp32 D: D[M,N] += A[M,K] * B[N,K]^T * (inv_a[0] * inv_b[0]), operands as in acco_gemm_fp8_run
+extern "C" int acco_gemm_fp8_acc_f32(const void* a, long long lda, const void* b, long long ldb, float* d, long long ldd, int M, int N, int K,
+                                     int a_e5m2, const float* inv_a, const float* inv_b, int bn_req, int splits_req, int sms, cudaStream_t st) {
+    return acco_gemm::launch(a, lda, 0, b, ldb, 0, d, ldd, nullptr, M, N, K, 1, bn_req, splits_req, 0, 0, 0, nullptr, sms, st,
+                             a_e5m2 ? acco_gemm::OP_E5M2 : acco_gemm::OP_E4M3, inv_a, inv_b, 1);
 }
 
 extern "C" int acco_gemm_tile_n() { return acco_gemm::BN_MAX; }

@@ -12,6 +12,7 @@
 // One WARP per row for H <= 1024 (every 16-byte vector of the row in flight at once, no block barrier in the row loop);
 // one CTA per row above that, up to H = 16384.  Both walk the rows grid-stride (persistent).
 #include "common.cuh"
+#include <type_traits>
 
 namespace acco {
 
@@ -230,10 +231,11 @@ __global__ void __launch_bounds__(CTA_ROW ? kMaxCtaThreads : kWarpsPerCta * 32) 
 }
 
 // out[col] = sum_p partial[p][col]   (deterministic).  Block (32, 32): 32 columns x 32 partial-groups.
-// If `accum` is given the sum is ADDED to the bf16 gradient there (fused AccumulateGrad), else it
-// is written to fp32 `out`.
+// If `accum` is given the sum is ADDED to the gradient there (fused AccumulateGrad; G = bf16: one rounding, G = float: an fp32
+// gradient accumulator), else it is written to fp32 `out`.
+template <typename G>
 __global__ void __launch_bounds__(1024) reduce_partials_kernel(const float* __restrict__ partial, float* __restrict__ out,
-                                                               __nv_bfloat16* __restrict__ accum, int nparts, int H, int pitch) {
+                                                               G* __restrict__ accum, int nparts, int H, int pitch) {
     __shared__ float sm[32][33];
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
     const int col = blockIdx.x * 32 + tx;
@@ -252,14 +254,19 @@ __global__ void __launch_bounds__(1024) reduce_partials_kernel(const float* __re
         float s = 0.f;
 #pragma unroll
         for (int k = 0; k < 32; ++k) s += sm[k][tx];
-        if (accum) accum[col] = __float2bfloat16(__bfloat162float(accum[col]) + s);
-        else out[col] = s;
+        if (accum) {
+            if constexpr (std::is_same<G, float>::value) accum[col] += s;
+            else accum[col] = __float2bfloat16(__bfloat162float(accum[col]) + s);
+        } else {
+            out[col] = s;
+        }
     }
 }
 
-// out[col] (fp32) = or accum[col] (bf16) += sum_p partial[p * pitch + col], col < width
-static void reduce_partials(const float* partial, float* out, void* accum_bf16, int nparts, int width, int pitch, cudaStream_t st) {
-    reduce_partials_kernel<<<(width + 31) / 32, 1024, 0, st>>>(partial, out, (__nv_bfloat16*)accum_bf16, nparts, width, pitch);
+// out[col] (fp32) = or accum[col] (bf16, or fp32 when accum_f32) += sum_p partial[p * pitch + col], col < width
+static void reduce_partials(const float* partial, float* out, void* accum, int accum_f32, int nparts, int width, int pitch, cudaStream_t st) {
+    if (accum_f32) reduce_partials_kernel<float><<<(width + 31) / 32, 1024, 0, st>>>(partial, out, (float*)accum, nparts, width, pitch);
+    else reduce_partials_kernel<__nv_bfloat16><<<(width + 31) / 32, 1024, 0, st>>>(partial, out, (__nv_bfloat16*)accum, nparts, width, pitch);
 }
 
 // CTA-per-row geometry (H > 1024): the fewest 16-byte vectors per thread (a power of two) that keep the row within
@@ -360,20 +367,32 @@ extern "C" int acco_norm_fwd(const void* a, const void* r, const void* w, const 
     return (int)cudaGetLastError();
 }
 
-// RMSNorm when mean == nullptr, LayerNorm otherwise.  partial: grid * NP * H floats.  dw (| db) are written to fp32
-// `dwdb_out` [NP * H], or, when `dw_accum` is given (and `db_accum` for LayerNorm), added in place to those bf16 gradients.
-extern "C" int acco_norm_bwd(const void* dy, const void* dh_extra, const void* h, const void* w, const float* mean, const float* rstd,
-                             void* dh, float* partial, float* dwdb_out, void* dw_accum, void* db_accum, int T, int H, int grid,
-                             cudaStream_t st) {
+static int norm_bwd(const void* dy, const void* dh_extra, const void* h, const void* w, const float* mean, const float* rstd, void* dh,
+                    float* partial, float* dwdb_out, void* dw_accum, void* db_accum, int accum_f32, int T, int H, int grid, cudaStream_t st) {
     if (!acco::supported(H)) return -1;
     ACCO_NORM_DISPATCH(H, acco::launch_bwd, dy, dh_extra, h, w, mean, rstd, dh, partial, T, H, grid, st);
     const int width = (mean ? 2 : 1) * H;
     // one reduction over the whole partial row when it lands in fp32, one per parameter when accumulated into the arena
     if (dw_accum) {
-        acco::reduce_partials(partial, nullptr, dw_accum, grid, H, width, st);
-        if (mean) acco::reduce_partials(partial + H, nullptr, db_accum, grid, H, width, st);
+        acco::reduce_partials(partial, nullptr, dw_accum, accum_f32, grid, H, width, st);
+        if (mean) acco::reduce_partials(partial + H, nullptr, db_accum, accum_f32, grid, H, width, st);
     } else {
-        acco::reduce_partials(partial, dwdb_out, nullptr, grid, width, width, st);
+        acco::reduce_partials(partial, dwdb_out, nullptr, 0, grid, width, width, st);
     }
     return (int)cudaGetLastError();
+}
+
+// RMSNorm when mean == nullptr, LayerNorm otherwise.  partial: grid * NP * H floats.  dw (| db) are written to fp32
+// `dwdb_out` [NP * H], or, when `dw_accum` is given (and `db_accum` for LayerNorm), added in place to those bf16 gradients.
+extern "C" int acco_norm_bwd(const void* dy, const void* dh_extra, const void* h, const void* w, const float* mean, const float* rstd,
+                             void* dh, float* partial, float* dwdb_out, void* dw_accum, void* db_accum, int T, int H, int grid,
+                             cudaStream_t st) {
+    return norm_bwd(dy, dh_extra, h, w, mean, rstd, dh, partial, dwdb_out, dw_accum, db_accum, 0, T, H, grid, st);
+}
+
+// As acco_norm_bwd with the sums added to fp32 gradients dw_accum [H] (and db_accum [H] for LayerNorm), both required.
+extern "C" int acco_norm_bwd_acc_f32(const void* dy, const void* dh_extra, const void* h, const void* w, const float* mean, const float* rstd,
+                                     void* dh, float* partial, float* dw_accum, float* db_accum, int T, int H, int grid, cudaStream_t st) {
+    if (!dw_accum || (mean && !db_accum)) return -1;
+    return norm_bwd(dy, dh_extra, h, w, mean, rstd, dh, partial, nullptr, dw_accum, db_accum, 1, T, H, grid, st);
 }

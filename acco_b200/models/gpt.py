@@ -176,7 +176,7 @@ class GPTForCausalLM(NativeCausalLM):
         scale = (1.0 / math.sqrt(D)) if cfg.scale_attn else 1.0
         seg = None
         if position_ids is None:
-            h = (ops.embedding(input_ids.reshape(T), tr.wte).view(B, S, H) + tr.wpe[:S]).view(T, H)
+            h = (ops.embedding(input_ids.reshape(T), tr.wte).view(B, S, H) + ops.main_grad_param(tr.wpe, S)).view(T, H)
         else:
             h = ops.embedding(input_ids.reshape(T), tr.wte) + ops.embedding(position_ids.reshape(T), tr.wpe)
             seg = ops.segment_starts(position_ids)

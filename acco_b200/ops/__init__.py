@@ -101,6 +101,36 @@ def use_kernels(*tensors: torch.Tensor, bf16_only: bool = True) -> bool:
         f"({_EXT_ERR}). Build it with __graft_entry__.build() or set ACCO_ALLOW_FALLBACK=1.")
 
 
+def accum_grad(p: torch.Tensor) -> Optional[torch.Tensor]:
+    """The gradient accumulator a backward adds ``p``'s gradient into: ``p.main_grad`` when the arena binds one (fp32 accumulators
+    under bf16 weights, train key ``grad_accum_dtype``), else ``p.grad`` (None when neither exists)."""
+    g = getattr(p, "main_grad", None)
+    return g if g is not None else p.grad
+
+
+class _IntoMainGrad(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, p, rows, dtype):
+        ctx.target = p.main_grad if rows is None else p.main_grad[:rows]
+        x = p.detach() if rows is None else p.detach()[:rows]
+        return x.to(dtype, copy=True)
+
+    @staticmethod
+    def backward(ctx, g):
+        ctx.target.add_(g.to(ctx.target.dtype))
+        return None, None, None
+
+
+def main_grad_param(p: torch.Tensor, rows: Optional[int] = None, dtype: Optional[torch.dtype] = None) -> torch.Tensor:
+    """``p`` (or ``p[:rows]``) for a plain torch op of the forward.  When ``p`` has a ``main_grad``, a copy (in ``dtype``, default
+    ``p``'s) whose gradient autograd adds into ``p.main_grad`` in its dtype, so no ``.grad`` is created beside the arena; otherwise
+    ``p`` itself (or its slice), unchanged."""
+    x = p if rows is None else p[:rows]
+    if getattr(p, "main_grad", None) is None or not (torch.is_grad_enabled() and p.requires_grad):
+        return x
+    return _IntoMainGrad.apply(p, rows, dtype or p.dtype)
+
+
 from .norm import rmsnorm, add_rmsnorm, rmsnorm_ref, add_rmsnorm_ref, layernorm, add_layernorm, layernorm_ref, add_layernorm_ref  # noqa: E402
 from .rope import rope_qkv, rope_qkv_ref, apply_rope_ref, rope_tables  # noqa: E402
 from .embedding import embedding  # noqa: E402
@@ -111,7 +141,7 @@ from .attention import causal_attention, causal_attention_ref, rope_causal_atten
 from .adam import fused_adamw_shard, grad_sumsq  # noqa: E402
 
 __all__ = [
-    "load_ext", "have_ext", "use_kernels", "ext_path",
+    "load_ext", "have_ext", "use_kernels", "ext_path", "accum_grad", "main_grad_param",
     "count_launch", "launch_counts", "reset_launch_counts", "total_launches",
     "rmsnorm", "add_rmsnorm", "rmsnorm_ref", "add_rmsnorm_ref",
     "layernorm", "add_layernorm", "gelu_new", "layernorm_ref", "add_layernorm_ref", "gelu_new_ref",

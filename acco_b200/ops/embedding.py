@@ -34,6 +34,18 @@ def embedding_bwd_ref(grad: torch.Tensor, ids: torch.Tensor, dy: torch.Tensor) -
     grad.index_put_((row,), (grad[row].float() + acc).to(grad.dtype))
 
 
+def embedding_bwd_f32(grad: torch.Tensor, ids: torch.Tensor, dy: torch.Tensor) -> None:
+    """Add the bf16 rows of ``dy [T, H]`` into an fp32 ``grad [R, H]`` (an fp32 gradient accumulator) at ``ids [T]``: per row hit,
+    ``grad[r] += sum_{i: ids[i] = r} dy[i]`` with the sum in fp32, in the order of the module docstring's kernel, and no rounding to
+    bf16.  CUDA: the fp32-row instantiation of ``embedding_bwd_kernel``, as capturable as the bf16 one."""
+    if use_kernels(grad, dy, bf16_only=False) and dy.dtype == torch.bfloat16:
+        sorted_ids, perm = torch.sort(ids.long(), stable=True)
+        load_ext(required=True).embedding_bwd_f32(grad, sorted_ids, perm, dy.contiguous())
+        count_launch("embedding_bwd_f32")
+        return
+    grad.index_add_(0, ids, dy.float())
+
+
 def embedding_bwd(grad: torch.Tensor, ids: torch.Tensor, dy: torch.Tensor) -> None:
     """Add the rows of ``dy [T, H]`` into ``grad [R, H]`` at ``ids [T]`` (see the module docstring)."""
     if use_kernels(grad):
@@ -61,6 +73,9 @@ class EmbeddingFn(torch.autograd.Function):
         w = ctx.weight_ref
         flat_ids = ids.reshape(-1)
         dy2 = dy.reshape(-1, dy.shape[-1])
+        if ctx.accumulate and getattr(w, "main_grad", None) is not None:
+            embedding_bwd_f32(w.main_grad, flat_ids, dy2)
+            return None, None, None
         if ctx.accumulate and w.grad is not None:
             embedding_bwd(w.grad, flat_ids, dy2)
             return None, None, None

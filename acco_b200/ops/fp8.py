@@ -83,6 +83,11 @@ def gemm_fp8(a, b, scale_a, scale_b, out=None, bias=None, accumulate=False, bn: 
     persistent grid (as in :func:`ops.gemm.gemm`)."""
     if not use_kernels(a, b, bf16_only=False):
         return gemm_fp8_ref(a, b, scale_a, scale_b, out, bias, accumulate)
+    if out is not None and out.dtype == torch.float32 and accumulate and bias is None:
+        # an fp32 gradient accumulator: the fp32-output instantiation adds the tile's fp32 sum without rounding to bf16
+        load_ext(required=True).gemm_fp8_acc_f32(a, b, scale_a, scale_b, out, int(bn), int(splits), int(max_ctas))
+        count_launch("gemm_fp8_f32acc")
+        return out
     y = load_ext(required=True).gemm_fp8(a, b, scale_a, scale_b, out, bias, bool(accumulate), int(bn), int(splits), int(max_ctas))
     count_launch("gemm_fp8")
     return y
@@ -131,7 +136,13 @@ class Fp8LinearFn(torch.autograd.Function):
                 dx = gemm_fp8(qg, qwT, sg, sw).view(ctx.x_shape)
             if need_dw:
                 w = ctx.weight_ref
-                if ctx.accumulate and w.grad is not None and _arena_view(w.grad):
+                main = getattr(w, "main_grad", None)
+                if ctx.accumulate and main is not None:
+                    if _arena_view(main, torch.float32):
+                        gemm_fp8(qgT, qxT, sg, sx, out=main, accumulate=True)  # fp32 accumulator: fp32 sum added, no bf16 rounding
+                    else:
+                        main.add_(gemm_fp8_ref(qgT, qxT, sg, sx, dtype=torch.float32))
+                elif ctx.accumulate and w.grad is not None and _arena_view(w.grad):
                     gemm_fp8(qgT, qxT, sg, sx, out=w.grad, accumulate=True)     # adds straight into the gradient
                 elif ctx.accumulate and w.grad is not None:
                     w.grad.add_(gemm_fp8(qgT, qxT, sg, sx).to(w.grad.dtype))
@@ -140,8 +151,9 @@ class Fp8LinearFn(torch.autograd.Function):
         return dx, dw, _bias_grad(ctx, g), None
 
 
-def _arena_view(grad: torch.Tensor) -> bool:
-    """A gradient the FP8 GEMM can add into in place: bf16, 2-D, unit inner stride, 16-byte aligned (CPU tensors: any bf16 matrix)."""
-    if grad.dtype != torch.bfloat16 or grad.dim() != 2 or grad.stride(1) != 1:
+def _arena_view(grad: torch.Tensor, dtype: torch.dtype = torch.bfloat16) -> bool:
+    """A gradient the FP8 GEMM can add into in place: ``dtype`` (bf16, or fp32 for an fp32 accumulator), 2-D, unit inner stride,
+    16-byte aligned (CPU tensors: any such matrix)."""
+    if grad.dtype != dtype or grad.dim() != 2 or grad.stride(1) != 1:
         return False
     return not grad.is_cuda or (grad.data_ptr() % 16 == 0 and grad.stride(0) % 8 == 0)

@@ -76,8 +76,22 @@ def gemm_nn(dy: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
 
 
 def gemm_tt_acc(dy: torch.Tensor, x: torch.Tensor, grad: torch.Tensor) -> torch.Tensor:
-    """wgrad: ``grad [N,K] += dy [M,N]^T @ x [M,K]`` - both operands MN-major, reduce-add epilogue into the arena view"""
+    """wgrad: ``grad [N,K] += dy [M,N]^T @ x [M,K]`` - both operands MN-major, reduce-add epilogue into the arena view.  An fp32
+    ``grad`` (fp32 gradient accumulator) takes the fp32-output instantiation: the tile's fp32 sum is added without rounding to bf16."""
+    if grad.dtype == torch.float32:
+        return gemm_wgrad_f32(dy, x, grad)
     return gemm(dy, x, out=grad, a_mn=True, b_mn=True, accumulate=True)
+
+
+def gemm_wgrad_f32(dy: torch.Tensor, x: torch.Tensor, grad: torch.Tensor, bn: int = 0, splits: int = 0, max_ctas: int = 0) -> torch.Tensor:
+    """``grad [N,K] (fp32) += dy [M,N]^T @ x [M,K]`` (bf16 operands): one K split reads, adds and writes ``grad`` in fp32 exactly once
+    per element; split-K adds each split's fp32 partial with TMA reduce-adds.  ``bn`` / ``splits`` / ``max_ctas`` as in :func:`gemm`."""
+    if not use_kernels(dy, x):
+        grad.addmm_(dy.t().float(), x.float())
+        return grad
+    load_ext(required=True).gemm_wgrad_f32(_rowmajor(dy), _rowmajor(x), grad, int(bn), int(splits), int(max_ctas))
+    count_launch("gemm_f32acc")
+    return grad
 
 
 class GatheredWeight:

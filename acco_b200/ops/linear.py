@@ -77,10 +77,13 @@ def _linear_backward(ctx, dy):
         weight_c, x2 = weight.to(dy2.dtype), x2.to(dy2.dtype)
     else:
         weight_c = weight
+    from . import accum_grad
     tc = _tc(dy2, weight_c, x2)
     w = ctx.weight_ref
-    acc_tc = (ctx.needs_input_grad[1] and ctx.accumulate and w.grad is not None and tc and w.grad.dtype == torch.bfloat16
-              and w.grad.dim() == 2 and w.grad.stride(1) == 1 and w.grad.data_ptr() % 16 == 0)
+    g = accum_grad(w)
+    main = getattr(w, "main_grad", None) is not None
+    acc_tc = (ctx.needs_input_grad[1] and ctx.accumulate and g is not None and tc and g.dtype in (torch.bfloat16, torch.float32)
+              and (g.dtype == torch.bfloat16 or main) and g.dim() == 2 and g.stride(1) == 1 and g.data_ptr() % 16 == 0)
     dx = dw = None
     side = _wgrad_stream(dy2.device) if (acc_tc and ctx.needs_input_grad[0]) else None
     if side is not None:
@@ -89,7 +92,7 @@ def _linear_backward(ctx, dy):
         cur = torch.cuda.current_stream(dy2.device)
         side.wait_stream(cur)
         with torch.cuda.stream(side):
-            gemm_tt_acc(dy2, x2, w.grad)
+            gemm_tt_acc(dy2, x2, g)
         dy2.record_stream(side)
         x2.record_stream(side)
     if ctx.needs_input_grad[0]:
@@ -101,10 +104,12 @@ def _linear_backward(ctx, dy):
     if side is not None:
         torch.cuda.current_stream(dy2.device).wait_stream(side)     # join: later kernels (and the round that consumes the arena) see dW
     elif ctx.needs_input_grad[1]:
-        if ctx.accumulate and w.grad is not None:
+        if ctx.accumulate and g is not None:
             if acc_tc:
                 from .gemm import gemm_tt_acc
-                gemm_tt_acc(dy2, x2, w.grad)             # split-K adds straight into the arena view
+                gemm_tt_acc(dy2, x2, g)                  # split-K adds straight into the arena view
+            elif main:
+                g.addmm_(dy2.t().float(), x2.float())    # fp32 accumulator: fp32 product, one fp32 add
             elif w.grad.dtype == dy2.dtype:
                 w.grad.addmm_(dy2.t(), x2)               # accumulate in the (library) GEMM epilogue
             else:
@@ -122,6 +127,9 @@ def _bias_grad(ctx, dy2):
     if not (ctx.has_bias and ctx.needs_input_grad[2]):
         return None
     b = ctx.bias_ref
+    if ctx.accumulate and getattr(b, "main_grad", None) is not None:
+        b.main_grad.add_(dy2.sum(0, dtype=torch.float32))
+        return None
     if ctx.accumulate and b.grad is not None:
         b.grad.add_(dy2.sum(0))
         return None

@@ -13,7 +13,7 @@ from typing import Tuple
 import torch
 import torch.nn.functional as F
 
-from . import count_launch, load_ext, use_kernels
+from . import accum_grad, count_launch, load_ext, main_grad_param, use_kernels
 
 _KERNEL_MAX_H = 16384
 
@@ -43,10 +43,10 @@ def _kernel_covers(H: int) -> bool:
 
 
 def _accum_target(weight):
-    """The weight's existing bf16 ``.grad`` (a view of the flat gradient arena) if dw can be
-    accumulated into it inside the reduction kernel (fused AccumulateGrad), else None."""
-    g = getattr(weight, "grad", None)
-    if g is not None and g.dtype == torch.bfloat16 and g.is_contiguous() and g.is_cuda:
+    """The weight's gradient accumulator (a view of the flat gradient arena: its bf16 ``.grad``, or its fp32 ``main_grad``) if dw can
+    be accumulated into it inside the reduction kernel (fused AccumulateGrad), else None."""
+    g = None if weight is None else accum_grad(weight)
+    if g is not None and g.dtype in (torch.bfloat16, torch.float32) and g.is_contiguous() and g.is_cuda:
         return g
     return None
 
@@ -82,7 +82,10 @@ class _NormFn(torch.autograd.Function):
         bg = _accum_target(ctx.bias_ref)
         if layer and (wg is None or bg is None):     # LayerNorm accumulates both parameters or neither
             wg = bg = None
-        dh, dwdb = C.norm_bwd(dy2, de2, h, weight, mean, rstd, wg, bg)
+        if wg is not None and wg.dtype == torch.float32:
+            dh, dwdb = C.norm_bwd_acc_f32(dy2, de2, h, weight, mean, rstd, wg, bg), None
+        else:
+            dh, dwdb = C.norm_bwd(dy2, de2, h, weight, mean, rstd, wg, bg)
         if layer:
             count_launch("layernorm_bwd", 3 if wg is not None else 2)
         else:
@@ -100,24 +103,24 @@ class _NormFn(torch.autograd.Function):
 def rmsnorm(x: torch.Tensor, weight: torch.Tensor, eps: float = 1e-5) -> torch.Tensor:
     if use_kernels(x, weight) and _kernel_covers(x.shape[-1]):
         return _NormFn.apply(x, None, weight, None, eps)
-    return rmsnorm_ref(x, weight, eps)
+    return rmsnorm_ref(x, main_grad_param(weight, dtype=torch.float32), eps)
 
 
 def add_rmsnorm(a: torch.Tensor, r: torch.Tensor, weight: torch.Tensor, eps: float = 1e-5):
     """Returns ``(rmsnorm(a + r) * weight, a + r)``."""
     if use_kernels(a, r, weight) and _kernel_covers(a.shape[-1]):
         return _NormFn.apply(a, r, weight, None, eps)
-    return add_rmsnorm_ref(a, r, weight, eps)
+    return add_rmsnorm_ref(a, r, main_grad_param(weight, dtype=torch.float32), eps)
 
 
 def layernorm(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, eps: float = 1e-5) -> torch.Tensor:
     if use_kernels(x, weight, bias) and _kernel_covers(x.shape[-1]):
         return _NormFn.apply(x, None, weight, bias, eps)
-    return layernorm_ref(x, weight, bias, eps)
+    return layernorm_ref(x, main_grad_param(weight, dtype=torch.float32), main_grad_param(bias, dtype=torch.float32), eps)
 
 
 def add_layernorm(a: torch.Tensor, r: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, eps: float = 1e-5):
     """Returns ``(layernorm(a + r), a + r)``."""
     if use_kernels(a, r, weight, bias) and _kernel_covers(a.shape[-1]):
         return _NormFn.apply(a, r, weight, bias, eps)
-    return add_layernorm_ref(a, r, weight, bias, eps)
+    return add_layernorm_ref(a, r, main_grad_param(weight, dtype=torch.float32), main_grad_param(bias, dtype=torch.float32), eps)

@@ -17,6 +17,10 @@ GPU-first redesign (no copies on the flip):
   elements, so kernels never need a ragged tail (the pad region is an all-zero fixed point of
   AdamW).  ``align=1`` reproduces the reference's slice math exactly.
 
+``grad_dtype`` other than the parameters' dtype (fp32 accumulators under bf16 weights, train key ``grad_accum_dtype``): a ``.grad``
+must have its parameter's dtype, so each trainable parameter's accumulator view is bound as ``p.main_grad`` instead and ``.grad``
+stays ``None``; the ops add into ``main_grad`` (``ops.accum_grad``).
+
 Buffers come from an ``allocator(numel, dtype) -> Tensor`` callback so the symmetric-memory
 backend can hand out NVLink-mapped (P2P + NVLS multicast) storage; the default is plain
 ``torch.zeros``.
@@ -125,6 +129,7 @@ class FlatArena:
         self.world, self.rank = world, rank
         self.dtype, self.device = dtype, torch.device(device)
         self.grad_dtype = grad_dtype or dtype
+        self.main_grad = self.grad_dtype != self.dtype     # accumulators bound as p.main_grad (module docstring)
         self.params: List[nn.Parameter] = unique_parameters(model)
         self.shapes = [tuple(p.shape) for p in self.params]
         self.numels = [p.numel() for p in self.params]
@@ -168,7 +173,11 @@ class FlatArena:
     def _bind_grads(self, idx: int) -> None:
         for p, v in zip(self.params, self._acc_views[idx]):
             if p.requires_grad:
-                p.grad = v
+                if self.main_grad:
+                    p.main_grad = v
+                    p.grad = None
+                else:
+                    p.grad = v
         self.grad_idx = idx
 
     def point_params(self, idx: int) -> None:
@@ -182,7 +191,7 @@ class FlatArena:
             self._bind_grads(idx)
 
     def rebind(self) -> None:
-        """Re-assert aliasing (e.g. after something replaced ``p.grad`` with ``None``)."""
+        """Re-assert aliasing (e.g. after something replaced ``p.grad`` with ``None``, or set one beside ``p.main_grad``)."""
         self._bind_params(self.live)
         self._bind_grads(self.grad_idx)
 

@@ -68,6 +68,7 @@ TRAIN_DEFAULTS: Dict[str, Any] = dict(
     max_grad_norm=None,             # global gradient-norm clipping of every round (.inf: log the norm only); logged as grad_norm
     fp8=False,                      # FP8 GEMMs (e4m3 / e5m2, per-tensor current scaling) for the block linears of native models (ops/fp8.py)
     no_decay_1d=False,              # True: trainable parameters with ndim <= 1 (norm gains, biases) are updated without weight decay
+    grad_accum_dtype=None,          # "fp32": fp32 gradient accumulators under bf16 weights (bound as p.main_grad); None: the weights' dtype
 )
 
 
@@ -156,6 +157,7 @@ class DecoupledTrainer:
         self.max_grad_norm = check_max_grad_norm(self.args.max_grad_norm)
         self._grad_norm: Optional[float] = None     # pre-clip norm of the last committed round (max_grad_norm set)
         self._check_fp8()
+        self._check_grad_accum_dtype()
         self._fused_smoothing = self._check_label_smoothing()
         if not isinstance(self.args.no_decay_1d, bool):
             raise ValueError(f"no_decay_1d must be true or false, got {self.args.no_decay_1d!r}")
@@ -232,9 +234,10 @@ class DecoupledTrainer:
         self.backend: CommBackend = make_backend(want, self.rank, self.world_size, self.device, n_nodes=self.n_nodes)
         if self.rank == 0:
             self.log.info(f">>> communication backend: {self.backend.name} (requested {str(self.args.comm_backend)!r})")
+        fp32_acc = self.args.grad_accum_dtype == "fp32" and self.param_dtype == torch.bfloat16
         self.arena = FlatArena(self.model, self.world_size, self.rank, self.param_dtype, self.device,
                                align=self.backend.slice_alignment(), allocator=self.backend.allocator(),
-                               double_buffer=not torch_ddp)
+                               double_buffer=not torch_ddp, grad_dtype=torch.float32 if fp32_acc else None)
         self.len_params = self.arena.numel
         self.size_slice = self.arena.layout.size_slice
         self.size_local_slice = self.arena.layout.size_local_slice(self.rank)
@@ -317,6 +320,22 @@ class DecoupledTrainer:
         if a.fused_ag_gemm:
             raise ValueError("fp8=True cannot be combined with fused_ag_gemm: the gathering GEMM has no FP8 instantiation")
         self.model.fp8 = True
+
+    def _check_grad_accum_dtype(self) -> None:
+        """``grad_accum_dtype``: None keeps the accumulators in the weights' dtype; "fp32" sums every micro-batch's gradient into fp32
+        accumulators (no rounding to bf16 per micro-batch), which only the native models' ops can add into (``p.main_grad``)."""
+        a = self.args
+        v = a.grad_accum_dtype
+        if v is None:
+            return
+        if v != "fp32":
+            raise ValueError(f"grad_accum_dtype must be null or 'fp32', got {v!r}")
+        from .models import NativeCausalLM
+        if not isinstance(self.model, NativeCausalLM):
+            raise ValueError(f"grad_accum_dtype=fp32 needs a native model (LlamaForCausalLM / GPTForCausalLM); {type(self.model).__name__}'s "
+                             "backward writes autograd's .grad, which must have the bf16 weights' dtype")
+        if self.method == "ddp" and str(a.ddp_impl) == "torch":
+            raise ValueError("grad_accum_dtype=fp32 cannot be combined with ddp_impl=torch: its gradient buckets take the parameters' dtype")
 
     def _check_label_smoothing(self) -> float:
         """``label_smoothing_factor`` on a native model is applied by its fused cross-entropy kernel (``model.label_smoothing``):

@@ -38,6 +38,11 @@ KERNELS = {
     "fp8_amax.sass": "_ZN8acco_fp815fp8_amax_kernelEPK5uint4xPj",
     "fp8_cast_e4m3.sass": "_ZN8acco_fp815fp8_cast_kernelILi0EEEvPK13__nv_bfloat16PKjiPhS6_Pfii",
     "embedding_bwd.sass": "_ZN4acco20embedding_bwd_kernelEP13__nv_bfloat16PKxS3_PKS0_ii",        # one write per row: no REDG
+    # grad_accum_dtype=fp32: wgrad / FP8 wgrad / embedding backward adding into fp32 gradient accumulators
+    "gemm_wgmma_bn128_tt_f32acc.sass": "_ZN9acco_gemm18gemm_f32acc_kernelILi128EEEvNS_6ParamsE",
+    "gemm_wgmma_bn256_tt_f32acc.sass": "_ZN9acco_gemm18gemm_f32acc_kernelILi256EEEvNS_6ParamsE",
+    "gemm_fp8_bn128_e5m2_f32acc.sass": "_ZN9acco_gemm22gemm_fp8_f32acc_kernelILi128ELi2EEEvNS_6ParamsE",
+    "embedding_bwd_f32.sass": "_ZN4acco20embedding_bwd_kernelEPfPKxS2_PK13__nv_bfloat16ii",
 }
 MNEMONICS = ["HGMMA", "UTMALDG", "UTMALDG.2D.MULTICAST", "UTMASTG", "UTMACMDFLUSH", "SYNCS", "USETMAXREG", "REDG", "LDGMC", "HMMA", "MUFU.SQRT",
              "MUFU.EX2", "CCTL"]

@@ -6,7 +6,7 @@
 Persistent buffers are exact (they follow the arena / optimizer layout: two bf16 parameter sets, two bf16 gradient accumulators and
 the fp32 optimizer shard); activations are an estimate of what the native Llama keeps for backward (bf16 tensors saved by the
 fused ops + the padded logits).  ``--fp8`` (train key ``fp8``): the block linears keep their GEMM inputs as FP8 copies, 1 byte per
-element instead of 2.  Budget: an 80 GB H100, of which 92 % is planned."""
+element instead of 2.  ``--grad-accum-dtype fp32`` (train key ``grad_accum_dtype``): the two gradient accumulators are fp32.  Budget: an 80 GB H100, of which 92 % is planned."""
 import argparse
 import json
 import os
@@ -21,7 +21,8 @@ from acco_b200.parallel.arena import ShardLayout
 GB = 1e9
 
 
-def plan(cfg: LlamaConfig, world: int, batch: int, seq: int, method: str = "acco", align: int = 1024, fp8: bool = False) -> dict:
+def plan(cfg: LlamaConfig, world: int, batch: int, seq: int, method: str = "acco", align: int = 1024, fp8: bool = False,
+         grad_accum_dtype=None) -> dict:
     n = cfg.num_parameters(padded=True)
     lay = ShardLayout(n, world, align)
     two = 2                                                    # bf16
@@ -32,6 +33,8 @@ def plan(cfg: LlamaConfig, world: int, batch: int, seq: int, method: str = "acco
     }
     if method == "ddp":
         buffers["gradient accumulators x2 (bf16)"] = lay.padded * two       # one accumulator is enough without overlap
+    if grad_accum_dtype == "fp32":
+        buffers["gradient accumulators x2 (fp32)"] = buffers.pop("gradient accumulators x2 (bf16)") * 2
     T = batch * seq
     H, I, L = cfg.hidden_size, cfg.intermediate_size, cfg.num_hidden_layers
     D, Hq, Hk = cfg.head_dim, cfg.num_attention_heads, cfg.num_key_value_heads
@@ -60,10 +63,15 @@ def main(argv=None):
     ap.add_argument("--seq", type=int, default=512)
     ap.add_argument("--method", default="acco", choices=["acco", "dpu", "ddp"])
     ap.add_argument("--fp8", action="store_true", help="train.fp8: FP8 copies of the block GEMM inputs are kept for backward")
+    ap.add_argument("--grad-accum-dtype", dest="grad_accum_dtype", default=None, choices=["fp32"],
+                    help="train.grad_accum_dtype: fp32 gradient accumulators")
     a = ap.parse_args(argv)
     cfg = LlamaConfig.from_dict(PRESETS[a.model][1])
-    out = plan(cfg, a.gpus, a.batch, a.seq, a.method, fp8=a.fp8)
-    print(json.dumps({"model": a.model, "gpus": a.gpus, "batch": a.batch, "seq": a.seq, "fp8": a.fp8, **out}, indent=1))
+    out = plan(cfg, a.gpus, a.batch, a.seq, a.method, fp8=a.fp8, grad_accum_dtype=a.grad_accum_dtype)
+    head = {"model": a.model, "gpus": a.gpus, "batch": a.batch, "seq": a.seq, "fp8": a.fp8}
+    if a.grad_accum_dtype:
+        head["grad_accum_dtype"] = a.grad_accum_dtype
+    print(json.dumps({**head, **out}, indent=1))
     return out
 
 
