@@ -19,6 +19,7 @@ import torch
 from . import count_launch, load_ext, use_kernels
 
 TILE_N, TILE_K = 256, 64
+MAX_PEERS = 8                  # peer tensor maps in the kernel's parameter block
 
 
 def gemm_tn_ref(x: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
@@ -102,10 +103,21 @@ class GatheredWeight:
     ``size_slice``   : elements per rank in the flat buffer
     A 256-row tile is gathered from rank ``r`` iff all of it lies inside rank ``r``'s slice and ``r`` is not
     this rank; tiles that straddle an ownership boundary (at most one per boundary) are pushed by the round
-    kernel as usual (``tile_owner == -1``)."""
+    kernel as usual (``tile_owner == -1``).
+
+    Raises ``ValueError`` for a table the kernel cannot serve: an offset, K or N that is not a multiple of 8 (the peer tensor maps
+    need 16-byte aligned rows), more than 8 peers, or a matrix that reaches past the last peer's slice (its owner index would have no
+    peer map, and the kernel would "gather" the stale local copy instead)."""
 
     def __init__(self, n: int, k: int, offset: int, peer_bases: List[int], size_slice: int, rank: int, device):
         self.n, self.k, self.offset, self.rank = int(n), int(k), int(offset), int(rank)
+        if self.offset % 8 or self.k % 8 or self.n % 8:
+            raise ValueError(f"GatheredWeight: offset ({self.offset}), K ({self.k}) and N ({self.n}) must be multiples of 8")
+        if len(peer_bases) > MAX_PEERS:
+            raise ValueError(f"GatheredWeight: at most {MAX_PEERS} peers, got {len(peer_bases)}")
+        if self.offset + self.n * self.k > int(size_slice) * len(peer_bases):
+            raise ValueError(f"GatheredWeight: elements [{self.offset}, {self.offset + self.n * self.k}) reach past the {len(peer_bases)} "
+                             f"peer slices of {size_slice} elements")
         self.peer_ptrs = [int(b) + 2 * self.offset for b in peer_bases]
         num_n = (self.n + TILE_N - 1) // TILE_N
         num_k = (self.k + TILE_K - 1) // TILE_K
@@ -130,6 +142,26 @@ class GatheredWeight:
             if lo // size_slice == (hi - 1) // size_slice == for_rank:
                 out.append((lo, hi))
         return out
+
+
+def fused_ag_tables(model, arena, bases_per_theta: List[List[int]], size_slice: int, rank: int, device):
+    """Ownership tables of the fused all-gather GEMM for every ``model.fused_ag_candidates()`` weight of ``arena``:
+    ``({id(param): [GatheredWeight on theta[i] for each i]}, pulled)``.  ``bases_per_theta[i]`` holds the base address of
+    ``arena.theta[i]`` on every rank; ``pulled`` is the union, over all ranks, of the flat-buffer ranges no rank pushes because
+    every peer pulls them inside its GEMM.  Weights whose offset, K or N is not a multiple of 8 stay on the push path."""
+    by_id = {id(p): o for p, o in zip(arena.params, arena.offsets)}
+    world = len(bases_per_theta[0])
+    table, pulled = {}, []
+    for p in model.fused_ag_candidates():
+        off = by_id[id(p)]
+        N, K = p.shape
+        if off % 8 or K % 8 or N % 8:
+            continue
+        gws = [GatheredWeight(N, K, off, bases, size_slice, rank, device) for bases in bases_per_theta]
+        table[id(p)] = gws
+        for r in range(world):
+            pulled += gws[0].pulled_ranges(r, size_slice)
+    return table, pulled
 
 
 def gemm_tn_gather(x: torch.Tensor, w_local: torch.Tensor, gw: GatheredWeight, max_ctas: int = 0) -> torch.Tensor:

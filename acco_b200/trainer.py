@@ -480,20 +480,9 @@ class DecoupledTrainer:
         if not (bool(self.args.fused_ag_gemm) and isinstance(self.backend, SymmBackend) and self.world_size > 1
                 and self.param_dtype == torch.bfloat16 and hasattr(self.model, "fused_ag_candidates")):
             return
-        from .ops.gemm import GatheredWeight
-        S = self.size_slice
-        by_id = {id(p): (o, n) for p, o, n in zip(self.arena.params, self.arena.offsets, self.arena.numels)}
+        from .ops.gemm import fused_ag_tables
         bases = [self.backend.peer_bases("theta", i) for i in range(len(self.arena.theta))]
-        table, ranges = {}, []
-        for p in self.model.fused_ag_candidates():
-            off, _ = by_id[id(p)]
-            N, K = p.shape
-            if off % 8 or K % 8 or N % 8:
-                continue
-            gws = [GatheredWeight(N, K, off, bases[i], S, self.rank, self.device) for i in range(len(bases))]
-            table[id(p)] = gws
-            for r in range(self.world_size):
-                ranges += gws[0].pulled_ranges(r, S)
+        table, ranges = fused_ag_tables(self.model, self.arena, bases, self.size_slice, self.rank, self.device)
         self.backend.set_pull_ranges(ranges)
         self.model._ag_table = table
         self._ag_on = bool(table)
