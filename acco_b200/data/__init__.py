@@ -1,4 +1,4 @@
-from .collate import PackedCollator, PadCollator, stack_collate
+from .collate import DocumentCollator, PackedCollator, PadCollator, stack_collate
 from .dataset import TokenDataset, load_from_disk
 from .loader import BatchLoader, DeviceFeeder
 from .packing import (make_const_len_tokenize_fn, make_packed_tokenize_fn, make_truncate_tokenize_fn, pack_const_len, pack_sft,
@@ -8,7 +8,7 @@ from .synthetic import (synthetic_documents, synthetic_pretrain_dataset, synthet
 from .tokenizer import ByteTokenizer
 
 __all__ = [
-    "PackedCollator", "PadCollator", "stack_collate", "TokenDataset", "load_from_disk", "BatchLoader", "DeviceFeeder",
+    "DocumentCollator", "PackedCollator", "PadCollator", "stack_collate", "TokenDataset", "load_from_disk", "BatchLoader", "DeviceFeeder",
     "make_const_len_tokenize_fn", "make_truncate_tokenize_fn", "make_packed_tokenize_fn", "pack_const_len", "pack_sft",
     "truncate_docs",
     "synthetic_documents", "synthetic_pretrain_dataset", "synthetic_sft_dataset", "synthetic_text_dataset",

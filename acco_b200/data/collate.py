@@ -9,6 +9,8 @@
   reproduced with ``mask_all_pad_tokens=True`` (default) and can be switched off.
 * :class:`PackedCollator` - packed SFT rows (``pack_sft``): fixed ``[B, max_length]`` batches with per-sample ``position_ids``
   (the models derive document masking from them) and labels that train exactly the (context, target) pairs of ``PadCollator``.
+* :class:`DocumentCollator` - const-len pre-training rows with document masking (``document_mask: True``): the same three
+  ``[B, S]`` tensors as ``PackedCollator``, with the documents found from the EOS tokens ``pack_const_len`` closed them with.
 """
 from __future__ import annotations
 
@@ -17,7 +19,7 @@ from typing import Any, Dict, Sequence
 import numpy as np
 import torch
 
-__all__ = ["stack_collate", "PadCollator", "PackedCollator"]
+__all__ = ["stack_collate", "PadCollator", "PackedCollator", "DocumentCollator"]
 
 
 def stack_collate(batch: Sequence[Dict[str, Any]]) -> Dict[str, torch.Tensor]:
@@ -88,3 +90,32 @@ class PackedCollator:
             if self.mask_all:
                 labels[b, :used][toks == self.pad] = self.label_pad
         return {"input_ids": torch.from_numpy(ids), "labels": torch.from_numpy(labels), "position_ids": torch.from_numpy(pos)}
+
+
+class DocumentCollator:
+    """Const-len rows (``pack_const_len``: documents each closed by ``eos_token_id``, cut into rows) -> ``input_ids``, ``labels``,
+    ``position_ids``, each ``[B, S]`` int64, following the ``PackedCollator`` rules so the models mask attention by document:
+
+    * a segment starts at column 0 and right after every EOS (the EOS closes its own document; consecutive EOS tokens make
+      one-token segments; an EOS in the last column opens no segment).  The first segment usually begins mid-document;
+    * ``position_ids[s] = s - start(s)``;
+    * ``labels = input_ids`` except ``labels[start] = -100`` at every segment start after column 0 (the models shift labels, so
+      this drops the one prediction whose context is the previous document).  EOS stays a target and nothing is masked by pad
+      id: const-len rows hold no padding, and with ``pad == eos`` that rule would erase every EOS target.
+
+    Segment starts are a running maximum along the row, so they never decrease within a row: the precondition of the segmented
+    attention kernels (``csrc/attention_wgmma.cu``).  Vectorised numpy, no per-token Python loop (it runs in the loader workers)."""
+
+    def __init__(self, eos_token_id: int, label_pad: int = -100):
+        self.eos, self.label_pad = int(eos_token_id), int(label_pad)
+
+    def __call__(self, batch: Sequence[Dict[str, Any]]) -> Dict[str, torch.Tensor]:
+        ids = np.stack([np.asarray(b["input_ids"], dtype=np.int64).reshape(-1) for b in batch])
+        S = ids.shape[1]
+        s = np.arange(S, dtype=np.int64)
+        opens = np.zeros_like(ids)
+        opens[:, 1:] = np.where(ids[:, :-1] == self.eos, s[1:], 0)       # column s opens a segment when column s-1 is an EOS
+        start = np.maximum.accumulate(opens, axis=1)
+        labels = ids.copy()
+        labels[(start == s) & (s > 0)] = self.label_pad
+        return {"input_ids": torch.from_numpy(ids), "labels": torch.from_numpy(labels), "position_ids": torch.from_numpy(s - start)}

@@ -25,6 +25,7 @@ from __future__ import annotations
 import contextlib
 import logging
 import math
+import numbers
 import os
 import threading
 import time
@@ -35,8 +36,8 @@ import torch.distributed as dist
 import torch.nn as nn
 
 from .config import to_container
-from .data import (BatchLoader, DeviceFeeder, PackedCollator, PadCollator, make_const_len_tokenize_fn, make_packed_tokenize_fn,
-                   make_truncate_tokenize_fn, pack_sft, stack_collate)
+from .data import (BatchLoader, DeviceFeeder, DocumentCollator, PackedCollator, PadCollator, make_const_len_tokenize_fn,
+                   make_packed_tokenize_fn, make_truncate_tokenize_fn, pack_sft, stack_collate)
 from .launch import DistEnv, discover_env, init_distributed
 from .obs import OverlapMeter, ScalarWriter, TrainingPrinter, create_dict_result, log_training_scalars, nvtx_range, save_result
 from .optim import ShardedAdamW, check_max_grad_norm
@@ -69,6 +70,7 @@ TRAIN_DEFAULTS: Dict[str, Any] = dict(
     fp8=False,                      # FP8 GEMMs (e4m3 / e5m2, per-tensor current scaling) for the block linears of native models (ops/fp8.py)
     no_decay_1d=False,              # True: trainable parameters with ndim <= 1 (norm gains, biases) are updated without weight decay
     grad_accum_dtype=None,          # "fp32": fp32 gradient accumulators under bf16 weights (bound as p.main_grad); None: the weights' dtype
+    document_mask=False,            # const-len rows: no attention across the documents of a row, positions restart per document
 )
 
 
@@ -307,6 +309,26 @@ class DecoupledTrainer:
             raise ValueError(f"packing=True needs a native model that masks attention by position_ids; {type(self.model).__name__} "
                              "would attend across the samples of a row")
 
+    def _check_document_mask(self) -> None:
+        """``document_mask`` needs const-len rows, a model that masks attention by ``position_ids`` and the EOS id the rows were
+        packed with (``DocumentCollator`` finds the documents from it)."""
+        a = self.args
+        if not isinstance(a.document_mask, bool):
+            raise ValueError(f"document_mask must be true or false, got {a.document_mask!r}")
+        if not a.document_mask:
+            return
+        if not a.const_len_batch:
+            raise ValueError("document_mask=True needs const_len_batch=True: padded SFT rows hold one sample each, and packed SFT rows "
+                             "(packing=True) are already document-masked")
+        from .models import NativeCausalLM
+        if not isinstance(self.model, NativeCausalLM):
+            raise ValueError(f"document_mask=True needs a native model that masks attention by position_ids; {type(self.model).__name__} "
+                             "would attend across the documents of a row")
+        eos = getattr(self.tokenizer, "eos_token_id", None)
+        if isinstance(eos, bool) or not isinstance(eos, numbers.Integral):
+            raise ValueError(f"document_mask=True needs a tokenizer with an integer eos_token_id (the token the rows were packed with), "
+                             f"got {eos!r}")
+
     def _check_fp8(self) -> None:
         """``fp8``: the native models' block linears run their training GEMMs in FP8 on bf16 weights and gradients."""
         a = self.args
@@ -354,6 +376,7 @@ class DecoupledTrainer:
     def prepare_data(self) -> None:
         """Per-rank sharding (`trainer_base.py:183-200`)."""
         self._check_packing()
+        self._check_document_mask()
         if self.train_dataset is not None and isinstance(self.train_dataset, torch.utils.data.IterableDataset) \
                 and self.args.group_by_length:
             raise ValueError("the `--group_by_length` option is only available for `Dataset`, not `IterableDataset")
@@ -400,7 +423,7 @@ class DecoupledTrainer:
 
     def _collator(self):
         if self.args.const_len_batch:
-            return stack_collate
+            return DocumentCollator(self.tokenizer.eos_token_id) if self.args.document_mask else stack_collate
         pad = getattr(self.tokenizer, "pad_token_id", None) if self.tokenizer is not None else None
         if pad is None:
             pad = getattr(self.tokenizer, "eos_token_id", 0) if self.tokenizer is not None else 0

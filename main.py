@@ -60,6 +60,8 @@ def load_data(cfg, vocab_size: int, tokenizer):
             tokenizer.pad_token_id = tokenizer.eos_token_id
     else:
         full = synthetic_pretrain_dataset(n_docs, mean_len, vocab_size, int(t.max_length), eos_token_id=vocab_size - 1, seed=seed)
+        if tokenizer is None:
+            tokenizer = ByteTokenizer(eos_token_id=vocab_size - 1)       # the EOS the rows were packed with (document_mask)
     split = full.train_test_split(0.05, seed=42)
     return split["train"], split["test"], tokenizer
 
