@@ -23,9 +23,9 @@ int acco_rope_qkv(void* qkv, const float* cos_t, const float* sin_t, int T, int 
 int acco_swiglu_fwd(const void* gu, void* out, long long T, int I, int sms, cudaStream_t st);
 int acco_swiglu_bwd(const void* dout, const void* gu, void* dgu, long long T, int I, int sms, cudaStream_t st);
 int acco_ce_fwd(const void* logits, const long long* labels, float* lse, float* row_loss, float* loss, float* inv_n, long long T,
-                int V, int Vp, long long ignore_index, float label_smoothing, cudaStream_t st);
+                int V, int Vp, long long ignore_index, float label_smoothing, float z_loss, float* z_out, cudaStream_t st);
 int acco_ce_bwd(void* logits, const long long* labels, const float* lse, const float* scale, long long T, int V, int Vp,
-                long long ignore_index, float label_smoothing, cudaStream_t st);
+                long long ignore_index, float label_smoothing, float z_loss, cudaStream_t st);
 int acco_norm_bwd_acc_f32(const void* dy, const void* dh_extra, const void* h, const void* w, const float* mean, const float* rstd, void* dh,
                           float* partial, float* dw_accum, float* db_accum, int T, int H, int grid, cudaStream_t st);
 int acco_embedding_bwd(void* grad, const long long* sorted, const long long* perm, const void* dy, int T, int H, int sms, cudaStream_t st);
@@ -293,10 +293,25 @@ void check_label_smoothing(double eps) {
     TORCH_CHECK(std::isfinite(eps) && eps >= 0.0 && eps <= 1.0, "label_smoothing must be finite and in [0, 1], got ", eps);
 }
 
-std::vector<torch::Tensor> ce_fwd(torch::Tensor logits, torch::Tensor labels, int64_t V, int64_t ignore_index, double label_smoothing) {
+void check_z_loss(double z) {
+    TORCH_CHECK(std::isfinite(z) && z >= 0.0 && std::isfinite((float)z), "z_loss must be finite and >= 0, got ", z);
+}
+
+// `z_out`: with z_loss > 0, a one-element fp32 tensor on the logits' device that receives the mean z-term (z lse^2 over the
+// non-ignored rows); the return value stays (loss, inv_n, lse), with loss = mean CE + that term.
+std::vector<torch::Tensor> ce_fwd(torch::Tensor logits, torch::Tensor labels, int64_t V, int64_t ignore_index, double label_smoothing,
+                                  double z_loss, c10::optional<torch::Tensor> z_out) {
     check_bf16(logits, "logits");
     check_label_smoothing(label_smoothing);
+    check_z_loss(z_loss);
     TORCH_CHECK(labels.is_cuda() && labels.scalar_type() == torch::kInt64 && labels.is_contiguous(), "labels must be contiguous CUDA int64");
+    float* z_ptr = nullptr;
+    if (z_loss != 0.0) {
+        TORCH_CHECK(z_out.has_value(), "ce_fwd: z_loss > 0 needs z_out");
+        TORCH_CHECK(z_out->is_cuda() && z_out->device() == logits.device() && z_out->scalar_type() == torch::kFloat32 && z_out->numel() == 1,
+                    "z_out must be a one-element fp32 tensor on the logits' device");
+        z_ptr = z_out->data_ptr<float>();
+    }
     const c10::cuda::CUDAGuard guard(logits.device());
     const int64_t T = logits.size(0), Vp = logits.size(1);
     TORCH_CHECK(labels.numel() == T, "labels/logits row mismatch");
@@ -307,19 +322,20 @@ std::vector<torch::Tensor> ce_fwd(torch::Tensor logits, torch::Tensor labels, in
     auto inv_n = torch::empty({1}, f32);
     TORCH_CHECK(acco_ce_fwd(logits.data_ptr(), (const long long*)labels.data_ptr<int64_t>(), lse.data_ptr<float>(), row_loss.data_ptr<float>(),
                             loss.data_ptr<float>(), inv_n.data_ptr<float>(), T, (int)V, (int)Vp, ignore_index, (float)label_smoothing,
-                            stream()) == 0,
+                            (float)z_loss, z_ptr, stream()) == 0,
                 "ce_fwd: padded vocab must be a multiple of 8 and >= V");
     return {loss, inv_n, lse};
 }
 
 void ce_bwd_inplace(torch::Tensor logits, torch::Tensor labels, torch::Tensor lse, torch::Tensor scale, int64_t V, int64_t ignore_index,
-                    double label_smoothing) {
+                    double label_smoothing, double z_loss) {
     check_bf16(logits, "logits"); check_f32(lse, "lse"); check_f32(scale, "scale");
     check_label_smoothing(label_smoothing);
+    check_z_loss(z_loss);
     const c10::cuda::CUDAGuard guard(logits.device());
     const int64_t T = logits.size(0), Vp = logits.size(1);
     TORCH_CHECK(acco_ce_bwd(logits.data_ptr(), (const long long*)labels.data_ptr<int64_t>(), lse.data_ptr<float>(), scale.data_ptr<float>(), T,
-                            (int)V, (int)Vp, ignore_index, (float)label_smoothing, stream()) == 0, "ce_bwd: bad shapes");
+                            (int)V, (int)Vp, ignore_index, (float)label_smoothing, (float)z_loss, stream()) == 0, "ce_bwd: bad shapes");
 }
 
 // ---------------------------------------------------------------- fused round kernel
@@ -774,9 +790,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("swiglu_bwd", &swiglu_bwd);
     m.def("embedding_bwd", &embedding_bwd);
     m.def("embedding_bwd_f32", &embedding_bwd_f32);
-    m.def("ce_fwd", &ce_fwd, py::arg("logits"), py::arg("labels"), py::arg("V"), py::arg("ignore_index"), py::arg("label_smoothing") = 0.0);
+    m.def("ce_fwd", &ce_fwd, py::arg("logits"), py::arg("labels"), py::arg("V"), py::arg("ignore_index"), py::arg("label_smoothing") = 0.0,
+          py::arg("z_loss") = 0.0, py::arg("z_out") = py::none());
     m.def("ce_bwd_inplace", &ce_bwd_inplace, py::arg("logits"), py::arg("labels"), py::arg("lse"), py::arg("scale"), py::arg("V"),
-          py::arg("ignore_index"), py::arg("label_smoothing") = 0.0);
+          py::arg("ignore_index"), py::arg("label_smoothing") = 0.0, py::arg("z_loss") = 0.0);
     m.def("adamw_shard", &adamw_shard, py::arg("grad_sum"), py::arg("master"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("stash"),
           py::arg("out"), py::arg("inv_count"), py::arg("scratch"), py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"), py::arg("wd"),
           py::arg("step"), py::arg("commit"), py::arg("add_stash"), py::arg("write_stash"), py::arg("no_decay_ranges") = py::none(),

@@ -52,6 +52,8 @@ class NativeCausalLM(nn.Module):
         self.config = config
         self.fp8 = False             # FP8 GEMMs for the block linears of training micro-batches (train key `fp8`, ops/fp8.py)
         self.label_smoothing = 0.0   # label smoothing of the loss when labels are given (train key `label_smoothing_factor`)
+        self.z_loss_weight = 0.0     # z * mean lse^2 added to the loss (train key `z_loss_weight`, ops/cross_entropy.py)
+        self.z_loss_out: Optional[torch.Tensor] = None   # one fp32 on the device: receives the z-term of each loss computed
 
     @property
     def embed_weight(self) -> torch.Tensor:
@@ -90,7 +92,8 @@ class NativeCausalLM(nn.Module):
         # HF shift: position t predicts token t+1; the last position has no target
         shifted = torch.full_like(labels, -100)
         shifted[:, :-1] = labels[:, 1:]
-        loss = ops.softmax_cross_entropy(logits, shifted.reshape(B * S), V, -100, label_smoothing=self.label_smoothing)
+        loss = ops.softmax_cross_entropy(logits, shifted.reshape(B * S), V, -100, label_smoothing=self.label_smoothing,
+                                         z_loss=self.z_loss_weight, z_loss_out=self.z_loss_out)
         return CausalLMOutput(loss=loss, logits=None)
 
     # ------------------------------------------------------------------ HF-compatible checkpoints

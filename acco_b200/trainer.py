@@ -71,6 +71,7 @@ TRAIN_DEFAULTS: Dict[str, Any] = dict(
     no_decay_1d=False,              # True: trainable parameters with ndim <= 1 (norm gains, biases) are updated without weight decay
     grad_accum_dtype=None,          # "fp32": fp32 gradient accumulators under bf16 weights (bound as p.main_grad); None: the weights' dtype
     document_mask=False,            # const-len rows: no attention across the documents of a row, positions restart per document
+    z_loss_weight=0,                # native models: add z * mean lse^2 (PaLM z-loss) to every training micro-batch's loss; logged as z_loss
 )
 
 
@@ -161,6 +162,7 @@ class DecoupledTrainer:
         self._check_fp8()
         self._check_grad_accum_dtype()
         self._fused_smoothing = self._check_label_smoothing()
+        self.z_loss_weight = self._check_z_loss()
         if not isinstance(self.args.no_decay_1d, bool):
             raise ValueError(f"no_decay_1d must be true or false, got {self.args.no_decay_1d!r}")
         self.no_decay_1d = self.args.no_decay_1d
@@ -169,6 +171,9 @@ class DecoupledTrainer:
         if self._fused_smoothing and self.rank == 0:
             self.log.info(f">>> label_smoothing_factor={self._fused_smoothing}: smoothed inside the fused cross-entropy kernel "
                           f"of {type(self.model).__name__} (CUDA graphs stay available)")
+        if self.z_loss_weight and self.rank == 0:
+            self.log.info(f">>> z_loss_weight={self.z_loss_weight}: z-loss inside the fused cross-entropy kernel of "
+                          f"{type(self.model).__name__} on every training micro-batch (eval stays pure cross-entropy)")
         self._init_writer()
         self.prepare_data()
         self._tokenize_if_needed()
@@ -179,6 +184,14 @@ class DecoupledTrainer:
         self.loss_host = torch.zeros(1, dtype=torch.float32)
         if self.is_cuda:
             self.loss_host = self.loss_host.pin_memory()
+        # z_loss_weight > 0: the cross-entropy writes each micro-batch's mean z-term here on the device (also under graph replay);
+        # it is copied to the host with the loss
+        self.z_loss_static = torch.zeros(1, device=self.device, dtype=torch.float32)
+        self.z_loss_host = torch.zeros(1, dtype=torch.float32)
+        if self.is_cuda:
+            self.z_loss_host = self.z_loss_host.pin_memory()
+        if self.z_loss_weight:
+            self.model.z_loss_out = self.z_loss_static
         self.n_grad_acc_ddp = 1
         self._hook_extra_microbatches: Optional[Callable[[int, int], int]] = None   # tests: (rank, round) -> extra
         self._nvtx = os.environ.get("ACCO_NVTX") == "1"
@@ -372,6 +385,21 @@ class DecoupledTrainer:
         self.model.label_smoothing = float(eps)
         self.label_smoother = None
         return float(eps)
+
+    def _check_z_loss(self) -> float:
+        """``z_loss_weight``: the native models add ``z * lse^2`` per non-ignored row inside their fused cross-entropy
+        (``model.z_loss_weight``); there is no route for other models.  Returns the weight (0 if off)."""
+        z = self.args.z_loss_weight
+        if isinstance(z, bool) or not isinstance(z, (int, float)) or not math.isfinite(z) or z < 0:
+            raise ValueError(f"z_loss_weight must be a finite number >= 0, got {z!r}")
+        if not z:
+            return 0.0
+        from .models import NativeCausalLM
+        if not isinstance(self.model, NativeCausalLM):
+            raise ValueError(f"z_loss_weight > 0 needs a native model (LlamaForCausalLM / GPTForCausalLM): the term is computed inside "
+                             f"their fused cross-entropy kernel, and {type(self.model).__name__} has no such loss")
+        self.model.z_loss_weight = float(z)
+        return float(z)
 
     def prepare_data(self) -> None:
         """Per-rank sharding (`trainer_base.py:183-200`)."""
@@ -768,10 +796,14 @@ class DecoupledTrainer:
                 self.gradient_step()
         if self.is_cuda:
             self.loss_host.copy_(self.loss_static, non_blocking=True)
+            if self.z_loss_weight:
+                self.z_loss_host.copy_(self.z_loss_static, non_blocking=True)
             self.end_of_grad.record(self.grad_stream)
             self._poll_phase_end()
         else:
             self.loss_host.copy_(self.loss_static)
+            if self.z_loss_weight:
+                self.z_loss_host.copy_(self.z_loss_static)
 
     def _poll_phase_end(self) -> None:
         """The flip decision must be taken when the *device* reaches the end of the phase ("if the com finished ... else accumulate
@@ -929,6 +961,8 @@ class DecoupledTrainer:
             sched.lr_steps += 1
             sched.count_grad_tot += self.world_size * int(a.n_grad_accumulation)
             self.loss_host.copy_(self.loss_static)
+            if self.z_loss_weight:
+                self.z_loss_host.copy_(self.z_loss_static)
             self._tail(None)
         return self._finish("_ddp")
 
@@ -986,6 +1020,8 @@ class DecoupledTrainer:
                 loss = float(self.loss_host.item())
                 nb_step = sched.count_com // 2 if self.method == "acco" else sched.count_com
                 gn = {} if self._grad_norm is None else {"grad_norm": self._grad_norm}
+                if self.z_loss_weight:
+                    gn["z_loss"] = float(self.z_loss_host.item())    # the loss's z-term: cross-entropy = loss - z_loss
                 log_training_scalars(self.writer, nb_step, sched.count_grad_tot, self.rank, loss, eval_loss, self.t_beg,
                                      extra={"lr": getattr(self, "_last_lr", 0.0), **gn})
                 self._fire("on_log", {"step": nb_step, "count_grad_tot": sched.count_grad_tot, "loss": loss,
@@ -997,6 +1033,8 @@ class DecoupledTrainer:
                     st["rate_mark"] = (now, seen)
                     rate = (seen - n0) / max(now - t0, 1e-9)
                     gn_txt = "" if self._grad_norm is None else f" | grad_norm {self._grad_norm:.4g}"
+                    if self.z_loss_weight:
+                        gn_txt += f" | z_loss {gn['z_loss']:.4g}"
                     pr.emit(sched.count_grad_tot, sched.count_com, loss, extra=f" | {rate:,.0f} tok/s/rank | lr {getattr(self, '_last_lr', 0.0):.3e}{gn_txt}")
                 self.epoch = pr.epoch
         if committed and plan is not None and self.callbacks:
@@ -1052,12 +1090,18 @@ class DecoupledTrainer:
         self.model.eval()
         losses: List[torch.Tensor] = []
         ctx = torch.autocast(device_type=self.device.type, dtype=self.dtype) if self.autocast else contextlib.nullcontext()
-        for i, inputs in enumerate(self.eval_dataloader):
-            if self.args.max_eval_batches is not None and i >= int(self.args.max_eval_batches):
-                break
-            inputs = {k: v.to(self.device, non_blocking=True) for k, v in inputs.items()}
-            with ctx:
-                losses.append(self._forward_loss(self.model, inputs).detach().float().reshape(1))
+        if self.z_loss_weight:
+            self.model.z_loss_weight = 0.0          # eval loss stays pure cross-entropy, comparable with runs without the key
+        try:
+            for i, inputs in enumerate(self.eval_dataloader):
+                if self.args.max_eval_batches is not None and i >= int(self.args.max_eval_batches):
+                    break
+                inputs = {k: v.to(self.device, non_blocking=True) for k, v in inputs.items()}
+                with ctx:
+                    losses.append(self._forward_loss(self.model, inputs).detach().float().reshape(1))
+        finally:
+            if self.z_loss_weight:
+                self.model.z_loss_weight = self.z_loss_weight
         self.model.train()
         if not losses:
             return torch.tensor(float("nan"))

@@ -43,6 +43,17 @@ KERNELS = {
     "gemm_wgmma_bn256_tt_f32acc.sass": "_ZN9acco_gemm18gemm_f32acc_kernelILi256EEEvNS_6ParamsE",
     "gemm_fp8_bn128_e5m2_f32acc.sass": "_ZN9acco_gemm22gemm_fp8_f32acc_kernelILi128ELi2EEEvNS_6ParamsE",
     "embedding_bwd_f32.sass": "_ZN4acco20embedding_bwd_kernelEPfPKxS2_PK13__nv_bfloat16ii",
+    # cross-entropy <kSmooth, kZ>: label smoothing and z-loss (train.z_loss_weight) add no pass over the logits (MUFU.EX2 counts)
+    "ce_fwd.sass": "_ZN4acco13ce_fwd_kernelILb0ELb0EEEvPK13__nv_bfloat16PKxPfS6_iixfff",
+    "ce_fwd_smooth.sass": "_ZN4acco13ce_fwd_kernelILb1ELb0EEEvPK13__nv_bfloat16PKxPfS6_iixfff",
+    "ce_fwd_z.sass": "_ZN4acco13ce_fwd_kernelILb0ELb1EEEvPK13__nv_bfloat16PKxPfS6_iixfff",
+    "ce_fwd_smooth_z.sass": "_ZN4acco13ce_fwd_kernelILb1ELb1EEEvPK13__nv_bfloat16PKxPfS6_iixfff",
+    "ce_reduce.sass": "_ZN4acco16ce_reduce_kernelILb0EEEvPKfPKxPfS5_xxS2_S5_f",
+    "ce_reduce_z.sass": "_ZN4acco16ce_reduce_kernelILb1EEEvPKfPKxPfS5_xxS2_S5_f",
+    "ce_bwd.sass": "_ZN4acco13ce_bwd_kernelILb0ELb0EEEvP13__nv_bfloat16PKxPKfS6_iixfff",
+    "ce_bwd_smooth.sass": "_ZN4acco13ce_bwd_kernelILb1ELb0EEEvP13__nv_bfloat16PKxPKfS6_iixfff",
+    "ce_bwd_z.sass": "_ZN4acco13ce_bwd_kernelILb0ELb1EEEvP13__nv_bfloat16PKxPKfS6_iixfff",
+    "ce_bwd_smooth_z.sass": "_ZN4acco13ce_bwd_kernelILb1ELb1EEEvP13__nv_bfloat16PKxPKfS6_iixfff",
 }
 MNEMONICS = ["HGMMA", "UTMALDG", "UTMALDG.2D.MULTICAST", "UTMASTG", "UTMACMDFLUSH", "SYNCS", "USETMAXREG", "REDG", "LDGMC", "HMMA", "MUFU.SQRT",
              "MUFU.EX2", "CCTL"]
