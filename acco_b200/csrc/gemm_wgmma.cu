@@ -30,6 +30,11 @@
 //                                  the mainloop runs and added in fp32 (one rounding).  The warpgroup does not wait for the stores:
 //                                  it goes on to its next tile and only reuses a staging buffer once its store has read it.
 //
+// Ping-pong schedule (gemm_pingpong_kernel, chosen by use_pingpong): the forward and dgrad GEMMs with a plain-store epilogue run on a
+// second kernel with the same producer / ring / epilogue building blocks, in which each consumer warpgroup owns whole 128 x 128 tiles
+// and the two warpgroups take turns on the tensor cores, so one warpgroup's epilogue runs under the other's wgmmas.  The cooperative
+// kernel above keeps every other call: wgrad, split-K, beta = 1, FP8, fp32 D, gather mode, multicast and explicit tile requests.
+//
 // Operand layouts in shared memory (wgmma canonical layouts, 128-byte swizzle):
 //   K-major  : rows of 64 k (128 B), 8-row swizzle atoms 1024 B apart (SBO); one TMA box {64 k, rows}
 //   MN-major : one TMA box {64 mn, 64 k} gives 64 rows (k) of 128 B = 8 KiB per 64-mn chunk;
@@ -548,6 +553,152 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_fp8_f32acc_kernel(const __gri
     gemm_body<BN, 0, 0, OP, true>(P);
 }
 
+// PING-PONG schedule for the bf16 GEMMs whose epilogue is a plain store: the forward (B K-major) and the dgrad (B MN-major), one K
+// split, no gather, no cluster.  A unit is a whole 128 x 128 tile and belongs to ONE consumer warpgroup (two m64n128k16 wgmmas per
+// k16 step, 2 x 64 fp32 accumulators per thread); the warpgroups take alternate units of the CTA's persistent sequence (the tile order
+// of decode_unit).  The producer walks that same sequence into one ring, so the i-th unit of the CTA starts at ring position
+// i * num_k.  An order barrier passes the tensor cores from unit i to unit i + 1: a warpgroup waits for its turn, issues its mainloop,
+// hands the turn over as soon as its last wgmma group is issued, and then runs its epilogue (+bias, bf16, 64 x 64 staging, TMA stores)
+// while the other warpgroup's wgmmas run.  The turn barrier of warpgroup w completes once per unit of the other warpgroup; unit i
+// (i >= 1) waits for completion (i - 1) / 2 of turn[i % 2], i.e. parity ((i - 1) >> 1) & 1.  Every stage has one reader, so the
+// empty barriers count one arrival.  tests/test_gemm_pingpong_protocol.py model-checks this protocol.
+template <int B_MN>
+__global__ void __launch_bounds__(THREADS, 1) gemm_pingpong_kernel(const __grid_constant__ Params P) {
+    constexpr int BN = 128;
+    constexpr int B_BYTES = BN * BK * 2;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+    uint8_t* epi_smem = smem + RING_BYTES;
+    uint64_t* full_bar = (uint64_t*)(epi_smem + EPI_BYTES);
+    uint64_t* empty_bar = full_bar + MAX_STAGES;
+    uint64_t* turn_bar = empty_bar + MAX_STAGES;              // [2]  turn[w]: warpgroup w may issue its next mainloop
+    const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
+    const int n_stages = P.stages, stage_bytes = P.stage_bytes;
+    const int num_n = (P.N + BN - 1) / BN, num_k = (P.K + BK - 1) / BK, num_mb = (P.M + BM - 1) / BM;
+    const int tiles = num_mb * num_n;
+
+    if (threadIdx.x == 0) {
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&P.map_a) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&P.map_b) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&P.map_d) : "memory");
+        for (int s = 0; s < n_stages; ++s) {
+            mbar_init(&full_bar[s], 1);
+            mbar_init(&empty_bar[s], 1);
+        }
+        mbar_init(&turn_bar[0], 1);
+        mbar_init(&turn_bar[1], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+
+    if (wg == 0) {
+        // ============================ TMA PRODUCER: every k-block of every unit of the CTA, in sequence order ============================
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (tid == 0) {
+            int stage = 0;
+            uint32_t phase = 0;
+            for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+                const Unit u = decode_unit(t, tiles, num_mb, num_n, P.band, num_k, num_k, 1, 1, 0, 0);
+                const int m0 = u.mb * BM, n0 = u.n_blk * BN;
+                for (int kb = 0; kb < num_k; ++kb) {
+                    mbar_wait(&empty_bar[stage], phase ^ 1);
+                    uint8_t* sa = smem + stage * stage_bytes;
+                    uint8_t* sb = sa + A_BYTES;
+                    mbar_expect_tx(&full_bar[stage], (uint32_t)(A_BYTES + B_BYTES));
+                    tma_load_2d(&P.map_a, &full_bar[stage], sa, kb * BK, m0);
+                    if (B_MN) {
+                        tma_load_2d(&P.map_b, &full_bar[stage], sb, n0, kb * BK);
+                        tma_load_2d(&P.map_b, &full_bar[stage], sb + MN_CHUNK_BYTES, n0 + 64, kb * BK);
+                    } else {
+                        tma_load_2d(&P.map_b, &full_bar[stage], sb, kb * BK, n0);
+                    }
+                    if (++stage == n_stages) { stage = 0; phase ^= 1; }
+                }
+            }
+        }
+    } else {
+        // ============================ CONSUMERS: warpgroup cw computes units cw, cw + 2, ... of the CTA's sequence ============================
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+        const int cw = wg - 1;
+        const int warp = tid >> 5, lane = tid & 31;
+        constexpr uint32_t b_lbo = B_MN ? (MN_CHUNK_BYTES >> 4) : 1, b_sbo = 1024 >> 4, b_kstep = B_MN ? 2048 : 32;
+        uint8_t* epi = epi_smem + cw * 2 * EPI_BUF_BYTES;
+        const int bar_id = 1 + cw;
+        float acc0[BN / 2], acc1[BN / 2];                  // rows [0, 64) and [64, 128) of the unit
+        for (int i = cw;; i += 2) {                        // i: the unit's index in the CTA's sequence
+            const int t = blockIdx.x + i * gridDim.x;
+            if (t >= tiles) break;
+            const Unit u = decode_unit(t, tiles, num_mb, num_n, P.band, num_k, num_k, 1, 1, 0, 0);
+            const int pos = i * num_k;                     // the unit's first ring position
+            int stage = pos % n_stages;
+            uint32_t phase = (uint32_t)(pos / n_stages) & 1u;
+            if (i > 0) mbar_wait(&turn_bar[cw], (uint32_t)((i - 1) >> 1) & 1u);
+            int prev = -1;
+            for (int kb = 0; kb < num_k; ++kb) {
+                mbar_wait(&full_bar[stage], phase);
+                const uint32_t a_addr = smem_u32(smem + stage * stage_bytes);
+                const uint32_t b_addr = a_addr + A_BYTES;
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k) {
+                    const uint64_t db = make_smem_desc(b_addr + k * b_kstep, b_lbo, b_sbo);
+                    const uint32_t sd = (uint32_t)((kb > 0) | (k != 0));
+                    wgmma_m64n128k16<0, B_MN>(acc0, make_smem_desc(a_addr + k * 32, 1, 1024 >> 4), db, sd);
+                    wgmma_m64n128k16<0, B_MN>(acc1, make_smem_desc(a_addr + 8192 + k * 32, 1, 1024 >> 4), db, sd);
+                }
+                wgmma_commit();
+                if (prev >= 0) {
+                    wgmma_wait<1>();
+                    if (tid == 0) mbar_arrive(&empty_bar[prev]);
+                }
+                prev = stage;
+                if (++stage == n_stages) { stage = 0; phase ^= 1; }
+            }
+            if (tid == 0) mbar_arrive(&turn_bar[cw ^ 1]);  // every wgmma of this unit is issued: the other warpgroup's turn
+            wgmma_wait<0>();
+            reg_fence(acc0);
+            reg_fence(acc1);
+            if (tid == 0) mbar_arrive(&empty_bar[prev]);
+            // ---------------- epilogue: 4 sub-tiles of 64 x 64 (row half h, column half s) through the two staging buffers, as in gemm_body
+            const uint32_t row_addr = smem_u32(epi) + (uint32_t)((warp * 16 + (lane >> 2)) * 128 + 4 * (lane & 3));
+            const int colb = u.n_blk * BN + 2 * (lane & 3);
+            const bool bias_on = P.bias != nullptr;
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const int h = q >> 1, s = q & 1;
+                float(&acc)[BN / 2] = h ? acc1 : acc0;
+                uint8_t* buf = epi + (q & 1) * EPI_BUF_BYTES;
+                const uint32_t buf_addr = row_addr + (uint32_t)((q & 1) * EPI_BUF_BYTES);
+                if (tid == 0) bulk_wait_read<1>();         // the store that last read this buffer (two commits back) is done reading
+                named_barrier(bar_id, 128);
+#pragma unroll
+                for (int jj = 0; jj < 8; ++jj) {
+                    const int j = s * 8 + jj;
+                    const int col = colb + 8 * j;
+                    uint32_t braw = 0;                     // bf16 pair (the register budget is tight with 128 accumulators)
+                    if (bias_on && col < P.N) braw = *reinterpret_cast<const uint32_t*>(P.bias + col);
+                    const float2 bf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&braw));
+                    const float b0 = bf.x, b1 = bf.y;
+                    const uint32_t chunk_addr = buf_addr + (uint32_t)((jj ^ (lane >> 2)) << 4);
+#pragma unroll
+                    for (int r = 0; r < 2; ++r)
+                        st_shared_u32(chunk_addr + r * 8 * 128, pack_bf16x2(acc[4 * j + 2 * r] + b0, acc[4 * j + 2 * r + 1] + b1));
+                }
+                fence_async_smem();
+                named_barrier(bar_id, 128);
+                if (tid == 0) {
+                    tma_store_2d(&P.map_d, buf, u.n_blk * BN + s * 64, u.mb * BM + h * 64);
+                    bulk_commit();
+                }
+            }
+        }
+        if (tid == 0) bulk_wait<0>();
+    }
+    __syncthreads();
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                              const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -667,6 +818,8 @@ static KernelFn fp8_f32acc_kernel_for(int bn, int op) {
     return op == OP_E5M2 ? gemm_fp8_f32acc_kernel<64, OP_E5M2> : gemm_fp8_f32acc_kernel<64, OP_E4M3>;
 }
 
+static KernelFn pingpong_kernel_for(int b_mn) { return b_mn ? gemm_pingpong_kernel<1> : gemm_pingpong_kernel<0>; }
+
 static int g_pm = 0, g_pn = 0;                     // ACCO_GEMM_CLUSTER="pm,pn": force the cluster shape (0 = heuristic)
 static unsigned long long* g_dbg = nullptr;        // device buffer for phase time stamps (acco_gemm_set_debug)
 static int g_pdl = 1;                              // ACCO_GEMM_PDL=0: no programmatic dependent launch
@@ -685,6 +838,8 @@ static int init_once() {
                     rc = -4;
         for (int bn : {64, 128, 256})
             if (cudaFuncSetAttribute(f32acc_kernel_for(bn), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) rc = -4;
+        for (int b_mn = 0; b_mn < 2; ++b_mn)
+            if (cudaFuncSetAttribute(pingpong_kernel_for(b_mn), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) rc = -4;
         const char* e;
         if ((e = getenv("ACCO_GEMM_CLUSTER")) && e[0] && e[1] == ',') { g_pm = e[0] - '0'; g_pn = e[2] - '0'; }
         if ((e = getenv("ACCO_GEMM_PDL")) && e[0] == '0') g_pdl = 0;
@@ -725,9 +880,10 @@ struct Config {
 
 // Tile / split-K / cluster choice: minimise (waves x per-unit cost).  Per k-block a CTA's tensor cores need 4 * bn cycles
 // (128 x bn x 64 multiply-adds at 2048 per clock on an H100 SM) and the operand bytes must come in through L2 (~64 B/clk/SM
-// assumed); `epi` charges the epilogue as if it were not overlapped (its TMA stores now drain while the next tile's mainloop runs,
-// so this over-estimates it; the picks are kept as they are).  Split-K needs an adding epilogue: accumulating GEMMs
-// (wgrad), or a zero-filled output.  FP8 passes K / 2: its 128-deep k-block moves the bytes of a bf16 one and takes the same tensor-core
+// assumed); `epi` charges the epilogue as if it were not overlapped.  On the cooperative kernel only the TMA stores drain under the
+// next tile's mainloop; the ping-pong kernel (use_pingpong) hides most of the epilogue under the other warpgroup's wgmmas, so for
+// the calls it runs this over-estimates the epilogue.  The picks are kept as they are: use_pingpong starts from them.
+// Split-K needs an adding epilogue: accumulating GEMMs (wgrad), or a zero-filled output.  FP8 passes K / 2: its 128-deep k-block moves the bytes of a bf16 one and takes the same tensor-core
 // time (twice the rate), and caps the tile at bn_max = 128.
 static Config choose_config(int M, int N, int K, int a_mn, int b_mn, int reduce, int sms, int bn_req, int splits_req, int pm_req, int pn_req,
                             int bn_max = BN_MAX) {
@@ -779,6 +935,20 @@ static Config choose_config(int M, int N, int K, int a_mn, int b_mn, int reduce,
         }
     }
     return bc;
+}
+
+// Schedule of a call: the ping-pong kernel (gemm_pingpong_kernel) for the non-accumulating bf16 GEMMs with a K-major A - the forward
+// and the dgrad - when the call requests nothing (tile width, K splits, multicast) and the cost model picks one K split and either
+// 128-wide tiles, or 256-wide tiles with K <= 1024; everything else keeps the cooperative kernel and choose_config's pick.
+//   * 64-wide picks (N <= 64, or too few tiles to fill the GPU): a 128 x 128 unit would compute wasted columns or leave SMs idle.
+//   * 256-wide picks: a 128 x 128 unit pulls 1.5x the operand bytes per FLOP of a 128 x 256 tile, which only pays while the epilogue is
+//     a large share of the tile (27-30 % at K = 768 by the cost model, 10-15 % at K = 2048-4096).  Measured on an H100 SXM (700 W):
+//     the Llama-125M K = 768 forward / dgrad calls with 256-wide picks run 8-20 % faster on ping-pong, the Llama-3.2-1B ones at K >= 2048
+//     from 6 % faster to 1.65x the time (the LM-head dgrad at K = 128256).
+static bool use_pingpong(const Config& c, int K, int a_mn, int accumulate, int op, int f32d, int gather, int bn_req, int splits_req,
+                         int pm_req, int pn_req) {
+    return op == OP_BF16 && !f32d && !gather && !accumulate && !a_mn && bn_req <= 0 && splits_req <= 0 && pm_req <= 0 && pn_req <= 0 &&
+           c.splits == 1 && c.pm == 1 && c.pn == 1 && (c.bn == 128 || (c.bn == 256 && K <= 16 * BK));
 }
 
 // Tile order (decode_unit): bands of G super-tile columns.  When all of A [M, K] fits in a third of L2 it stays resident while
@@ -833,7 +1003,8 @@ static int launch(const void* a, long long lda, int a_mn, const void* b, long lo
         if (g_pn > 0 && pn_req <= 0) pn_req = g_pn;
         cfgc = choose_config(M, N, op ? (K + 1) / 2 : K, a_mn, b_mn, accumulate, sms, bn_req, splits_req, pm_req, pn_req, op ? 128 : BN_MAX);
     }
-    const int bn = cfgc.bn, pm = cfgc.pm, pn = cfgc.pn;
+    const bool pingpong = use_pingpong(cfgc, K, a_mn, accumulate, op, f32d, gather, bn_req, splits_req, pm_req, pn_req);
+    const int bn = pingpong ? 128 : cfgc.bn, pm = cfgc.pm, pn = cfgc.pn;   // ping-pong units are 128 x 128
     int splits = cfgc.splits;
     if ((bn_req > 0 && bn != bn_req) || (pm_req > 0 && pm != pm_req) || (pn_req > 0 && pn != pn_req)) return -1;   // request not realisable
     if (b_mn ? ((bn / 64) % pm != 0) : ((bn / pm) % 8 != 0)) return -1;
@@ -917,7 +1088,9 @@ static int launch(const void* a, long long lda, int a_mn, const void* b, long lo
     }
     cfg.attrs = attr;
     cfg.numAttrs = na;
-    const KernelFn fn = f32d ? (op ? fp8_f32acc_kernel_for(bn, op) : f32acc_kernel_for(bn)) : (op ? fp8_kernel_for(bn, op) : kernel_for(bn, a_mn, b_mn));
+    const KernelFn fn = pingpong ? pingpong_kernel_for(b_mn)
+                        : f32d ? (op ? fp8_f32acc_kernel_for(bn, op) : f32acc_kernel_for(bn))
+                               : (op ? fp8_kernel_for(bn, op) : kernel_for(bn, a_mn, b_mn));
     return (int)cudaLaunchKernelEx(&cfg, fn, P);
 }
 
@@ -977,4 +1150,10 @@ extern "C" int acco_gemm_max_clusters(int cl, int sms) {
 extern "C" void acco_gemm_choose(int M, int N, int K, int a_mn, int b_mn, int accumulate, int sms, int* out5) {
     const acco_gemm::Config c = acco_gemm::choose_config(M, N, K, a_mn, b_mn, accumulate, sms, 0, 0, acco_gemm::g_pm, acco_gemm::g_pn);
     out5[0] = c.bn; out5[1] = c.splits; out5[2] = c.pm; out5[3] = c.pn; out5[4] = 1;
+}
+// the schedule launch() runs an unrequested bf16 call of that shape on (introspection for tools / tests): 1 = ping-pong, 0 = cooperative.
+// A call that requests a tile width, K splits or multicast always runs on the cooperative kernel.
+extern "C" int acco_gemm_schedule(int M, int N, int K, int a_mn, int b_mn, int accumulate, int sms) {
+    const acco_gemm::Config c = acco_gemm::choose_config(M, N, K, a_mn, b_mn, accumulate, sms, 0, 0, acco_gemm::g_pm, acco_gemm::g_pn);
+    return acco_gemm::use_pingpong(c, K, a_mn, accumulate, acco_gemm::OP_BF16, 0, 0, 0, 0, acco_gemm::g_pm, acco_gemm::g_pn) ? 1 : 0;
 }

@@ -22,6 +22,8 @@ KERNELS = {
     "gemm_wgmma_bn256_tn.sass": "_ZN9acco_gemm11gemm_kernelILi256ELi0ELi0EEEvNS_6ParamsE",
     "gemm_wgmma_bn256_nn.sass": "_ZN9acco_gemm11gemm_kernelILi256ELi0ELi1EEEvNS_6ParamsE",
     "gemm_wgmma_bn128_tt.sass": "_ZN9acco_gemm11gemm_kernelILi128ELi1ELi1EEEvNS_6ParamsE",
+    "gemm_pingpong_tn.sass": "_ZN9acco_gemm20gemm_pingpong_kernelILi0EEEvNS_6ParamsE",     # forward: ping-pong schedule
+    "gemm_pingpong_nn.sass": "_ZN9acco_gemm20gemm_pingpong_kernelILi1EEEvNS_6ParamsE",     # dgrad: ping-pong schedule
     "rs_adam_ag_multimem_bf16.sass": "_ZN4acco17rs_adam_ag_kernelI13__nv_bfloat16S1_Li2ELb0ELb0EEEvNS_11RoundParamsE",
     "rs_adam_ag_p2p_bf16.sass": "_ZN4acco17rs_adam_ag_kernelI13__nv_bfloat16S1_Li1ELb0ELb0EEEvNS_11RoundParamsE",
     "rs_adam_ag_multimem_bf16_nodecay.sass": "_ZN4acco17rs_adam_ag_kernelI13__nv_bfloat16S1_Li2ELb0ELb1EEEvNS_11RoundParamsE",   # no_decay_1d
