@@ -26,6 +26,10 @@ int acco_ce_fwd(const void* logits, const long long* labels, float* lse, float* 
                 int V, int Vp, long long ignore_index, float label_smoothing, float z_loss, float* z_out, cudaStream_t st);
 int acco_ce_bwd(void* logits, const long long* labels, const float* lse, const float* scale, long long T, int V, int Vp,
                 long long ignore_index, float label_smoothing, float z_loss, cudaStream_t st);
+int acco_kd_fwd(const void* student, const void* teacher, const long long* labels, float* lse3, float* rows, float* loss, float* inv_n,
+                float* out, long long T, int V, int Vp, long long ignore_index, float alpha, float temperature, cudaStream_t st);
+int acco_kd_bwd(void* student, const void* teacher, const long long* labels, const float* lse3, const float* scale, long long T, int V, int Vp,
+                long long ignore_index, float alpha, float temperature, cudaStream_t st);
 int acco_norm_bwd_acc_f32(const void* dy, const void* dh_extra, const void* h, const void* w, const float* mean, const float* rstd, void* dh,
                           float* partial, float* dw_accum, float* db_accum, int T, int H, int grid, cudaStream_t st);
 int acco_embedding_bwd(void* grad, const long long* sorted, const long long* perm, const void* dy, int T, int H, int sms, cudaStream_t st);
@@ -336,6 +340,51 @@ void ce_bwd_inplace(torch::Tensor logits, torch::Tensor labels, torch::Tensor ls
     const int64_t T = logits.size(0), Vp = logits.size(1);
     TORCH_CHECK(acco_ce_bwd(logits.data_ptr(), (const long long*)labels.data_ptr<int64_t>(), lse.data_ptr<float>(), scale.data_ptr<float>(), T,
                             (int)V, (int)Vp, ignore_index, (float)label_smoothing, (float)z_loss, stream()) == 0, "ce_bwd: bad shapes");
+}
+
+// ---------------------------------------------------------------- knowledge distillation
+void check_distill(const torch::Tensor& s, const torch::Tensor& t, const torch::Tensor& labels, int64_t V, double alpha, double temperature) {
+    check_bf16(s, "logits"); check_bf16(t, "teacher_logits");
+    TORCH_CHECK(s.dim() == 2 && t.sizes() == s.sizes() && t.device() == s.device(), "teacher_logits must match the student logits' [T, Vp] shape "
+                "and device, got ", t.sizes(), " vs ", s.sizes());
+    TORCH_CHECK(labels.is_cuda() && labels.scalar_type() == torch::kInt64 && labels.is_contiguous() && labels.numel() == s.size(0),
+                "labels must be contiguous CUDA int64 with one entry per row");
+    TORCH_CHECK(s.size(1) % 8 == 0 && V > 0 && V <= s.size(1), "distillation: padded vocab must be a multiple of 8 and >= V, got V=", V,
+                " Vp=", s.size(1));
+    TORCH_CHECK(std::isfinite(alpha) && alpha > 0.0 && alpha <= 1.0 && (float)alpha > 0.f, "alpha must be in (0, 1], got ", alpha);
+    TORCH_CHECK(std::isfinite(temperature) && temperature > 0.0 && std::isfinite((float)temperature) && (float)temperature > 0.f,
+                "temperature must be finite and > 0, got ", temperature);
+}
+
+// Returns (loss, inv_n, lse3 [3, T]); `out` (two fp32 on the logits' device) receives the mean CE and the mean KL.
+std::vector<torch::Tensor> kd_fwd(torch::Tensor logits, torch::Tensor teacher_logits, torch::Tensor labels, int64_t V, int64_t ignore_index,
+                                  double alpha, double temperature, torch::Tensor out) {
+    check_distill(logits, teacher_logits, labels, V, alpha, temperature);
+    TORCH_CHECK(out.is_cuda() && out.device() == logits.device() && out.scalar_type() == torch::kFloat32 && out.numel() == 2 && out.is_contiguous(),
+                "out must be a contiguous two-element fp32 tensor on the logits' device");
+    const c10::cuda::CUDAGuard guard(logits.device());
+    const int64_t T = logits.size(0), Vp = logits.size(1);
+    auto f32 = logits.options().dtype(torch::kFloat32);
+    auto lse3 = torch::empty({3, T}, f32);
+    auto rows = torch::empty({2, T}, f32);
+    auto loss = torch::empty({}, f32);
+    auto inv_n = torch::empty({1}, f32);
+    TORCH_CHECK(acco_kd_fwd(logits.data_ptr(), teacher_logits.data_ptr(), (const long long*)labels.data_ptr<int64_t>(), lse3.data_ptr<float>(),
+                            rows.data_ptr<float>(), loss.data_ptr<float>(), inv_n.data_ptr<float>(), out.data_ptr<float>(), T, (int)V, (int)Vp,
+                            ignore_index, (float)alpha, (float)temperature, stream()) == 0, "kd_fwd: bad arguments");
+    return {loss, inv_n, lse3};
+}
+
+void kd_bwd_inplace(torch::Tensor logits, torch::Tensor teacher_logits, torch::Tensor labels, torch::Tensor lse3, torch::Tensor scale, int64_t V,
+                    int64_t ignore_index, double alpha, double temperature) {
+    check_distill(logits, teacher_logits, labels, V, alpha, temperature);
+    check_f32(lse3, "lse3"); check_f32(scale, "scale");
+    TORCH_CHECK(lse3.numel() == 3 * logits.size(0), "lse3 must hold 3 x T values");
+    const c10::cuda::CUDAGuard guard(logits.device());
+    const int64_t T = logits.size(0), Vp = logits.size(1);
+    TORCH_CHECK(acco_kd_bwd(logits.data_ptr(), teacher_logits.data_ptr(), (const long long*)labels.data_ptr<int64_t>(), lse3.data_ptr<float>(),
+                            scale.data_ptr<float>(), T, (int)V, (int)Vp, ignore_index, (float)alpha, (float)temperature, stream()) == 0,
+                "kd_bwd: bad arguments");
 }
 
 // ---------------------------------------------------------------- fused round kernel
@@ -794,6 +843,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("z_loss") = 0.0, py::arg("z_out") = py::none());
     m.def("ce_bwd_inplace", &ce_bwd_inplace, py::arg("logits"), py::arg("labels"), py::arg("lse"), py::arg("scale"), py::arg("V"),
           py::arg("ignore_index"), py::arg("label_smoothing") = 0.0, py::arg("z_loss") = 0.0);
+    m.def("kd_fwd", &kd_fwd, py::arg("logits"), py::arg("teacher_logits"), py::arg("labels"), py::arg("V"), py::arg("ignore_index"),
+          py::arg("alpha"), py::arg("temperature"), py::arg("out"));
+    m.def("kd_bwd_inplace", &kd_bwd_inplace, py::arg("logits"), py::arg("teacher_logits"), py::arg("labels"), py::arg("lse3"), py::arg("scale"),
+          py::arg("V"), py::arg("ignore_index"), py::arg("alpha"), py::arg("temperature"));
     m.def("adamw_shard", &adamw_shard, py::arg("grad_sum"), py::arg("master"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("stash"),
           py::arg("out"), py::arg("inv_count"), py::arg("scratch"), py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"), py::arg("wd"),
           py::arg("step"), py::arg("commit"), py::arg("add_stash"), py::arg("write_stash"), py::arg("no_decay_ranges") = py::none(),

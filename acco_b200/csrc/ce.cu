@@ -19,6 +19,17 @@
 // The forward adds the term at the row end from the lse it already has; ce_reduce also writes the mean z-term over the
 // non-ignored rows to `z_out`; the backward forms 1 + 2 z lse once per row.  z = 0 launches the kZ = false instantiations,
 // which ignore `z` and `z_out` and compile to the same code as before the z-loss existed.
+//
+// Knowledge distillation (kd_*, separate kernels; the ce_* instantiations above are untouched).  Student logits s and frozen
+// teacher logits t, both bf16 [T, Vp], temperature T > 0 and weight a in (0, 1]; per non-ignored row
+//   row = (1 - a) (lse(s) - s[y])  +  a T^2 KL(softmax(t/T) || softmax(s/T)),
+//   KL  = sum_c q_c (t_c/T - s_c/T) - lse(t/T) + lse(s/T),   q = softmax(t/T),
+//   d s_c = scale ((1 - a) (softmax(s)_c - [c = y]) + a T (softmax(s/T)_c - q_c))      (c < V; padding, ignored rows: 0).
+//   kd_fwd : one CTA per row, ONE streaming pass over both rows: online max/sum of s, of s/T and of t/T, plus the running sum
+//            K = sum e^{t/T - m} (t/T - s/T) rescaled with the t/T sum, so sum_c q_c (t/T - s/T) = K / S at the row end.
+//            Stores lse(s), lse(s/T), lse(t/T) [3, T] and the row's CE and KL [2, T].  kT1 (T == 1) shares the first two.
+//   kd_reduce : ce_reduce's order -> objective, inv_n, and out[2] = (mean CE, mean KL) over the non-ignored rows.
+//   kd_bwd : in place on s, reading t once more.
 #include "common.cuh"
 
 namespace acco {
@@ -182,6 +193,193 @@ void launch_ce_bwd(void* logits, const long long* labels, const float* lse, cons
                                                                    one_m_eps, eps_v, z);
 }
 
+// ---------------------------------------------------------------- knowledge distillation
+// Online update of (m, sum) with 8 values already in the softmax's scale.
+ACCO_DEVINL void online8(const float (&f)[8], float& m, float& s) {
+    float lm = f[0];
+#pragma unroll
+    for (int j = 1; j < 8; ++j) lm = fmaxf(lm, f[j]);
+    const float nm = fmaxf(m, lm);
+    float acc = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc += __expf(f[j] - nm);
+    s = s * __expf(m - nm) + acc;
+    m = nm;
+}
+
+// lse of the CTA from each thread's (m, s); every thread gets it.
+ACCO_DEVINL float block_lse(float m, float s, float* red) {
+    const float gm = block_max(m, red);
+    const float part = (m == -INFINITY) ? 0.f : s * __expf(m - gm);
+    return gm + __logf(block_sum(part, red));
+}
+
+// lse3 [3, T]: lse(s), lse(s/T), lse(t/T); rows [2, T]: CE and KL of the row (all 0 on ignored rows).  inv_t = 1/T (fp32, host).
+template <bool kT1>
+__global__ void __launch_bounds__(kCEThreads) kd_fwd_kernel(const __nv_bfloat16* __restrict__ student, const __nv_bfloat16* __restrict__ teacher,
+                                                            const long long* __restrict__ labels, float* __restrict__ lse3,
+                                                            float* __restrict__ rows, long long T, int V, int Vp, long long ignore_index,
+                                                            float inv_t) {
+    __shared__ float red[32];
+    const long long row = blockIdx.x;
+    const __nv_bfloat16* x = student + row * (size_t)Vp;
+    const __nv_bfloat16* y = teacher + row * (size_t)Vp;
+    const long long label = labels[row];
+    if (label == ignore_index) {
+        if (threadIdx.x == 0) {
+            lse3[row] = lse3[T + row] = lse3[2 * T + row] = 0.f;
+            rows[row] = rows[T + row] = 0.f;
+        }
+        return;
+    }
+    const int nvec_full = V >> 3;
+    float m1 = -INFINITY, s1 = 0.f;        // s
+    float m2 = -INFINITY, s2 = 0.f;        // s / T  (!kT1)
+    float m3 = -INFINITY, s3 = 0.f;        // t / T
+    float k3 = 0.f;                        // sum e^{t/T - m3} (t/T - s/T), rescaled with s3
+    for (int v = threadIdx.x; v < nvec_full; v += kCEThreads) {
+        float f[8], g[8];
+        unpack8(ld_stream(x + 8 * v), f);
+        unpack8(ld_stream(y + 8 * v), g);
+        online8(f, m1, s1);
+        if constexpr (!kT1) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) { f[j] *= inv_t; g[j] *= inv_t; }
+            online8(f, m2, s2);
+        }
+        float lm = g[0];
+#pragma unroll
+        for (int j = 1; j < 8; ++j) lm = fmaxf(lm, g[j]);
+        const float nm = fmaxf(m3, lm);
+        float acc = 0.f, acck = 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const float e = __expf(g[j] - nm);
+            acc += e;
+            acck += e * (g[j] - f[j]);
+        }
+        const float r = __expf(m3 - nm);
+        s3 = s3 * r + acc;
+        k3 = k3 * r + acck;
+        m3 = nm;
+    }
+    for (int c = (nvec_full << 3) + threadIdx.x; c < V; c += kCEThreads) {
+        float f = __bfloat162float(x[c]), g = __bfloat162float(y[c]);
+        float nm = fmaxf(m1, f);
+        s1 = s1 * __expf(m1 - nm) + __expf(f - nm);
+        m1 = nm;
+        if constexpr (!kT1) {
+            f *= inv_t;
+            g *= inv_t;
+            nm = fmaxf(m2, f);
+            s2 = s2 * __expf(m2 - nm) + __expf(f - nm);
+            m2 = nm;
+        }
+        nm = fmaxf(m3, g);
+        const float r = __expf(m3 - nm), e = __expf(g - nm);
+        s3 = s3 * r + e;
+        k3 = k3 * r + e * (g - f);
+        m3 = nm;
+    }
+    const float lse1 = block_lse(m1, s1, red);
+    float lse2 = lse1;
+    if constexpr (!kT1) lse2 = block_lse(m2, s2, red);
+    const float gm3 = block_max(m3, red);
+    const float w = (m3 == -INFINITY) ? 0.f : __expf(m3 - gm3);
+    const float gs3 = block_sum(s3 * w, red);
+    const float gk3 = block_sum(k3 * w, red);
+    if (threadIdx.x == 0) {
+        const float lse_t = gm3 + __logf(gs3);
+        lse3[row] = lse1;
+        lse3[T + row] = lse2;
+        lse3[2 * T + row] = lse_t;
+        rows[row] = lse1 - __bfloat162float(x[label]);
+        rows[T + row] = (gk3 / gs3 - lse_t) + lse2;
+    }
+}
+
+// loss = (one_m_a sum CE + a_t2 sum KL) / n; out = (sum CE / n, sum KL / n); the sums in ce_reduce_kernel's order.
+__global__ void __launch_bounds__(1024) kd_reduce_kernel(const float* __restrict__ rows, const long long* __restrict__ labels,
+                                                         float* __restrict__ loss, float* __restrict__ inv_n, float* __restrict__ out,
+                                                         long long T, long long ignore_index, float one_m_a, float a_t2) {
+    __shared__ float red[32];
+    float sc = 0.f, sk = 0.f, n = 0.f;
+    for (long long i = threadIdx.x; i < T; i += blockDim.x) {
+        if (labels[i] != ignore_index) {
+            sc += rows[i];
+            sk += rows[T + i];
+            n += 1.f;
+        }
+    }
+    sc = block_sum(sc, red);
+    sk = block_sum(sk, red);
+    n = block_sum(n, red);
+    if (threadIdx.x == 0) {
+        const float inv = n > 0.f ? 1.f / n : 0.f;
+        const float ce = sc * inv, kl = sk * inv;
+        *loss = one_m_a * ce + a_t2 * kl;
+        *inv_n = inv;
+        out[0] = ce;
+        out[1] = kl;
+    }
+}
+
+// s <- scale ((1 - a)(softmax(s) - onehot) + a T (softmax(s/T) - softmax(t/T))); kT1: scale (softmax(s) - (1 - a) onehot - a q).
+template <bool kT1>
+__global__ void __launch_bounds__(kCEThreads) kd_bwd_kernel(__nv_bfloat16* __restrict__ student, const __nv_bfloat16* __restrict__ teacher,
+                                                            const long long* __restrict__ labels, const float* __restrict__ lse3,
+                                                            const float* __restrict__ scale_ptr, long long T, int V, int Vp,
+                                                            long long ignore_index, float one_m_a, float a_t, float inv_t) {
+    const long long row = blockIdx.x;
+    __nv_bfloat16* x = student + row * (size_t)Vp;
+    const __nv_bfloat16* y = teacher + row * (size_t)Vp;
+    const long long label = labels[row];
+    const int nvec = Vp >> 3;
+    if (label == ignore_index) {
+        bf16x8 z;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) z.v[i] = __floats2bfloat162_rn(0.f, 0.f);
+        for (int v = threadIdx.x; v < nvec; v += kCEThreads) st_stream(x + 8 * v, z);
+        return;
+    }
+    const float lse1 = lse3[row], lse2 = lse3[T + row], lse_t = lse3[2 * T + row];
+    const float scale = *scale_ptr;
+    for (int v = threadIdx.x; v < nvec; v += kCEThreads) {
+        float f[8], g[8];
+        unpack8(ld_stream_rw(x + 8 * v), f);
+        unpack8(ld_stream(y + 8 * v), g);
+        const int c0 = 8 * v;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int c = c0 + j;
+            float d = 0.f;
+            if (c < V) {
+                const float p = __expf(f[j] - lse1);
+                if constexpr (kT1) {
+                    d = p - a_t * __expf(g[j] - lse_t);                  // a_t = a when T == 1
+                } else {
+                    d = one_m_a * p + a_t * (__expf(f[j] * inv_t - lse2) - __expf(g[j] * inv_t - lse_t));
+                }
+                if (c == label) d -= one_m_a;
+            }
+            f[j] = d * scale;
+        }
+        st_stream(x + 8 * v, pack8(f));
+    }
+}
+
+template <bool kT1>
+void launch_kd(const void* s, const void* t, const long long* labels, float* lse3, float* rows, float* loss, float* inv_n, float* out,
+               long long T, int V, int Vp, long long ignore_index, float one_m_a, float a_t2, float inv_t, cudaStream_t st) {
+    kd_fwd_kernel<kT1><<<(unsigned)T, kCEThreads, 0, st>>>((const __nv_bfloat16*)s, (const __nv_bfloat16*)t, labels, lse3, rows, T, V, Vp,
+                                                           ignore_index, inv_t);
+    kd_reduce_kernel<<<1, 1024, 0, st>>>(rows, labels, loss, inv_n, out, T, ignore_index, one_m_a, a_t2);
+}
+
+bool kd_args_ok(int V, int Vp, float alpha, float temperature) {
+    return Vp % 8 == 0 && V > 0 && V <= Vp && alpha > 0.f && alpha <= 1.f && temperature > 0.f && temperature < INFINITY;
+}
+
 }  // namespace acco
 
 // `label_smoothing` in [0, 1] and `z_loss` >= 0 (checked by the binding); 0 runs the instantiation without the term.  With
@@ -206,5 +404,27 @@ extern "C" int acco_ce_bwd(void* logits, const long long* labels, const float* l
     auto f = smooth ? (zl ? acco::launch_ce_bwd<true, true> : acco::launch_ce_bwd<true, false>)
                     : (zl ? acco::launch_ce_bwd<false, true> : acco::launch_ce_bwd<false, false>);
     f(logits, labels, lse, scale, T, V, Vp, ignore_index, one_m_eps, eps_v, z_loss, st);
+    return 0;
+}
+
+// Knowledge distillation: `alpha` in (0, 1], finite `temperature` > 0, Vp % 8 == 0 and V <= Vp, else -1 (nothing launched).
+// `out` (two fp32) receives the mean CE and the mean KL over the non-ignored rows.
+extern "C" int acco_kd_fwd(const void* student, const void* teacher, const long long* labels, float* lse3, float* rows, float* loss,
+                           float* inv_n, float* out, long long T, int V, int Vp, long long ignore_index, float alpha, float temperature,
+                           cudaStream_t st) {
+    if (!acco::kd_args_ok(V, Vp, alpha, temperature) || out == nullptr) return -1;
+    const float one_m_a = 1.f - alpha, a_t2 = alpha * temperature * temperature, inv_t = 1.f / temperature;
+    auto f = temperature == 1.f ? acco::launch_kd<true> : acco::launch_kd<false>;
+    f(student, teacher, labels, lse3, rows, loss, inv_n, out, T, V, Vp, ignore_index, one_m_a, a_t2, inv_t, st);
+    return 0;
+}
+
+extern "C" int acco_kd_bwd(void* student, const void* teacher, const long long* labels, const float* lse3, const float* scale, long long T,
+                           int V, int Vp, long long ignore_index, float alpha, float temperature, cudaStream_t st) {
+    if (!acco::kd_args_ok(V, Vp, alpha, temperature)) return -1;
+    const float one_m_a = 1.f - alpha, a_t = alpha * temperature, inv_t = 1.f / temperature;
+    auto k = temperature == 1.f ? acco::kd_bwd_kernel<true> : acco::kd_bwd_kernel<false>;
+    k<<<(unsigned)T, acco::kCEThreads, 0, st>>>((__nv_bfloat16*)student, (const __nv_bfloat16*)teacher, labels, lse3, scale, T, V, Vp,
+                                                ignore_index, one_m_a, a_t, inv_t);
     return 0;
 }

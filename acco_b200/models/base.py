@@ -54,6 +54,11 @@ class NativeCausalLM(nn.Module):
         self.label_smoothing = 0.0   # label smoothing of the loss when labels are given (train key `label_smoothing_factor`)
         self.z_loss_weight = 0.0     # z * mean lse^2 added to the loss (train key `z_loss_weight`, ops/cross_entropy.py)
         self.z_loss_out: Optional[torch.Tensor] = None   # one fp32 on the device: receives the z-term of each loss computed
+        # knowledge distillation (train key `distill_teacher`): the weight a and temperature T of a forward given teacher_logits,
+        # and two fp32 on the device that receive each such loss's mean CE and mean KL (ops.distill_cross_entropy)
+        self.distill_alpha = 0.5
+        self.distill_temperature = 1.0
+        self.distill_out: Optional[torch.Tensor] = None
 
     @property
     def embed_weight(self) -> torch.Tensor:
@@ -84,17 +89,30 @@ class NativeCausalLM(nn.Module):
             self.lm_head[V:].zero_()
 
     # ------------------------------------------------------------------ loss
-    def _lm_output(self, logits: torch.Tensor, labels: Optional[torch.Tensor], B: int, S: int) -> CausalLMOutput:
-        """Logits ``[B*S, Vp]`` -> the logits cut to ``vocab_size`` without labels, else the mean cross-entropy loss."""
+    def _lm_output(self, logits: torch.Tensor, labels: Optional[torch.Tensor], B: int, S: int,
+                   teacher_logits: Optional[torch.Tensor] = None) -> CausalLMOutput:
+        """Logits ``[B*S, Vp]`` -> the logits cut to ``vocab_size`` without labels, else the mean cross-entropy loss, or with
+        ``teacher_logits`` (a teacher's :meth:`padded_logits` on the same tokens) the distillation objective, over the same rows."""
         V = self.config.vocab_size
         if labels is None:
+            if teacher_logits is not None:
+                raise ValueError("teacher_logits needs labels: the distillation loss is taken over the rows the labels keep")
             return CausalLMOutput(loss=None, logits=logits.view(B, S, -1)[..., :V])
         # HF shift: position t predicts token t+1; the last position has no target
         shifted = torch.full_like(labels, -100)
         shifted[:, :-1] = labels[:, 1:]
+        if teacher_logits is not None:
+            if self.label_smoothing or self.z_loss_weight:
+                raise ValueError("distillation cannot be combined with label smoothing or the z-loss")
+            loss = ops.distill_cross_entropy(logits, teacher_logits, shifted.reshape(B * S), V, self.distill_alpha,
+                                             self.distill_temperature, out=self.distill_out)
+            return CausalLMOutput(loss=loss, logits=None)
         loss = ops.softmax_cross_entropy(logits, shifted.reshape(B * S), V, -100, label_smoothing=self.label_smoothing,
                                          z_loss=self.z_loss_weight, z_loss_out=self.z_loss_out)
         return CausalLMOutput(loss=loss, logits=None)
+
+    def padded_logits(self, input_ids: torch.Tensor, position_ids: Optional[torch.Tensor] = None) -> torch.Tensor:
+        raise NotImplementedError
 
     # ------------------------------------------------------------------ HF-compatible checkpoints
     def _hf_tensors(self) -> List[Tuple[str, torch.Tensor]]:

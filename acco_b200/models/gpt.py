@@ -162,10 +162,17 @@ class GPTForCausalLM(NativeCausalLM):
         return n
 
     def forward(self, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor] = None,
-                labels: Optional[torch.Tensor] = None, position_ids: Optional[torch.Tensor] = None, **unused) -> CausalLMOutput:
+                labels: Optional[torch.Tensor] = None, position_ids: Optional[torch.Tensor] = None,
+                teacher_logits: Optional[torch.Tensor] = None, **unused) -> CausalLMOutput:
         """HF-style call; ``attention_mask`` is accepted for API compatibility (right padding + causal attention: logits at
         non-pad positions do not depend on it; pad positions carry ``labels == -100``).  ``position_ids [B, S]`` marks packed rows
-        (``PackedCollator``): the learned positions are gathered per token and no token attends to another sample."""
+        (``PackedCollator``): the learned positions are gathered per token and no token attends to another sample.
+        ``teacher_logits [B*S, Vp]`` (with labels): the loss is the distillation objective (:meth:`_lm_output`)."""
+        B, S = input_ids.shape
+        return self._lm_output(self.padded_logits(input_ids, position_ids), labels, B, S, teacher_logits)
+
+    def padded_logits(self, input_ids: torch.Tensor, position_ids: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The LM head's output ``[B*S, Vp]``, vocabulary padding included (a distillation teacher's logits)."""
         cfg = self.config
         B, S = input_ids.shape
         T = B * S
@@ -198,8 +205,7 @@ class GPTForCausalLM(NativeCausalLM):
             n = ops.layernorm(h, tr.ln_f.weight, tr.ln_f.bias, eps)
         else:
             n, h = ops.add_layernorm(branch, h, tr.ln_f.weight, tr.ln_f.bias, eps)
-        logits = ops.linear(n, self.head_weight)                                                  # [T, Vp]
-        return self._lm_output(logits, labels, B, S)
+        return ops.linear(n, self.head_weight)                                                  # [T, Vp]
 
     def _hf_tensors(self) -> List[Tuple[str, torch.Tensor]]:
         """HF ``GPTNeoForCausalLM`` keys: the fused QKV weight is split back into HF's three projections."""

@@ -159,12 +159,19 @@ class LlamaForCausalLM(NativeCausalLM):
 
     # ------------------------------------------------------------------ forward
     def forward(self, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor] = None,
-                labels: Optional[torch.Tensor] = None, position_ids: Optional[torch.Tensor] = None, **unused) -> CausalLMOutput:
+                labels: Optional[torch.Tensor] = None, position_ids: Optional[torch.Tensor] = None,
+                teacher_logits: Optional[torch.Tensor] = None, **unused) -> CausalLMOutput:
         """HF-style call.  ``attention_mask`` is accepted for API compatibility; with right
         padding and causal attention the logits at non-pad positions do not depend on it, and pad
         positions carry ``labels == -100`` (the collator's job), so it is not applied.
         ``position_ids [B, S]`` marks packed rows (``PackedCollator``): positions restart at 0 for every sample, RoPE uses them
-        and no token attends to another sample."""
+        and no token attends to another sample.
+        ``teacher_logits [B*S, Vp]`` (with labels): the loss is the distillation objective (:meth:`_lm_output`)."""
+        B, S = input_ids.shape
+        return self._lm_output(self.padded_logits(input_ids, position_ids), labels, B, S, teacher_logits)
+
+    def padded_logits(self, input_ids: torch.Tensor, position_ids: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The LM head's output ``[B*S, Vp]``, vocabulary padding included (a distillation teacher's logits)."""
         cfg = self.config
         B, S = input_ids.shape
         T = B * S
@@ -195,8 +202,7 @@ class LlamaForCausalLM(NativeCausalLM):
             n = ops.rmsnorm(h, self.model.norm.weight, eps)
         else:
             n, h = ops.add_rmsnorm(branch, h, self.model.norm.weight, eps)
-        logits = ops.linear(n, self.head_weight, gathered=self._gw(self.head_weight) if self.lm_head is not None else None)   # [T, Vp]
-        return self._lm_output(logits, labels, B, S)
+        return ops.linear(n, self.head_weight, gathered=self._gw(self.head_weight) if self.lm_head is not None else None)   # [T, Vp]
 
     def _hf_tensors(self) -> List[Tuple[str, torch.Tensor]]:
         """HF ``LlamaForCausalLM`` keys: the fused QKV and gate|up weights are split back into HF's projections."""

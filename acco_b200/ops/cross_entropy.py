@@ -19,7 +19,16 @@ The kernels take the row sum of the logits in the same streaming pass; ``eps = 0
 
 with ``ce_r`` the (smoothed) row loss above.  The forward adds the term from the ``lse`` it already computes, the backward forms
 ``1 + 2 z lse`` once per row; ``z = 0`` runs the kernels without the term.  ``z_loss_out`` (a one-element fp32 tensor) receives the
-mean z-term, so the cross-entropy alone is ``loss - z_loss_out``; it is written on the device, without a host sync."""
+mean z-term, so the cross-entropy alone is ``loss - z_loss_out``; it is written on the device, without a host sync.
+
+:func:`distill_cross_entropy` is knowledge distillation from a frozen teacher's logits ``t`` (same padded ``[T, Vp]`` layout),
+temperature ``T > 0`` and weight ``a`` in (0, 1] (Hinton's forward KL, teacher entropy included, so >= 0 and 0 for ``t == s``)::
+
+    loss = mean over rows r with label != -100 of  (1 - a) (lse(s_r) - s_r[y_r])  +  a T^2 KL(softmax(t_r / T) || softmax(s_r / T))
+    d s_rc = scale ((1 - a) (softmax(s_r)_c - [c = y_r]) + a T (softmax(s_r / T)_c - softmax(t_r / T)_c))      (c < V; else 0)
+
+The kernels make one streaming pass over both rows forward and one more backward (in place on ``s``), with no fp32 copy of
+either; ``out`` (two fp32) receives the mean CE and the mean KL on the device.  The teacher logits are read, never written."""
 from __future__ import annotations
 
 import math
@@ -90,3 +99,70 @@ def softmax_cross_entropy(logits: torch.Tensor, labels: torch.Tensor, valid_voca
     if use_kernels(logits) and logits.dtype == torch.bfloat16:
         return _CEFn.apply(logits, labels, V, ignore_index, label_smoothing, z_loss, z_loss_out)
     return softmax_cross_entropy_ref(logits, labels, V, ignore_index, label_smoothing, z_loss, z_loss_out)
+
+
+# ------------------------------------------------------------------------------------------------ knowledge distillation
+def distill_cross_entropy_ref(logits: torch.Tensor, teacher_logits: torch.Tensor, labels: torch.Tensor, valid_vocab: int, alpha: float,
+                              temperature: float, out: Optional[torch.Tensor] = None, ignore_index: int = -100) -> torch.Tensor:
+    """fp32 reference of :func:`distill_cross_entropy` (the CPU and non-bf16 path)."""
+    V, T, a = int(valid_vocab), float(temperature), float(alpha)
+    x = logits[..., :V].float().reshape(-1, V)
+    t = teacher_logits[..., :V].detach().float().reshape(-1, V)
+    lb = labels.reshape(-1)
+    valid = lb != ignore_index
+    n = valid.sum().clamp(min=1)
+    ce = F.cross_entropy(x, lb, ignore_index=ignore_index, reduction="sum") / n
+    lq = torch.log_softmax(t[valid] / T, -1)
+    kl = (lq.exp() * (lq - torch.log_softmax(x[valid] / T, -1))).sum() / n
+    if out is not None:
+        out.copy_(torch.stack([ce.detach(), kl.detach()]).reshape(out.shape))
+    return (1.0 - a) * ce + a * T * T * kl
+
+
+def _check_distill(alpha: float, temperature: float, out: Optional[torch.Tensor]) -> None:
+    if isinstance(alpha, bool) or not (math.isfinite(alpha) and 0.0 < alpha <= 1.0):
+        raise ValueError(f"alpha must be in (0, 1], got {alpha!r}")
+    if isinstance(temperature, bool) or not (math.isfinite(temperature) and temperature > 0.0):
+        raise ValueError(f"temperature must be finite and > 0, got {temperature!r}")
+    if out is not None and (out.numel() != 2 or out.dtype != torch.float32):
+        raise ValueError("out must be a two-element fp32 tensor")
+
+
+class _KDFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, logits, teacher_logits, labels, valid_vocab, alpha, temperature, out):
+        C = load_ext(required=True)
+        lg = logits.reshape(-1, logits.shape[-1])
+        tl = teacher_logits.reshape(-1, teacher_logits.shape[-1])
+        assert lg.is_contiguous() and tl.is_contiguous()
+        lb = labels.reshape(-1).contiguous()
+        if out is None:
+            out = torch.empty(2, device=lg.device, dtype=torch.float32)
+        loss, inv_n, lse3 = C.kd_fwd(lg, tl, lb, int(valid_vocab), -100, float(alpha), float(temperature), out)
+        count_launch("kd_fwd", 2)
+        ctx.save_for_backward(lg, tl, lb, lse3, inv_n)
+        ctx.valid_vocab, ctx.shape, ctx.alpha, ctx.temperature = int(valid_vocab), logits.shape, float(alpha), float(temperature)
+        return loss
+
+    @staticmethod
+    def backward(ctx, dloss):
+        C = load_ext(required=True)
+        lg, tl, lb, lse3, inv_n = ctx.saved_tensors
+        scale = dloss.float().reshape(1) * inv_n
+        C.kd_bwd_inplace(lg, tl, lb, lse3, scale, ctx.valid_vocab, -100, ctx.alpha, ctx.temperature)
+        count_launch("kd_bwd")
+        return lg.view(ctx.shape), None, None, None, None, None, None
+
+
+def distill_cross_entropy(logits: torch.Tensor, teacher_logits: torch.Tensor, labels: torch.Tensor, V: int, alpha: float,
+                          temperature: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``(1 - alpha)`` mean CE plus ``alpha T^2`` mean forward KL to the teacher's tempered softmax over the rows whose (shifted)
+    label is not -100; ``out`` (two fp32), when given, receives the mean CE and the mean KL.  The teacher gets no gradient.
+    NOTE (kernel path): ``logits`` is consumed - its storage is reused for the gradient during backward."""
+    _check_distill(alpha, temperature, out)
+    alpha, temperature = float(alpha), float(temperature)
+    if teacher_logits.shape != logits.shape:
+        raise ValueError(f"teacher_logits {tuple(teacher_logits.shape)} must match the student logits {tuple(logits.shape)}")
+    if use_kernels(logits, teacher_logits) and logits.dtype == torch.bfloat16:
+        return _KDFn.apply(logits, teacher_logits.detach(), labels, int(V), alpha, temperature, out)
+    return distill_cross_entropy_ref(logits, teacher_logits, labels, V, alpha, temperature, out)

@@ -72,6 +72,9 @@ TRAIN_DEFAULTS: Dict[str, Any] = dict(
     grad_accum_dtype=None,          # "fp32": fp32 gradient accumulators under bf16 weights (bound as p.main_grad); None: the weights' dtype
     document_mask=False,            # const-len rows: no attention across the documents of a row, positions restart per document
     z_loss_weight=0,                # native models: add z * mean lse^2 (PaLM z-loss) to every training micro-batch's loss; logged as z_loss
+    distill_teacher=None,           # HF checkpoint dir of a frozen native teacher: train on (1-a) CE + a T^2 KL(teacher || student)
+    distill_alpha=0.5,              # a in (0, 1]: weight of the distillation term
+    distill_temperature=1.0,        # T > 0: temperature of both softmaxes in the KL
 )
 
 
@@ -140,7 +143,7 @@ class DecoupledTrainer:
     # ================================================================== construction
     def __init__(self, model: nn.Module = None, tokenizer=None, train_dataset=None, eval_dataset=None, args=None,
                  log=None, text_column_name: str = "text", preprocess_dataset_fn: Optional[Callable] = None,
-                 run_name: str = "", env: Optional[DistEnv] = None):
+                 run_name: str = "", env: Optional[DistEnv] = None, teacher: Optional[nn.Module] = None):
         self.model, self.tokenizer = model, tokenizer
         self.train_dataset, self.eval_dataset = train_dataset, eval_dataset
         self.raw_args = args
@@ -163,11 +166,13 @@ class DecoupledTrainer:
         self._check_grad_accum_dtype()
         self._fused_smoothing = self._check_label_smoothing()
         self.z_loss_weight = self._check_z_loss()
+        teacher_src = self._check_distill(teacher)
         if not isinstance(self.args.no_decay_1d, bool):
             raise ValueError(f"no_decay_1d must be true or false, got {self.args.no_decay_1d!r}")
         self.no_decay_1d = self.args.no_decay_1d
 
         self.initialize_com(env)
+        self.teacher = self._setup_teacher(teacher_src)
         if self._fused_smoothing and self.rank == 0:
             self.log.info(f">>> label_smoothing_factor={self._fused_smoothing}: smoothed inside the fused cross-entropy kernel "
                           f"of {type(self.model).__name__} (CUDA graphs stay available)")
@@ -192,6 +197,13 @@ class DecoupledTrainer:
             self.z_loss_host = self.z_loss_host.pin_memory()
         if self.z_loss_weight:
             self.model.z_loss_out = self.z_loss_static
+        # distillation: each micro-batch's mean CE and mean KL, written on the device like the z-term
+        self.distill_static = torch.zeros(2, device=self.device, dtype=torch.float32)
+        self.distill_host = torch.zeros(2, dtype=torch.float32)
+        if self.is_cuda:
+            self.distill_host = self.distill_host.pin_memory()
+        if self.teacher is not None:
+            self.model.distill_out = self.distill_static
         self.n_grad_acc_ddp = 1
         self._hook_extra_microbatches: Optional[Callable[[int, int], int]] = None   # tests: (rank, round) -> extra
         self._nvtx = os.environ.get("ACCO_NVTX") == "1"
@@ -401,6 +413,55 @@ class DecoupledTrainer:
         self.model.z_loss_weight = float(z)
         return float(z)
 
+    def _check_distill(self, teacher: Optional[nn.Module]):
+        """Validates the distillation keys and returns the teacher source: the ``teacher`` module, the ``distill_teacher``
+        checkpoint directory, or None (off).  The student must be native; label smoothing and the z-loss are not combined with it."""
+        a = self.args
+        path = a.distill_teacher
+        if teacher is not None and path is not None:
+            raise ValueError("give the distillation teacher either as the trainer's teacher= argument or as distill_teacher, not both")
+        src = teacher if teacher is not None else path
+        if src is None:
+            return None
+        if path is not None and not isinstance(path, (str, os.PathLike)):
+            raise ValueError(f"distill_teacher must be a checkpoint directory, got {path!r}")
+        alpha, temp = a.distill_alpha, a.distill_temperature
+        if isinstance(alpha, bool) or not isinstance(alpha, (int, float)) or not math.isfinite(alpha) or not 0.0 < alpha <= 1.0:
+            raise ValueError(f"distill_alpha must be a number in (0, 1], got {alpha!r}")
+        if isinstance(temp, bool) or not isinstance(temp, (int, float)) or not math.isfinite(temp) or not temp > 0.0:
+            raise ValueError(f"distill_temperature must be a finite number > 0, got {temp!r}")
+        from .models import NativeCausalLM
+        if not isinstance(self.model, NativeCausalLM):
+            raise ValueError(f"distillation needs a native student (LlamaForCausalLM / GPTForCausalLM): the loss is computed inside "
+                             f"their fused kernels, and {type(self.model).__name__} has no such loss")
+        if self.label_smoothing_factor or self.z_loss_weight:
+            raise ValueError("distillation cannot be combined with label_smoothing_factor > 0 or z_loss_weight > 0")
+        if teacher is self.model:
+            raise ValueError("the distillation teacher must be a separate model from the student")
+        self.model.distill_alpha, self.model.distill_temperature = float(alpha), float(temp)
+        return src
+
+    def _setup_teacher(self, src) -> Optional[nn.Module]:
+        """The frozen teacher on this rank's device in the student's weight dtype (a full copy per rank).  It is held by the trainer
+        only, never by the student, so its parameters stay out of the arena, ``parameters()`` and the checkpoints."""
+        if src is None:
+            return None
+        from .models import NativeCausalLM, from_pretrained
+        teacher = from_pretrained(str(src), device=self.device, dtype=self.param_dtype, native=True) if not isinstance(src, nn.Module) else src
+        if not isinstance(teacher, NativeCausalLM):
+            raise ValueError(f"the distillation teacher must be a native model (LlamaForCausalLM / GPTForCausalLM), got {type(teacher).__name__}")
+        if teacher.config.vocab_size != self.model.config.vocab_size or teacher.config.padded_vocab != self.model.config.padded_vocab:
+            raise ValueError(f"teacher and student vocabularies differ: {teacher.config.vocab_size} (padded {teacher.config.padded_vocab}) vs "
+                             f"{self.model.config.vocab_size} (padded {self.model.config.padded_vocab})")
+        teacher.to(device=self.device, dtype=self.param_dtype)
+        teacher.requires_grad_(False)
+        teacher.eval()
+        if self.rank == 0:
+            n = sum(p.numel() for p in teacher.parameters())
+            self.log.info(f">>> distillation from {type(teacher).__name__} ({n / 1e6:.1f}M parameters, one copy per rank): "
+                          f"alpha={self.model.distill_alpha}, temperature={self.model.distill_temperature} (eval stays pure cross-entropy)")
+        return teacher
+
     def prepare_data(self) -> None:
         """Per-rank sharding (`trainer_base.py:183-200`)."""
         self._check_packing()
@@ -588,10 +649,16 @@ class DecoupledTrainer:
         self.overlap = OverlapMeter(enabled=False)
 
     # ================================================================== step primitives
-    def _forward_loss(self, model: nn.Module, inputs: Dict[str, torch.Tensor]) -> torch.Tensor:
+    def _forward_loss(self, model: nn.Module, inputs: Dict[str, torch.Tensor], teacher: Optional[nn.Module] = None) -> torch.Tensor:
         if self.label_smoother is not None and "labels" in inputs:
             return self.compute_loss(model, dict(inputs))
-        if "labels" in inputs:
+        if teacher is not None:
+            # the teacher sees the same tokens and positions, so packed / document-masked rows are masked alike for both models
+            with torch.no_grad():
+                t_logits = teacher.padded_logits(inputs["input_ids"], inputs.get("position_ids"))
+            labels = inputs["labels"] if "labels" in inputs else inputs["input_ids"]
+            out = model(**{k: v for k, v in inputs.items() if k != "labels"}, labels=labels, teacher_logits=t_logits)
+        elif "labels" in inputs:
             out = model(**inputs)
         elif self._fused_smoothing:
             # a batch without labels is scored on its own tokens unsmoothed, as on the LabelSmoother route (it smooths labels only)
@@ -637,7 +704,7 @@ class DecoupledTrainer:
         model = model or self.model
         ctx = torch.autocast(device_type=self.device.type, dtype=self.dtype) if self.autocast else contextlib.nullcontext()
         with ctx:
-            loss = self._forward_loss(model, inputs)
+            loss = self._forward_loss(model, inputs) if self.teacher is None else self._forward_loss(model, inputs, self.teacher)
             scaled = loss / self.n_grad_acc_ddp if self.n_grad_acc_ddp != 1 else loss
         scaled.backward()
         return loss.detach()
@@ -798,12 +865,16 @@ class DecoupledTrainer:
             self.loss_host.copy_(self.loss_static, non_blocking=True)
             if self.z_loss_weight:
                 self.z_loss_host.copy_(self.z_loss_static, non_blocking=True)
+            if self.teacher is not None:
+                self.distill_host.copy_(self.distill_static, non_blocking=True)
             self.end_of_grad.record(self.grad_stream)
             self._poll_phase_end()
         else:
             self.loss_host.copy_(self.loss_static)
             if self.z_loss_weight:
                 self.z_loss_host.copy_(self.z_loss_static)
+            if self.teacher is not None:
+                self.distill_host.copy_(self.distill_static)
 
     def _poll_phase_end(self) -> None:
         """The flip decision must be taken when the *device* reaches the end of the phase ("if the com finished ... else accumulate
@@ -963,6 +1034,8 @@ class DecoupledTrainer:
             self.loss_host.copy_(self.loss_static)
             if self.z_loss_weight:
                 self.z_loss_host.copy_(self.z_loss_static)
+            if self.teacher is not None:
+                self.distill_host.copy_(self.distill_static)
             self._tail(None)
         return self._finish("_ddp")
 
@@ -1022,6 +1095,8 @@ class DecoupledTrainer:
                 gn = {} if self._grad_norm is None else {"grad_norm": self._grad_norm}
                 if self.z_loss_weight:
                     gn["z_loss"] = float(self.z_loss_host.item())    # the loss's z-term: cross-entropy = loss - z_loss
+                if self.teacher is not None:                          # loss = (1 - a) distill_ce + a T^2 distill_kl
+                    gn["distill_ce"], gn["distill_kl"] = (float(v) for v in self.distill_host.tolist())
                 log_training_scalars(self.writer, nb_step, sched.count_grad_tot, self.rank, loss, eval_loss, self.t_beg,
                                      extra={"lr": getattr(self, "_last_lr", 0.0), **gn})
                 self._fire("on_log", {"step": nb_step, "count_grad_tot": sched.count_grad_tot, "loss": loss,
@@ -1035,6 +1110,8 @@ class DecoupledTrainer:
                     gn_txt = "" if self._grad_norm is None else f" | grad_norm {self._grad_norm:.4g}"
                     if self.z_loss_weight:
                         gn_txt += f" | z_loss {gn['z_loss']:.4g}"
+                    if self.teacher is not None:
+                        gn_txt += f" | distill_ce {gn['distill_ce']:.4g} | distill_kl {gn['distill_kl']:.4g}"
                     pr.emit(sched.count_grad_tot, sched.count_com, loss, extra=f" | {rate:,.0f} tok/s/rank | lr {getattr(self, '_last_lr', 0.0):.3e}{gn_txt}")
                 self.epoch = pr.epoch
         if committed and plan is not None and self.callbacks:

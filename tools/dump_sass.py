@@ -56,6 +56,12 @@ KERNELS = {
     "ce_bwd_smooth.sass": "_ZN4acco13ce_bwd_kernelILb1ELb0EEEvP13__nv_bfloat16PKxPKfS6_iixfff",
     "ce_bwd_z.sass": "_ZN4acco13ce_bwd_kernelILb0ELb1EEEvP13__nv_bfloat16PKxPKfS6_iixfff",
     "ce_bwd_smooth_z.sass": "_ZN4acco13ce_bwd_kernelILb1ELb1EEEvP13__nv_bfloat16PKxPKfS6_iixfff",
+    # knowledge distillation <kT1> (train.distill_teacher): one pass over both rows forward, one more backward
+    "kd_fwd.sass": "_ZN4acco13kd_fwd_kernelILb0EEEvPK13__nv_bfloat16S3_PKxPfS6_xiixf",
+    "kd_fwd_t1.sass": "_ZN4acco13kd_fwd_kernelILb1EEEvPK13__nv_bfloat16S3_PKxPfS6_xiixf",
+    "kd_reduce.sass": "_ZN4acco16kd_reduce_kernelEPKfPKxPfS4_S4_xxff",
+    "kd_bwd.sass": "_ZN4acco13kd_bwd_kernelILb0EEEvP13__nv_bfloat16PKS1_PKxPKfS8_xiixfff",
+    "kd_bwd_t1.sass": "_ZN4acco13kd_bwd_kernelILb1EEEvP13__nv_bfloat16PKS1_PKxPKfS8_xiixfff",
 }
 MNEMONICS = ["HGMMA", "UTMALDG", "UTMALDG.2D.MULTICAST", "UTMASTG", "UTMACMDFLUSH", "SYNCS", "USETMAXREG", "REDG", "LDGMC", "HMMA", "MUFU.SQRT",
              "MUFU.EX2", "CCTL"]
