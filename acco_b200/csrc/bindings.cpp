@@ -30,6 +30,10 @@ int acco_kd_fwd(const void* student, const void* teacher, const long long* label
                 float* out, long long T, int V, int Vp, long long ignore_index, float alpha, float temperature, cudaStream_t st);
 int acco_kd_bwd(void* student, const void* teacher, const long long* labels, const float* lse3, const float* scale, long long T, int V, int Vp,
                 long long ignore_index, float alpha, float temperature, cudaStream_t st);
+int acco_dpo_fwd(const void* policy, const void* ref, const long long* labels, float* lse, float* d, float* rowbuf, float* w, float* loss,
+                 float* out, int P, int S, int V, int Vp, long long ignore_index, float beta, cudaStream_t st);
+int acco_dpo_bwd(void* policy, const long long* labels, const float* lse, const float* w, const float* dloss, int P, int S, int V, int Vp,
+                 long long ignore_index, cudaStream_t st);
 int acco_norm_bwd_acc_f32(const void* dy, const void* dh_extra, const void* h, const void* w, const float* mean, const float* rstd, void* dh,
                           float* partial, float* dw_accum, float* db_accum, int T, int H, int grid, cudaStream_t st);
 int acco_embedding_bwd(void* grad, const long long* sorted, const long long* perm, const void* dy, int T, int H, int sms, cudaStream_t st);
@@ -385,6 +389,56 @@ void kd_bwd_inplace(torch::Tensor logits, torch::Tensor teacher_logits, torch::T
     TORCH_CHECK(acco_kd_bwd(logits.data_ptr(), teacher_logits.data_ptr(), (const long long*)labels.data_ptr<int64_t>(), lse3.data_ptr<float>(),
                             scale.data_ptr<float>(), T, (int)V, (int)Vp, ignore_index, (float)alpha, (float)temperature, stream()) == 0,
                 "kd_bwd: bad arguments");
+}
+
+// ---------------------------------------------------------------- DPO
+// logits / ref_logits [2 P S, Vp] bf16, labels [2 P S] int64 (shifted, -100 = not a response token); returns S.
+int64_t check_dpo(const torch::Tensor& s, const torch::Tensor& labels, int64_t P, int64_t V) {
+    check_bf16(s, "logits");
+    TORCH_CHECK(s.dim() == 2 && s.size(1) % 8 == 0 && V > 0 && V <= s.size(1), "dpo: logits must be [T, Vp] with Vp a multiple of 8 and >= V, "
+                "got ", s.sizes(), " and V=", V);
+    TORCH_CHECK(labels.is_cuda() && labels.device() == s.device() && labels.scalar_type() == torch::kInt64 && labels.is_contiguous() &&
+                labels.numel() == s.size(0), "labels must be contiguous CUDA int64 with one entry per row");
+    TORCH_CHECK(P > 0 && s.size(0) % (2 * P) == 0 && s.size(0) / (2 * P) <= INT32_MAX && P <= INT32_MAX,
+                "dpo: the rows must be 2 P S token rows, got ", s.size(0), " for P=", P);
+    return s.size(0) / (2 * P);
+}
+
+// Returns (loss, lse [T], w [2P]); `out` (three fp32 on the logits' device) receives the mean chosen reward, the mean rejected reward
+// and the accuracy over the valid pairs.
+std::vector<torch::Tensor> dpo_fwd(torch::Tensor logits, torch::Tensor ref_logits, torch::Tensor labels, int64_t P, int64_t V,
+                                   int64_t ignore_index, double beta, torch::Tensor out) {
+    const int64_t S = check_dpo(logits, labels, P, V);
+    check_bf16(ref_logits, "ref_logits");
+    TORCH_CHECK(ref_logits.sizes() == logits.sizes() && ref_logits.device() == logits.device(), "ref_logits must match the policy logits' "
+                "[T, Vp] shape and device, got ", ref_logits.sizes(), " vs ", logits.sizes());
+    TORCH_CHECK(std::isfinite(beta) && beta > 0.0 && std::isfinite((float)beta) && (float)beta > 0.f, "beta must be finite and > 0, got ", beta);
+    TORCH_CHECK(out.is_cuda() && out.device() == logits.device() && out.scalar_type() == torch::kFloat32 && out.numel() == 3 && out.is_contiguous(),
+                "out must be a contiguous three-element fp32 tensor on the logits' device");
+    const c10::cuda::CUDAGuard guard(logits.device());
+    const int64_t T = logits.size(0), Vp = logits.size(1);
+    auto f32 = logits.options().dtype(torch::kFloat32);
+    auto lse = torch::empty({T}, f32);
+    auto d = torch::empty({T}, f32);
+    auto rowbuf = torch::empty({4 * P}, f32);
+    auto w = torch::empty({2 * P}, f32);
+    auto loss = torch::empty({}, f32);
+    TORCH_CHECK(acco_dpo_fwd(logits.data_ptr(), ref_logits.data_ptr(), (const long long*)labels.data_ptr<int64_t>(), lse.data_ptr<float>(),
+                             d.data_ptr<float>(), rowbuf.data_ptr<float>(), w.data_ptr<float>(), loss.data_ptr<float>(), out.data_ptr<float>(),
+                             (int)P, (int)S, (int)V, (int)Vp, ignore_index, (float)beta, stream()) == 0, "dpo_fwd: bad arguments");
+    return {loss, lse, w};
+}
+
+// In place: logits <- dloss w[row] (softmax - onehot) on the response tokens' valid columns, 0 elsewhere.
+void dpo_bwd_inplace(torch::Tensor logits, torch::Tensor labels, torch::Tensor lse, torch::Tensor w, torch::Tensor dloss, int64_t P, int64_t V,
+                     int64_t ignore_index) {
+    const int64_t S = check_dpo(logits, labels, P, V);
+    check_f32(lse, "lse"); check_f32(w, "w"); check_f32(dloss, "dloss");
+    TORCH_CHECK(lse.numel() == logits.size(0) && w.numel() == 2 * P && dloss.numel() == 1, "lse must hold T values, w 2P and dloss one");
+    const c10::cuda::CUDAGuard guard(logits.device());
+    TORCH_CHECK(acco_dpo_bwd(logits.data_ptr(), (const long long*)labels.data_ptr<int64_t>(), lse.data_ptr<float>(), w.data_ptr<float>(),
+                             dloss.data_ptr<float>(), (int)P, (int)S, (int)V, (int)logits.size(1), ignore_index, stream()) == 0,
+                "dpo_bwd: bad arguments");
 }
 
 // ---------------------------------------------------------------- fused round kernel
@@ -845,6 +899,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("ignore_index"), py::arg("label_smoothing") = 0.0, py::arg("z_loss") = 0.0);
     m.def("kd_fwd", &kd_fwd, py::arg("logits"), py::arg("teacher_logits"), py::arg("labels"), py::arg("V"), py::arg("ignore_index"),
           py::arg("alpha"), py::arg("temperature"), py::arg("out"));
+    m.def("dpo_fwd", &dpo_fwd, py::arg("logits"), py::arg("ref_logits"), py::arg("labels"), py::arg("P"), py::arg("V"), py::arg("ignore_index"),
+          py::arg("beta"), py::arg("out"));
+    m.def("dpo_bwd_inplace", &dpo_bwd_inplace, py::arg("logits"), py::arg("labels"), py::arg("lse"), py::arg("w"), py::arg("dloss"), py::arg("P"),
+          py::arg("V"), py::arg("ignore_index"));
     m.def("kd_bwd_inplace", &kd_bwd_inplace, py::arg("logits"), py::arg("teacher_logits"), py::arg("labels"), py::arg("lse3"), py::arg("scale"),
           py::arg("V"), py::arg("ignore_index"), py::arg("alpha"), py::arg("temperature"));
     m.def("adamw_shard", &adamw_shard, py::arg("grad_sum"), py::arg("master"), py::arg("exp_avg"), py::arg("exp_avg_sq"), py::arg("stash"),

@@ -30,6 +30,16 @@
 //            Stores lse(s), lse(s/T), lse(t/T) [3, T] and the row's CE and KL [2, T].  kT1 (T == 1) shares the first two.
 //   kd_reduce : ce_reduce's order -> objective, inv_n, and out[2] = (mean CE, mean KL) over the non-ignored rows.
 //   kd_bwd : in place on s, reading t once more.
+//
+// DPO (dpo_*, separate kernels).  Policy logits s and frozen reference logits r, both bf16 [2P S, Vp]: rows [0, P) of the
+// [2P, S] token layout are the chosen responses, rows [P, 2P) the rejected ones, pair i = (i, P + i); R(row) = its non-ignored
+// positions.  l(row) = sum_{t in R(row)} (s_t[y_t] - lse(s_t)), l_ref the same over r;
+//   z_i = beta [(l(c_i) - l_ref(c_i)) - (l(r_i) - l_ref(r_i))],  loss = mean over valid pairs (both rows non-empty) of softplus(-z_i),
+//   d s_tc = dloss (+-beta sigma(-z_i) / n) (softmax(s_t)_c - [c = y_t])   (+ chosen, - rejected; padding, ignored, invalid: 0).
+//   dpo_fwd : one CTA per token row, ONE streaming pass over both rows -> lse(s_t) and d_t = (s_t[y] - lse(s_t)) - (r_t[y] - lse(r_t)).
+//             Subtracting per token keeps the cancellation out of the long fp32 sums and makes d == 0 exact for s == r.
+//   dpo_reduce : one CTA, fixed order: row sums of d, z, the loss, the per-row weight w and three logged means.
+//   dpo_bwd : in place on s, like ce_bwd with the scale dloss * w[row].
 #include "common.cuh"
 
 namespace acco {
@@ -380,6 +390,142 @@ bool kd_args_ok(int V, int Vp, float alpha, float temperature) {
     return Vp % 8 == 0 && V > 0 && V <= Vp && alpha > 0.f && alpha <= 1.f && temperature > 0.f && temperature < INFINITY;
 }
 
+// ---------------------------------------------------------------- DPO
+// d [T]: per token (s[y] - lse(s)) - (r[y] - lse(r)), lse [T]: lse(s); both 0 on ignored rows.  The two log-probabilities are
+// formed by the same instructions, so d == 0 exactly when s and r are bitwise equal.
+__global__ void __launch_bounds__(kCEThreads) dpo_fwd_kernel(const __nv_bfloat16* __restrict__ policy, const __nv_bfloat16* __restrict__ ref,
+                                                             const long long* __restrict__ labels, float* __restrict__ lse_out,
+                                                             float* __restrict__ d_out, int V, int Vp, long long ignore_index) {
+    __shared__ float red[32];
+    const long long row = blockIdx.x;
+    const __nv_bfloat16* x = policy + row * (size_t)Vp;
+    const __nv_bfloat16* y = ref + row * (size_t)Vp;
+    const long long label = labels[row];
+    if (label == ignore_index) {
+        if (threadIdx.x == 0) lse_out[row] = d_out[row] = 0.f;
+        return;
+    }
+    const int nvec_full = V >> 3;
+    float m1 = -INFINITY, s1 = 0.f, m2 = -INFINITY, s2 = 0.f;
+    for (int v = threadIdx.x; v < nvec_full; v += kCEThreads) {
+        float f[8], g[8];
+        unpack8(ld_stream(x + 8 * v), f);
+        unpack8(ld_stream(y + 8 * v), g);
+        online8(f, m1, s1);
+        online8(g, m2, s2);
+    }
+    for (int c = (nvec_full << 3) + threadIdx.x; c < V; c += kCEThreads) {
+        const float f = __bfloat162float(x[c]), g = __bfloat162float(y[c]);
+        float nm = fmaxf(m1, f);
+        s1 = s1 * __expf(m1 - nm) + __expf(f - nm);
+        m1 = nm;
+        nm = fmaxf(m2, g);
+        s2 = s2 * __expf(m2 - nm) + __expf(g - nm);
+        m2 = nm;
+    }
+    const float lse1 = block_lse(m1, s1, red);
+    const float lse2 = block_lse(m2, s2, red);
+    if (threadIdx.x == 0) {
+        lse_out[row] = lse1;
+        d_out[row] = (__bfloat162float(x[label]) - lse1) - (__bfloat162float(y[label]) - lse2);
+    }
+}
+
+// One CTA of 1024 threads, fixed order (two launches are bitwise equal).  Rows are [2P, S] token rows: pair i is (i, P + i).
+//   rowbuf [2, 2P]: per row sum of d and count of non-ignored tokens (warp w sums rows w, w + 32, ...).
+//   z_i = beta (D[i] - D[P + i]); a pair is valid when both rows have a token; n = #valid.
+//   loss = sum_valid softplus(-z_i) / n;  w[i] = beta sigma(-z_i) / n = -w[P + i] (0 for invalid pairs);
+//   out = (mean beta D[i], mean beta D[P + i], mean [z_i > 0]) over the valid pairs.  n = 0: all 0.
+__global__ void __launch_bounds__(1024) dpo_reduce_kernel(const float* __restrict__ d, const long long* __restrict__ labels,
+                                                          float* __restrict__ rowbuf, float* __restrict__ w, float* __restrict__ loss,
+                                                          float* __restrict__ out, int P, int S, long long ignore_index, float beta) {
+    __shared__ float red[32];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    const int R = 2 * P;
+    for (int r = wid; r < R; r += nw) {
+        float sd = 0.f, cnt = 0.f;
+        for (int t = lane; t < S; t += 32) {
+            const long long i = (long long)r * S + t;
+            if (labels[i] != ignore_index) {
+                sd += d[i];
+                cnt += 1.f;
+            }
+        }
+        sd = warp_sum(sd);
+        cnt = warp_sum(cnt);
+        if (lane == 0) {
+            rowbuf[r] = sd;
+            rowbuf[R + r] = cnt;
+        }
+    }
+    __syncthreads();
+    float n = 0.f, sl = 0.f, sc = 0.f, sr = 0.f, sa = 0.f;
+    for (int i = threadIdx.x; i < P; i += blockDim.x) {
+        if (rowbuf[R + i] > 0.f && rowbuf[R + P + i] > 0.f) {
+            const float rc = __fmul_rn(beta, rowbuf[i]), rr = __fmul_rn(beta, rowbuf[P + i]), z = __fsub_rn(rc, rr);
+            n += 1.f;
+            sl += fmaxf(-z, 0.f) + log1pf(__expf(-fabsf(z)));      // softplus(-z), stable for any |z|
+            sc += rc;
+            sr += rr;
+            sa += z > 0.f ? 1.f : 0.f;
+        }
+    }
+    n = block_sum(n, red);
+    sl = block_sum(sl, red);
+    sc = block_sum(sc, red);
+    sr = block_sum(sr, red);
+    sa = block_sum(sa, red);
+    const float inv = n > 0.f ? 1.f / n : 0.f;
+    for (int i = threadIdx.x; i < P; i += blockDim.x) {
+        float c = 0.f;
+        if (rowbuf[R + i] > 0.f && rowbuf[R + P + i] > 0.f) {
+            const float z = __fsub_rn(__fmul_rn(beta, rowbuf[i]), __fmul_rn(beta, rowbuf[P + i]));   // as above
+            const float e = __expf(-fabsf(z));
+            c = beta * (z >= 0.f ? e / (1.f + e) : 1.f / (1.f + e)) * inv;    // beta sigma(-z) / n
+        }
+        w[i] = c;
+        w[P + i] = -c;
+    }
+    if (threadIdx.x == 0) {
+        *loss = sl * inv;
+        out[0] = sc * inv;
+        out[1] = sr * inv;
+        out[2] = sa * inv;
+    }
+}
+
+// In place on the policy logits: dloss w[row / S] (softmax - onehot) on non-ignored rows and valid columns, else 0.
+__global__ void __launch_bounds__(kCEThreads) dpo_bwd_kernel(__nv_bfloat16* __restrict__ logits, const long long* __restrict__ labels,
+                                                             const float* __restrict__ lse_in, const float* __restrict__ w,
+                                                             const float* __restrict__ dloss, int S, int V, int Vp, long long ignore_index) {
+    const long long row = blockIdx.x;
+    __nv_bfloat16* x = logits + row * (size_t)Vp;
+    const long long label = labels[row];
+    const int nvec = Vp >> 3;
+    if (label == ignore_index) {
+        bf16x8 z;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) z.v[i] = __floats2bfloat162_rn(0.f, 0.f);
+        for (int v = threadIdx.x; v < nvec; v += kCEThreads) st_stream(x + 8 * v, z);
+        return;
+    }
+    const float lse = lse_in[row];
+    const float scale = *dloss * w[row / S];
+    for (int v = threadIdx.x; v < nvec; v += kCEThreads) {
+        float f[8];
+        unpack8(ld_stream_rw(x + 8 * v), f);
+        const int c0 = 8 * v;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int c = c0 + j;
+            float p = (c < V) ? __expf(f[j] - lse) : 0.f;
+            if (c == label) p -= 1.f;
+            f[j] = p * scale;
+        }
+        st_stream(x + 8 * v, pack8(f));
+    }
+}
+
 }  // namespace acco
 
 // `label_smoothing` in [0, 1] and `z_loss` >= 0 (checked by the binding); 0 runs the instantiation without the term.  With
@@ -426,5 +572,25 @@ extern "C" int acco_kd_bwd(void* student, const void* teacher, const long long* 
     auto k = temperature == 1.f ? acco::kd_bwd_kernel<true> : acco::kd_bwd_kernel<false>;
     k<<<(unsigned)T, acco::kCEThreads, 0, st>>>((__nv_bfloat16*)student, (const __nv_bfloat16*)teacher, labels, lse3, scale, T, V, Vp,
                                                 ignore_index, one_m_a, a_t, inv_t);
+    return 0;
+}
+
+// DPO over T = 2 P S token rows (pair i = rows [i S, (i+1) S) and [(P+i) S, (P+i+1) S)): finite beta > 0, P, S > 0, Vp % 8 == 0 and
+// V <= Vp, else -1 (nothing launched).  Writes lse, d [T], rowbuf [4P], w [2P], the loss and `out` (three fp32).
+extern "C" int acco_dpo_fwd(const void* policy, const void* ref, const long long* labels, float* lse, float* d, float* rowbuf, float* w,
+                            float* loss, float* out, int P, int S, int V, int Vp, long long ignore_index, float beta, cudaStream_t st) {
+    if (Vp % 8 != 0 || V <= 0 || V > Vp || P <= 0 || S <= 0 || !(beta > 0.f && beta < INFINITY) || out == nullptr) return -1;
+    const long long T = 2LL * P * S;
+    acco::dpo_fwd_kernel<<<(unsigned)T, acco::kCEThreads, 0, st>>>((const __nv_bfloat16*)policy, (const __nv_bfloat16*)ref, labels, lse, d, V,
+                                                                   Vp, ignore_index);
+    acco::dpo_reduce_kernel<<<1, 1024, 0, st>>>(d, labels, rowbuf, w, loss, out, P, S, ignore_index, beta);
+    return 0;
+}
+
+extern "C" int acco_dpo_bwd(void* policy, const long long* labels, const float* lse, const float* w, const float* dloss, int P, int S, int V,
+                            int Vp, long long ignore_index, cudaStream_t st) {
+    if (Vp % 8 != 0 || V <= 0 || V > Vp || P <= 0 || S <= 0) return -1;
+    acco::dpo_bwd_kernel<<<(unsigned)(2LL * P * S), acco::kCEThreads, 0, st>>>((__nv_bfloat16*)policy, labels, lse, w, dloss, S, V, Vp,
+                                                                               ignore_index);
     return 0;
 }

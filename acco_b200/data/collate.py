@@ -11,6 +11,8 @@
   (the models derive document masking from them) and labels that train exactly the (context, target) pairs of ``PadCollator``.
 * :class:`DocumentCollator` - const-len pre-training rows with document masking (``document_mask: True``): the same three
   ``[B, S]`` tensors as ``PackedCollator``, with the documents found from the EOS tokens ``pack_const_len`` closed them with.
+* :class:`PreferenceCollator` - DPO preference pairs (``prompt_ids`` / ``chosen_ids`` / ``rejected_ids``): ``[2P, S]`` rows, the
+  ``P`` chosen responses first, labels only on the response tokens.
 """
 from __future__ import annotations
 
@@ -19,7 +21,9 @@ from typing import Any, Dict, Sequence
 import numpy as np
 import torch
 
-__all__ = ["stack_collate", "PadCollator", "PackedCollator", "DocumentCollator"]
+__all__ = ["stack_collate", "PadCollator", "PackedCollator", "DocumentCollator", "PreferenceCollator", "PREFERENCE_COLUMNS"]
+
+PREFERENCE_COLUMNS = ("prompt_ids", "chosen_ids", "rejected_ids")
 
 
 def stack_collate(batch: Sequence[Dict[str, Any]]) -> Dict[str, torch.Tensor]:
@@ -119,3 +123,33 @@ class DocumentCollator:
         labels = ids.copy()
         labels[(start == s) & (s > 0)] = self.label_pad
         return {"input_ids": torch.from_numpy(ids), "labels": torch.from_numpy(labels), "position_ids": torch.from_numpy(s - start)}
+
+
+class PreferenceCollator:
+    """``P`` preference pairs (token lists ``prompt_ids``, ``chosen_ids``, ``rejected_ids``) -> ``input_ids``, ``attention_mask``,
+    ``labels``, each ``[2P, S]`` int64: row ``i`` is ``prompt + chosen`` of pair ``i``, row ``P + i`` is ``prompt + rejected``, each cut
+    at ``max_length`` from the right.  ``S`` is the longest row rounded up to ``pad_to_multiple_of`` (as ``PadCollator``, so CUDA
+    graphs replay).  ``labels`` equal the response tokens and are -100 on the prompt and the padding; a row whose response was cut
+    away has no label, and its pair then counts as invalid in the DPO loss."""
+
+    def __init__(self, pad_token_id: int, max_length: int, pad_to_multiple_of: int = 1, label_pad: int = -100):
+        self.pad, self.L, self.label_pad = int(pad_token_id), int(max_length), int(label_pad)
+        self.mult = max(int(pad_to_multiple_of), 1)
+
+    def __call__(self, batch: Sequence[Dict[str, Any]]) -> Dict[str, torch.Tensor]:
+        rows, starts = [], []
+        for key in ("chosen_ids", "rejected_ids"):
+            for b in batch:
+                prompt = list(b["prompt_ids"])
+                rows.append((prompt + list(b[key]))[: self.L])
+                starts.append(len(prompt))
+        S = max(max(len(r) for r in rows), 1)
+        S = ((S + self.mult - 1) // self.mult) * self.mult
+        ids = np.full((len(rows), S), self.pad, dtype=np.int64)
+        mask = np.zeros((len(rows), S), dtype=np.int64)
+        labels = np.full((len(rows), S), self.label_pad, dtype=np.int64)
+        for i, (r, a) in enumerate(zip(rows, starts)):
+            ids[i, : len(r)] = r
+            mask[i, : len(r)] = 1
+            labels[i, a: len(r)] = r[a:]
+        return {"input_ids": torch.from_numpy(ids), "attention_mask": torch.from_numpy(mask), "labels": torch.from_numpy(labels)}

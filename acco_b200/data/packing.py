@@ -103,3 +103,18 @@ def make_packed_tokenize_fn(tokenizer, text_column: str, max_length: int):
         ids = tokenizer(batch[text_column], truncation=True, max_length=max_length)["input_ids"]
         return pack_sft(ids, max_length)
     return fn
+
+
+def make_preference_tokenize_fn(tokenizer):
+    """Batched ``datasets.map`` function: TRL's ``prompt`` / ``chosen`` / ``rejected`` text columns -> ``prompt_ids``, ``chosen_ids``,
+    ``rejected_ids`` token lists, each response closed by the tokenizer's EOS when it has one.  ``PreferenceCollator`` joins the
+    prompt and each response and cuts the row at ``max_length``."""
+    eos = getattr(tokenizer, "eos_token_id", None)
+    tail = [] if eos is None else [int(eos)]
+
+    def fn(batch: Dict[str, Any]) -> Dict[str, Any]:
+        out = {"prompt_ids": tokenizer(batch["prompt"])["input_ids"]}
+        for key in ("chosen", "rejected"):
+            out[f"{key}_ids"] = [list(r) + tail for r in tokenizer(batch[key], add_special_tokens=False)["input_ids"]]
+        return out
+    return fn

@@ -20,8 +20,8 @@ import torch
 from .dataset import TokenDataset
 from .packing import pack_const_len
 
-__all__ = ["synthetic_documents", "synthetic_pretrain_dataset", "synthetic_sft_dataset", "synthetic_text_dataset",
-           "synthetic_token_batches"]
+__all__ = ["synthetic_documents", "synthetic_pretrain_dataset", "synthetic_preference_dataset", "synthetic_sft_dataset",
+           "synthetic_text_dataset", "synthetic_token_batches"]
 
 
 def _markov_tokens(rng: np.random.Generator, n: int, vocab: int, reserved_top: int = 1) -> np.ndarray:
@@ -72,6 +72,23 @@ def synthetic_sft_dataset(n_rows: int, mean_len: int, vocab_size: int, max_lengt
     pads with EOS like the reference."""
     docs = synthetic_documents(n_rows, mean_len, vocab_size, seed, min_len=4, max_len=max_length)
     return TokenDataset({"input_ids": [d[:max_length].tolist() for d in docs]})
+
+
+def synthetic_preference_dataset(n_pairs: int, mean_len: int, vocab_size: int, seed: int = 0) -> TokenDataset:
+    """DPO pairs (columns ``prompt_ids``, ``chosen_ids``, ``rejected_ids``).  The chosen response continues the prompt's Markov source
+    (the successor map ``x -> 31 x + 7`` of :func:`_markov_tokens`); the rejected one comes from another source (uniform tokens), so a
+    model can learn to prefer the chosen response and the DPO accuracy can rise.  Prompts and responses each average ``mean_len / 2``
+    tokens."""
+    rng = np.random.default_rng(seed)
+    half = max(mean_len // 2, 2)
+    prompts, chosen, rejected = [], [], []
+    for _ in range(n_pairs):
+        lp, lc, lr = (int(v) for v in rng.integers(max(half // 2, 1), half + half // 2 + 1, size=3))
+        doc = _markov_tokens(rng, lp + lc, vocab_size)
+        prompts.append(doc[:lp].tolist())
+        chosen.append(doc[lp:].tolist())
+        rejected.append(rng.integers(0, max(vocab_size - 1, 2), size=lr).tolist())
+    return TokenDataset({"prompt_ids": prompts, "chosen_ids": chosen, "rejected_ids": rejected})
 
 
 def synthetic_text_dataset(n_docs: int, mean_words: int, seed: int = 0) -> TokenDataset:

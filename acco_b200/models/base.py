@@ -59,6 +59,10 @@ class NativeCausalLM(nn.Module):
         self.distill_alpha = 0.5
         self.distill_temperature = 1.0
         self.distill_out: Optional[torch.Tensor] = None
+        # DPO (train key `dpo_beta`): beta of a forward given reference_logits, and three fp32 on the device that receive each such
+        # loss's mean chosen reward, mean rejected reward and accuracy (ops.dpo_loss)
+        self.dpo_beta = 0.1
+        self.dpo_out: Optional[torch.Tensor] = None
 
     @property
     def embed_weight(self) -> torch.Tensor:
@@ -90,14 +94,18 @@ class NativeCausalLM(nn.Module):
 
     # ------------------------------------------------------------------ loss
     def _lm_output(self, logits: torch.Tensor, labels: Optional[torch.Tensor], B: int, S: int,
-                   teacher_logits: Optional[torch.Tensor] = None) -> CausalLMOutput:
+                   teacher_logits: Optional[torch.Tensor] = None, reference_logits: Optional[torch.Tensor] = None) -> CausalLMOutput:
         """Logits ``[B*S, Vp]`` -> the logits cut to ``vocab_size`` without labels, else the mean cross-entropy loss, or with
-        ``teacher_logits`` (a teacher's :meth:`padded_logits` on the same tokens) the distillation objective, over the same rows."""
+        ``teacher_logits`` (a teacher's :meth:`padded_logits` on the same tokens) the distillation objective, over the same rows.
+        With ``reference_logits`` (a frozen reference's :meth:`padded_logits`) the ``B = 2P`` rows are ``P`` preference pairs, chosen
+        rows first, and the loss is the DPO objective over the response tokens the labels keep (``ops.dpo_loss``)."""
         V = self.config.vocab_size
         if labels is None:
-            if teacher_logits is not None:
-                raise ValueError("teacher_logits needs labels: the distillation loss is taken over the rows the labels keep")
+            if teacher_logits is not None or reference_logits is not None:
+                raise ValueError("teacher_logits / reference_logits need labels: the loss is taken over the rows the labels keep")
             return CausalLMOutput(loss=None, logits=logits.view(B, S, -1)[..., :V])
+        if teacher_logits is not None and reference_logits is not None:
+            raise ValueError("give teacher_logits (distillation) or reference_logits (DPO), not both")
         # HF shift: position t predicts token t+1; the last position has no target
         shifted = torch.full_like(labels, -100)
         shifted[:, :-1] = labels[:, 1:]
@@ -106,6 +114,13 @@ class NativeCausalLM(nn.Module):
                 raise ValueError("distillation cannot be combined with label smoothing or the z-loss")
             loss = ops.distill_cross_entropy(logits, teacher_logits, shifted.reshape(B * S), V, self.distill_alpha,
                                              self.distill_temperature, out=self.distill_out)
+            return CausalLMOutput(loss=loss, logits=None)
+        if reference_logits is not None:
+            if self.label_smoothing or self.z_loss_weight:
+                raise ValueError("DPO cannot be combined with label smoothing or the z-loss")
+            if B % 2:
+                raise ValueError(f"DPO needs an even number of rows (P chosen, then P rejected), got {B}")
+            loss = ops.dpo_loss(logits, reference_logits, shifted.reshape(B * S), B // 2, V, self.dpo_beta, out=self.dpo_out)
             return CausalLMOutput(loss=loss, logits=None)
         loss = ops.softmax_cross_entropy(logits, shifted.reshape(B * S), V, -100, label_smoothing=self.label_smoothing,
                                          z_loss=self.z_loss_weight, z_loss_out=self.z_loss_out)

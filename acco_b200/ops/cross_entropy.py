@@ -28,7 +28,21 @@ temperature ``T > 0`` and weight ``a`` in (0, 1] (Hinton's forward KL, teacher e
     d s_rc = scale ((1 - a) (softmax(s_r)_c - [c = y_r]) + a T (softmax(s_r / T)_c - softmax(t_r / T)_c))      (c < V; else 0)
 
 The kernels make one streaming pass over both rows forward and one more backward (in place on ``s``), with no fp32 copy of
-either; ``out`` (two fp32) receives the mean CE and the mean KL on the device.  The teacher logits are read, never written."""
+either; ``out`` (two fp32) receives the mean CE and the mean KL on the device.  The teacher logits are read, never written.
+
+:func:`dpo_loss` is DPO (Rafailov et al. 2023) against a frozen reference's logits ``r`` (same padded layout).  The ``2P S`` rows are
+``[2P, S]`` token rows: rows ``0..P-1`` the chosen responses, ``P..2P-1`` the rejected ones, pair ``i`` = rows ``(i, P+i)``; ``R(row)``
+its positions whose (shifted) label is not -100::
+
+    l(row) = sum_{t in R(row)} (s_t[y_t] - lse(s_t)),   l_ref(row) the same over r
+    z_i    = beta ((l(c_i) - l_ref(c_i)) - (l(r_i) - l_ref(r_i)))
+    loss   = (1/n) sum over valid pairs (both rows have a response token) of softplus(-z_i)        (n = 0: loss 0, gradient 0)
+    d s_tc = +-(beta sigma(-z_i) / n) (softmax(s_t)_c - [c = y_t])       (+ chosen, - rejected; c < V; else 0)
+
+The forward makes one streaming pass over both rows and takes the per-token difference of the two log-probabilities before any
+sum, so equal policy and reference logits give ``z = 0`` exactly; a one-CTA reduction forms the loss and the per-row weights, and
+the backward writes the gradient in place over ``s``.  ``out`` (three fp32) receives the mean chosen reward ``beta (l - l_ref)(c)``,
+the mean rejected reward and the accuracy (fraction of valid pairs with ``z > 0``) on the device."""
 from __future__ import annotations
 
 import math
@@ -166,3 +180,78 @@ def distill_cross_entropy(logits: torch.Tensor, teacher_logits: torch.Tensor, la
     if use_kernels(logits, teacher_logits) and logits.dtype == torch.bfloat16:
         return _KDFn.apply(logits, teacher_logits.detach(), labels, int(V), alpha, temperature, out)
     return distill_cross_entropy_ref(logits, teacher_logits, labels, V, alpha, temperature, out)
+
+
+# ------------------------------------------------------------------------------------------------ DPO
+def dpo_loss_ref(logits: torch.Tensor, ref_logits: torch.Tensor, labels: torch.Tensor, P: int, valid_vocab: int, beta: float,
+                 out: Optional[torch.Tensor] = None, ignore_index: int = -100) -> torch.Tensor:
+    """fp32 reference of :func:`dpo_loss` (the CPU and non-bf16 path)."""
+    V, P = int(valid_vocab), int(P)
+    x = logits[..., :V].float().reshape(-1, V)
+    r = ref_logits[..., :V].detach().float().reshape(-1, V)
+    lb = labels.reshape(-1)
+    mask = lb != ignore_index
+    idx = torch.where(mask, lb, torch.zeros_like(lb))[:, None]
+    d = torch.log_softmax(x, -1).gather(1, idx)[:, 0] - torch.log_softmax(r, -1).gather(1, idx)[:, 0]
+    D = torch.where(mask, d, torch.zeros_like(d)).view(2 * P, -1).sum(1)
+    cnt = mask.view(2 * P, -1).sum(1)
+    valid = (cnt[:P] > 0) & (cnt[P:] > 0)
+    n = valid.sum().clamp(min=1)
+    rc, rr = beta * D[:P], beta * D[P:]
+    z = rc - rr
+    loss = torch.where(valid, F.softplus(-z), torch.zeros_like(z)).sum() / n
+    if out is not None:
+        zero = torch.zeros_like(z)
+        vals = [torch.where(valid, v, zero).sum() / n for v in (rc.detach(), rr.detach(), (z.detach() > 0).float())]
+        out.copy_(torch.stack(vals).reshape(out.shape))
+    return loss
+
+
+def _check_dpo(beta: float, out: Optional[torch.Tensor]) -> None:
+    if isinstance(beta, bool) or not (math.isfinite(beta) and beta > 0.0):
+        raise ValueError(f"beta must be finite and > 0, got {beta!r}")
+    if out is not None and (out.numel() != 3 or out.dtype != torch.float32):
+        raise ValueError("out must be a three-element fp32 tensor")
+
+
+class _DPOFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, logits, ref_logits, labels, P, valid_vocab, beta, out):
+        C = load_ext(required=True)
+        lg = logits.reshape(-1, logits.shape[-1])
+        rl = ref_logits.reshape(-1, ref_logits.shape[-1])
+        assert lg.is_contiguous() and rl.is_contiguous()
+        lb = labels.reshape(-1).contiguous()
+        if out is None:
+            out = torch.empty(3, device=lg.device, dtype=torch.float32)
+        loss, lse, w = C.dpo_fwd(lg, rl, lb, int(P), int(valid_vocab), -100, float(beta), out)
+        count_launch("dpo_fwd", 2)
+        ctx.save_for_backward(lg, lb, lse, w)
+        ctx.P, ctx.valid_vocab, ctx.shape = int(P), int(valid_vocab), logits.shape
+        return loss
+
+    @staticmethod
+    def backward(ctx, dloss):
+        C = load_ext(required=True)
+        lg, lb, lse, w = ctx.saved_tensors
+        C.dpo_bwd_inplace(lg, lb, lse, w, dloss.float().reshape(1).contiguous(), ctx.P, ctx.valid_vocab, -100)
+        count_launch("dpo_bwd")
+        return lg.view(ctx.shape), None, None, None, None, None, None
+
+
+def dpo_loss(logits: torch.Tensor, ref_logits: torch.Tensor, labels: torch.Tensor, P: int, V: int, beta: float,
+             out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The DPO objective of ``P`` preference pairs laid out as ``2P`` rows of ``S`` tokens (chosen rows first); ``labels`` are the
+    shifted labels of the ``2P S`` rows, -100 off the responses.  ``out`` (three fp32), when given, receives the mean chosen reward,
+    the mean rejected reward and the accuracy.  The reference gets no gradient.
+    NOTE (kernel path): ``logits`` is consumed - its storage is reused for the gradient during backward."""
+    _check_dpo(beta, out)
+    beta, P = float(beta), int(P)
+    if ref_logits.shape != logits.shape:
+        raise ValueError(f"ref_logits {tuple(ref_logits.shape)} must match the policy logits {tuple(logits.shape)}")
+    rows = logits.reshape(-1, logits.shape[-1]).shape[0]
+    if P <= 0 or rows % (2 * P) != 0 or labels.numel() != rows:
+        raise ValueError(f"dpo_loss needs 2 P S rows and one label per row, got {rows} rows, {labels.numel()} labels and P={P}")
+    if use_kernels(logits, ref_logits) and logits.dtype == torch.bfloat16:
+        return _DPOFn.apply(logits, ref_logits.detach(), labels, P, int(V), beta, out)
+    return dpo_loss_ref(logits, ref_logits, labels, P, V, beta, out)

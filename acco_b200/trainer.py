@@ -36,8 +36,9 @@ import torch.distributed as dist
 import torch.nn as nn
 
 from .config import to_container
-from .data import (BatchLoader, DeviceFeeder, DocumentCollator, PackedCollator, PadCollator, make_const_len_tokenize_fn,
-                   make_packed_tokenize_fn, make_truncate_tokenize_fn, pack_sft, stack_collate)
+from .data import (PREFERENCE_COLUMNS, BatchLoader, DeviceFeeder, DocumentCollator, PackedCollator, PadCollator, PreferenceCollator,
+                   make_const_len_tokenize_fn, make_packed_tokenize_fn, make_preference_tokenize_fn, make_truncate_tokenize_fn, pack_sft,
+                   stack_collate)
 from .launch import DistEnv, discover_env, init_distributed
 from .obs import OverlapMeter, ScalarWriter, TrainingPrinter, create_dict_result, log_training_scalars, nvtx_range, save_result
 from .optim import ShardedAdamW, check_max_grad_norm
@@ -75,6 +76,8 @@ TRAIN_DEFAULTS: Dict[str, Any] = dict(
     distill_teacher=None,           # HF checkpoint dir of a frozen native teacher: train on (1-a) CE + a T^2 KL(teacher || student)
     distill_alpha=0.5,              # a in (0, 1]: weight of the distillation term
     distill_temperature=1.0,        # T > 0: temperature of both softmaxes in the KL
+    dpo_beta=None,                  # beta > 0 (TRL's usual 0.1): DPO on preference pairs against a frozen reference; None: off
+    dpo_reference=None,             # HF checkpoint dir of the frozen native reference (main.py: model.pretrained when unset)
 )
 
 
@@ -143,7 +146,8 @@ class DecoupledTrainer:
     # ================================================================== construction
     def __init__(self, model: nn.Module = None, tokenizer=None, train_dataset=None, eval_dataset=None, args=None,
                  log=None, text_column_name: str = "text", preprocess_dataset_fn: Optional[Callable] = None,
-                 run_name: str = "", env: Optional[DistEnv] = None, teacher: Optional[nn.Module] = None):
+                 run_name: str = "", env: Optional[DistEnv] = None, teacher: Optional[nn.Module] = None,
+                 reference: Optional[nn.Module] = None):
         self.model, self.tokenizer = model, tokenizer
         self.train_dataset, self.eval_dataset = train_dataset, eval_dataset
         self.raw_args = args
@@ -167,12 +171,20 @@ class DecoupledTrainer:
         self._fused_smoothing = self._check_label_smoothing()
         self.z_loss_weight = self._check_z_loss()
         teacher_src = self._check_distill(teacher)
+        reference_src = self._check_dpo(reference, teacher_src is not None)
         if not isinstance(self.args.no_decay_1d, bool):
             raise ValueError(f"no_decay_1d must be true or false, got {self.args.no_decay_1d!r}")
         self.no_decay_1d = self.args.no_decay_1d
 
         self.initialize_com(env)
-        self.teacher = self._setup_teacher(teacher_src)
+        self.teacher = self._setup_frozen(teacher_src, "distillation teacher", "student")
+        self.reference = self._setup_frozen(reference_src, "DPO reference", "policy")
+        if self.teacher is not None and self.rank == 0:
+            self.log.info(f">>> distillation: alpha={self.model.distill_alpha}, temperature={self.model.distill_temperature} "
+                          f"(eval stays pure cross-entropy)")
+        if self.reference is not None and self.rank == 0:
+            self.log.info(f">>> DPO: beta={self.model.dpo_beta} on preference pairs, {self.batch_size} pairs = {2 * self.batch_size} rows "
+                          f"per micro-batch (eval reports the same objective)")
         if self._fused_smoothing and self.rank == 0:
             self.log.info(f">>> label_smoothing_factor={self._fused_smoothing}: smoothed inside the fused cross-entropy kernel "
                           f"of {type(self.model).__name__} (CUDA graphs stay available)")
@@ -204,6 +216,14 @@ class DecoupledTrainer:
             self.distill_host = self.distill_host.pin_memory()
         if self.teacher is not None:
             self.model.distill_out = self.distill_static
+        # DPO: each micro-batch's mean chosen reward, mean rejected reward and accuracy, written on the device like the z-term
+        self.dpo_static = torch.zeros(3, device=self.device, dtype=torch.float32)
+        self.dpo_host = torch.zeros(3, dtype=torch.float32)
+        if self.is_cuda:
+            self.dpo_host = self.dpo_host.pin_memory()
+        if self.reference is not None:
+            self.model.dpo_out = self.dpo_static
+        self.eval_dpo_accuracy: Optional[float] = None
         self.n_grad_acc_ddp = 1
         self._hook_extra_microbatches: Optional[Callable[[int, int], int]] = None   # tests: (rank, round) -> extra
         self._nvtx = os.environ.get("ACCO_NVTX") == "1"
@@ -441,26 +461,61 @@ class DecoupledTrainer:
         self.model.distill_alpha, self.model.distill_temperature = float(alpha), float(temp)
         return src
 
-    def _setup_teacher(self, src) -> Optional[nn.Module]:
-        """The frozen teacher on this rank's device in the student's weight dtype (a full copy per rank).  It is held by the trainer
-        only, never by the student, so its parameters stay out of the arena, ``parameters()`` and the checkpoints."""
+    def _check_dpo(self, reference: Optional[nn.Module], distilling: bool):
+        """Validates ``dpo_beta`` and returns the reference source: the ``reference`` module, the ``dpo_reference`` checkpoint directory,
+        or None (off).  The policy must be native, the data preference pairs (checked in :meth:`_tokenize_if_needed`), and no other
+        loss option may be on."""
+        a = self.args
+        beta, path = a.dpo_beta, a.dpo_reference
+        if beta is None:
+            if reference is not None:
+                raise ValueError("a DPO reference= was given without dpo_beta")
+            return None
+        if isinstance(beta, bool) or not isinstance(beta, (int, float)) or not math.isfinite(beta) or not beta > 0.0:
+            raise ValueError(f"dpo_beta must be a finite number > 0, got {beta!r}")
+        if reference is not None and path is not None:
+            raise ValueError("give the DPO reference either as the trainer's reference= argument or as dpo_reference, not both")
+        src = reference if reference is not None else path
+        if src is None:
+            raise ValueError("dpo_beta needs a frozen reference model: set dpo_reference (an HF checkpoint dir) or pass reference=")
+        if path is not None and not isinstance(path, (str, os.PathLike)):
+            raise ValueError(f"dpo_reference must be a checkpoint directory, got {path!r}")
+        from .models import NativeCausalLM
+        if not isinstance(self.model, NativeCausalLM):
+            raise ValueError(f"DPO needs a native policy (LlamaForCausalLM / GPTForCausalLM): the loss is computed inside their fused "
+                             f"kernels, and {type(self.model).__name__} has no such loss")
+        if distilling:
+            raise ValueError("dpo_beta cannot be combined with distill_teacher: at most one frozen model trains alongside the policy")
+        for key, on in (("label_smoothing_factor > 0", self.label_smoothing_factor), ("z_loss_weight > 0", self.z_loss_weight),
+                        ("packing", a.packing), ("document_mask", a.document_mask), ("const_len_batch", a.const_len_batch)):
+            if on:
+                raise ValueError(f"dpo_beta cannot be combined with {key}: DPO trains on padded preference pairs, one sample per row, "
+                                 f"with its own loss")
+        if reference is self.model:
+            raise ValueError("the DPO reference must be a separate model from the policy")
+        self.model.dpo_beta = float(beta)
+        return src
+
+    def _setup_frozen(self, src, role: str, trained: str) -> Optional[nn.Module]:
+        """The frozen ``role`` model (distillation teacher or DPO reference) on this rank's device in the trained model's weight dtype (a
+        full copy per rank).  It is held by the trainer only, never by the trained model, so its parameters stay out of the arena,
+        ``parameters()`` and the checkpoints."""
         if src is None:
             return None
         from .models import NativeCausalLM, from_pretrained
-        teacher = from_pretrained(str(src), device=self.device, dtype=self.param_dtype, native=True) if not isinstance(src, nn.Module) else src
-        if not isinstance(teacher, NativeCausalLM):
-            raise ValueError(f"the distillation teacher must be a native model (LlamaForCausalLM / GPTForCausalLM), got {type(teacher).__name__}")
-        if teacher.config.vocab_size != self.model.config.vocab_size or teacher.config.padded_vocab != self.model.config.padded_vocab:
-            raise ValueError(f"teacher and student vocabularies differ: {teacher.config.vocab_size} (padded {teacher.config.padded_vocab}) vs "
+        frozen = from_pretrained(str(src), device=self.device, dtype=self.param_dtype, native=True) if not isinstance(src, nn.Module) else src
+        if not isinstance(frozen, NativeCausalLM):
+            raise ValueError(f"the {role} must be a native model (LlamaForCausalLM / GPTForCausalLM), got {type(frozen).__name__}")
+        if frozen.config.vocab_size != self.model.config.vocab_size or frozen.config.padded_vocab != self.model.config.padded_vocab:
+            raise ValueError(f"{role} and {trained} vocabularies differ: {frozen.config.vocab_size} (padded {frozen.config.padded_vocab}) vs "
                              f"{self.model.config.vocab_size} (padded {self.model.config.padded_vocab})")
-        teacher.to(device=self.device, dtype=self.param_dtype)
-        teacher.requires_grad_(False)
-        teacher.eval()
+        frozen.to(device=self.device, dtype=self.param_dtype)
+        frozen.requires_grad_(False)
+        frozen.eval()
         if self.rank == 0:
-            n = sum(p.numel() for p in teacher.parameters())
-            self.log.info(f">>> distillation from {type(teacher).__name__} ({n / 1e6:.1f}M parameters, one copy per rank): "
-                          f"alpha={self.model.distill_alpha}, temperature={self.model.distill_temperature} (eval stays pure cross-entropy)")
-        return teacher
+            n = sum(p.numel() for p in frozen.parameters())
+            self.log.info(f">>> {role}: {type(frozen).__name__} ({n / 1e6:.1f}M parameters, frozen, one copy per rank)")
+        return frozen
 
     def prepare_data(self) -> None:
         """Per-rank sharding (`trainer_base.py:183-200`)."""
@@ -482,6 +537,11 @@ class DecoupledTrainer:
                 self.eval_dataset = self.eval_dataset.map(self.preprocess_dataset_fn, batched=True)
         if self.train_dataset is None:
             return
+        if self.args.dpo_beta is not None:
+            self.train_dataset = self._preference_pairs(self.train_dataset)
+            if self.eval_dataset is not None:
+                self.eval_dataset = self._preference_pairs(self.eval_dataset)
+            return
         if "input_ids" in self.train_dataset.column_names:
             if a.packing and "doc_lens" not in self.train_dataset.column_names:
                 L = int(a.max_length)
@@ -500,6 +560,20 @@ class DecoupledTrainer:
             self.eval_dataset = self.eval_dataset.map(fn, batched=True, remove_columns=self.eval_dataset.column_names, num_proc=nproc)
         if a.packing:
             self._log_packing()
+
+    def _preference_pairs(self, ds):
+        """DPO data: token columns ``prompt_ids`` / ``chosen_ids`` / ``rejected_ids`` as they are, or TRL's ``prompt`` / ``chosen`` /
+        ``rejected`` text columns tokenised; anything else is not preference data."""
+        cols = set(ds.column_names)
+        if set(PREFERENCE_COLUMNS) <= cols:
+            return ds
+        if not {"prompt", "chosen", "rejected"} <= cols:
+            raise ValueError(f"dpo_beta needs preference pairs: columns prompt / chosen / rejected (text) or {' / '.join(PREFERENCE_COLUMNS)} "
+                             f"(token ids), got {sorted(cols)}")
+        if self.tokenizer is None:
+            raise ValueError("the preference dataset has text columns and no tokenizer was given")
+        nproc = int(self.args.dataloader_num_workers) or None
+        return ds.map(make_preference_tokenize_fn(self.tokenizer), batched=True, remove_columns=ds.column_names, num_proc=nproc)
 
     def _log_packing(self) -> None:
         if self.rank != 0:
@@ -521,6 +595,8 @@ class DecoupledTrainer:
             mult = 64 if self.is_cuda else 1        # few distinct padded lengths -> one CUDA graph per length
             if self.is_cuda and os.environ.get("ACCO_ATTN", "").lower() == "own":
                 mult = 128                          # the own attention kernels tile the sequence in blocks of 128
+        if self.args.dpo_beta is not None:
+            return PreferenceCollator(pad_token_id=pad, max_length=int(self.args.max_length), pad_to_multiple_of=int(mult))
         return PadCollator(pad_token_id=pad, max_length=int(self.args.max_length), pad_to_multiple_of=int(mult))
 
     def get_train_dataloader(self) -> Optional[BatchLoader]:
@@ -649,10 +725,16 @@ class DecoupledTrainer:
         self.overlap = OverlapMeter(enabled=False)
 
     # ================================================================== step primitives
-    def _forward_loss(self, model: nn.Module, inputs: Dict[str, torch.Tensor], teacher: Optional[nn.Module] = None) -> torch.Tensor:
+    def _forward_loss(self, model: nn.Module, inputs: Dict[str, torch.Tensor], teacher: Optional[nn.Module] = None,
+                      reference: Optional[nn.Module] = None) -> torch.Tensor:
         if self.label_smoother is not None and "labels" in inputs:
             return self.compute_loss(model, dict(inputs))
-        if teacher is not None:
+        if reference is not None:
+            # the reference scores the same [2P, S] pair rows; its forward is captured with the policy's in one micro-batch graph
+            with torch.no_grad():
+                r_logits = reference.padded_logits(inputs["input_ids"])
+            out = model(**inputs, reference_logits=r_logits)
+        elif teacher is not None:
             # the teacher sees the same tokens and positions, so packed / document-masked rows are masked alike for both models
             with torch.no_grad():
                 t_logits = teacher.padded_logits(inputs["input_ids"], inputs.get("position_ids"))
@@ -704,7 +786,8 @@ class DecoupledTrainer:
         model = model or self.model
         ctx = torch.autocast(device_type=self.device.type, dtype=self.dtype) if self.autocast else contextlib.nullcontext()
         with ctx:
-            loss = self._forward_loss(model, inputs) if self.teacher is None else self._forward_loss(model, inputs, self.teacher)
+            frozen = self.teacher is not None or self.reference is not None
+            loss = self._forward_loss(model, inputs, self.teacher, self.reference) if frozen else self._forward_loss(model, inputs)
             scaled = loss / self.n_grad_acc_ddp if self.n_grad_acc_ddp != 1 else loss
         scaled.backward()
         return loss.detach()
@@ -861,20 +944,20 @@ class DecoupledTrainer:
         with nvtx_range(f"acco/phase r{self.sched.round}") if self._nvtx else contextlib.nullcontext():
             for _ in range(n):
                 self.gradient_step()
+        self._copy_scalars_to_host(non_blocking=self.is_cuda)
         if self.is_cuda:
-            self.loss_host.copy_(self.loss_static, non_blocking=True)
-            if self.z_loss_weight:
-                self.z_loss_host.copy_(self.z_loss_static, non_blocking=True)
-            if self.teacher is not None:
-                self.distill_host.copy_(self.distill_static, non_blocking=True)
             self.end_of_grad.record(self.grad_stream)
             self._poll_phase_end()
-        else:
-            self.loss_host.copy_(self.loss_static)
-            if self.z_loss_weight:
-                self.z_loss_host.copy_(self.z_loss_static)
-            if self.teacher is not None:
-                self.distill_host.copy_(self.distill_static)
+
+    def _copy_scalars_to_host(self, non_blocking: bool) -> None:
+        """The loss and the loss options' logged device scalars -> their (pinned) host copies."""
+        self.loss_host.copy_(self.loss_static, non_blocking=non_blocking)
+        if self.z_loss_weight:
+            self.z_loss_host.copy_(self.z_loss_static, non_blocking=non_blocking)
+        if self.teacher is not None:
+            self.distill_host.copy_(self.distill_static, non_blocking=non_blocking)
+        if self.reference is not None:
+            self.dpo_host.copy_(self.dpo_static, non_blocking=non_blocking)
 
     def _poll_phase_end(self) -> None:
         """The flip decision must be taken when the *device* reaches the end of the phase ("if the com finished ... else accumulate
@@ -1031,11 +1114,7 @@ class DecoupledTrainer:
             sched.opt_steps += 1
             sched.lr_steps += 1
             sched.count_grad_tot += self.world_size * int(a.n_grad_accumulation)
-            self.loss_host.copy_(self.loss_static)
-            if self.z_loss_weight:
-                self.z_loss_host.copy_(self.z_loss_static)
-            if self.teacher is not None:
-                self.distill_host.copy_(self.distill_static)
+            self._copy_scalars_to_host(non_blocking=False)
             self._tail(None)
         return self._finish("_ddp")
 
@@ -1097,6 +1176,10 @@ class DecoupledTrainer:
                     gn["z_loss"] = float(self.z_loss_host.item())    # the loss's z-term: cross-entropy = loss - z_loss
                 if self.teacher is not None:                          # loss = (1 - a) distill_ce + a T^2 distill_kl
                     gn["distill_ce"], gn["distill_kl"] = (float(v) for v in self.distill_host.tolist())
+                if self.reference is not None:                        # loss = the DPO objective
+                    gn["dpo_reward_chosen"], gn["dpo_reward_rejected"], gn["dpo_accuracy"] = (float(v) for v in self.dpo_host.tolist())
+                    if eval_loss is not None and self.eval_dpo_accuracy is not None:
+                        gn["eval_dpo_accuracy"] = self.eval_dpo_accuracy
                 log_training_scalars(self.writer, nb_step, sched.count_grad_tot, self.rank, loss, eval_loss, self.t_beg,
                                      extra={"lr": getattr(self, "_last_lr", 0.0), **gn})
                 self._fire("on_log", {"step": nb_step, "count_grad_tot": sched.count_grad_tot, "loss": loss,
@@ -1112,6 +1195,9 @@ class DecoupledTrainer:
                         gn_txt += f" | z_loss {gn['z_loss']:.4g}"
                     if self.teacher is not None:
                         gn_txt += f" | distill_ce {gn['distill_ce']:.4g} | distill_kl {gn['distill_kl']:.4g}"
+                    if self.reference is not None:
+                        gn_txt += (f" | dpo_reward_chosen {gn['dpo_reward_chosen']:.4g} | dpo_reward_rejected {gn['dpo_reward_rejected']:.4g}"
+                                   f" | dpo_accuracy {gn['dpo_accuracy']:.3f}")
                     pr.emit(sched.count_grad_tot, sched.count_com, loss, extra=f" | {rate:,.0f} tok/s/rank | lr {getattr(self, '_last_lr', 0.0):.3e}{gn_txt}")
                 self.epoch = pr.epoch
         if committed and plan is not None and self.callbacks:
@@ -1162,10 +1248,14 @@ class DecoupledTrainer:
 
     @torch.no_grad()
     def eval_loop(self) -> torch.Tensor:
-        """Mean loss over this rank's eval shard (`trainer_decoupled.py:399-415`)."""
+        """Mean loss over this rank's eval shard (`trainer_decoupled.py:399-415`).  With DPO the loss is the DPO objective (reference
+        forward included) and ``eval_dpo_accuracy`` the mean accuracy over the eval micro-batches."""
         self._ensure_gathered()
         self.model.eval()
         losses: List[torch.Tensor] = []
+        accs: List[torch.Tensor] = []
+        if self.reference is not None:
+            self.model.dpo_out = torch.zeros(3, device=self.device, dtype=torch.float32)   # the training scalars stay as logged
         ctx = torch.autocast(device_type=self.device.type, dtype=self.dtype) if self.autocast else contextlib.nullcontext()
         if self.z_loss_weight:
             self.model.z_loss_weight = 0.0          # eval loss stays pure cross-entropy, comparable with runs without the key
@@ -1175,15 +1265,25 @@ class DecoupledTrainer:
                     break
                 inputs = {k: v.to(self.device, non_blocking=True) for k, v in inputs.items()}
                 with ctx:
-                    losses.append(self._forward_loss(self.model, inputs).detach().float().reshape(1))
+                    loss = self._forward_loss(self.model, inputs) if self.reference is None else \
+                        self._forward_loss(self.model, inputs, reference=self.reference)
+                    losses.append(loss.detach().float().reshape(1))
+                if self.reference is not None:
+                    accs.append(self.model.dpo_out[2:].clone())
         finally:
             if self.z_loss_weight:
                 self.model.z_loss_weight = self.z_loss_weight
+            if self.reference is not None:
+                self.model.dpo_out = self.dpo_static
         self.model.train()
         if not losses:
             return torch.tensor(float("nan"))
         mean = torch.cat(losses).mean().cpu()
-        self.log.info(f"eval loss {float(mean):.4f}")
+        if accs:
+            self.eval_dpo_accuracy = float(torch.cat(accs).mean())
+            self.log.info(f"eval loss {float(mean):.4f} | eval dpo_accuracy {self.eval_dpo_accuracy:.3f}")
+        else:
+            self.log.info(f"eval loss {float(mean):.4f}")
         return mean
 
     # ------------------------------------------------------------------ end of run

@@ -35,7 +35,7 @@ logger = logging.getLogger("distributed_worker")
 
 def load_data(cfg, vocab_size: int, tokenizer):
     """-> (train, test, tokenizer).  Tries the HF hub id first unless ``data.synthetic`` is true."""
-    from acco_b200.data import ByteTokenizer, synthetic_pretrain_dataset, synthetic_sft_dataset
+    from acco_b200.data import ByteTokenizer, synthetic_preference_dataset, synthetic_pretrain_dataset, synthetic_sft_dataset
     d, t = cfg.data, cfg.train
     mode = str(d.get("synthetic", "auto")).lower()
     if mode not in ("true", "1", "yes") and d.get("path"):
@@ -53,7 +53,12 @@ def load_data(cfg, vocab_size: int, tokenizer):
             logger.info(f"could not load dataset {d.path!r} ({type(e).__name__}); using a synthetic {d.get('kind', 'pretrain')} corpus")
     n_docs, mean_len = int(d.get("synthetic_docs", 4096)), int(d.get("synthetic_mean_len", 900))
     seed = int(cfg.get("seed", 0))
-    if str(d.get("kind", "pretrain")) == "sft" or not t.const_len_batch:
+    if str(d.get("kind", "pretrain")) == "preference":
+        full = synthetic_preference_dataset(n_docs, mean_len, vocab_size - 1, seed=seed)
+        if tokenizer is None:
+            tokenizer = ByteTokenizer(eos_token_id=vocab_size - 1)
+            tokenizer.pad_token_id = tokenizer.eos_token_id
+    elif str(d.get("kind", "pretrain")) == "sft" or not t.const_len_batch:
         full = synthetic_sft_dataset(n_docs, mean_len, vocab_size - 1, int(t.max_length), seed=seed)
         if tokenizer is None:
             tokenizer = ByteTokenizer(eos_token_id=vocab_size - 1)
@@ -113,6 +118,10 @@ def main(argv=None):
         dev = torch.device("cuda", discover_env().local_rank)
     mdtype = torch.bfloat16 if (dev is not None and cfg.train.use_mixed_precision) else None
     pretrained = cfg.model.get("pretrained")
+    if cfg.train.get("dpo_beta") is not None and cfg.train.get("dpo_reference") is None and pretrained:
+        # DPO's reference is the pretrained checkpoint the policy starts from, reloaded from disk: a resume_from run then gets the
+        # same reference again, not a copy of the resumed policy
+        cfg.train["dpo_reference"] = str(pretrained)
     if cfg.train.finetune and pretrained:
         # reference: AutoModelForCausalLM.from_pretrained(config_path) (`main.py:33-35`)
         from acco_b200.models import from_pretrained

@@ -62,6 +62,10 @@ KERNELS = {
     "kd_reduce.sass": "_ZN4acco16kd_reduce_kernelEPKfPKxPfS4_S4_xxff",
     "kd_bwd.sass": "_ZN4acco13kd_bwd_kernelILb0EEEvP13__nv_bfloat16PKS1_PKxPKfS8_xiixfff",
     "kd_bwd_t1.sass": "_ZN4acco13kd_bwd_kernelILb1EEEvP13__nv_bfloat16PKS1_PKxPKfS8_xiixfff",
+    # DPO (train.dpo_beta): one pass over the policy and reference rows forward, one over the policy backward
+    "dpo_fwd.sass": "_ZN4acco14dpo_fwd_kernelEPK13__nv_bfloat16S2_PKxPfS5_iix",
+    "dpo_reduce.sass": "_ZN4acco17dpo_reduce_kernelEPKfPKxPfS4_S4_S4_iixf",
+    "dpo_bwd.sass": "_ZN4acco14dpo_bwd_kernelEP13__nv_bfloat16PKxPKfS5_S5_iiix",
 }
 MNEMONICS = ["HGMMA", "UTMALDG", "UTMALDG.2D.MULTICAST", "UTMASTG", "UTMACMDFLUSH", "SYNCS", "USETMAXREG", "REDG", "LDGMC", "HMMA", "MUFU.SQRT",
              "MUFU.EX2", "CCTL"]
