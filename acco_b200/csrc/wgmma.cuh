@@ -62,6 +62,20 @@ __device__ __forceinline__ void tma_load_2d_mc(const CUtensorMap* map, uint64_t*
         "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
         : "memory");
 }
+__device__ __forceinline__ void tma_load_3d(const CUtensorMap* map, uint64_t* bar, void* smem, int c0, int c1, int c2) {
+    asm volatile(
+        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(
+            smem_u32(smem)),
+        "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+        : "memory");
+}
+__device__ __forceinline__ void tma_load_3d_mc(const CUtensorMap* map, uint64_t* bar, void* smem, int c0, int c1, int c2, uint16_t mask) {
+    asm volatile(
+        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(
+            smem_u32(smem)),
+        "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "h"(mask)
+        : "memory");
+}
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* smem, int c0, int c1) {
     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map), "r"(smem_u32(smem)),
                  "r"(c0), "r"(c1)
