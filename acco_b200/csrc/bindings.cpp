@@ -32,6 +32,8 @@ int acco_kd_bwd(void* student, const void* teacher, const long long* labels, con
                 long long ignore_index, float alpha, float temperature, cudaStream_t st);
 int acco_dpo_fwd(const void* policy, const void* ref, const long long* labels, float* lse, float* d, float* rowbuf, float* w, float* loss,
                  float* out, int P, int S, int V, int Vp, long long ignore_index, float beta, cudaStream_t st);
+int acco_pref_fwd(const void* logits, const long long* labels, float* lse, float* row_loss, float* rowbuf, float* w, float* loss, float* out,
+                  int P, int S, int V, int Vp, long long ignore_index, int orpo, float coef, float gamma, cudaStream_t st);
 int acco_dpo_bwd(void* policy, const long long* labels, const float* lse, const float* w, const float* dloss, int P, int S, int V, int Vp,
                  long long ignore_index, cudaStream_t st);
 int acco_norm_bwd_acc_f32(const void* dy, const void* dh_extra, const void* h, const void* w, const float* mean, const float* rstd, void* dh,
@@ -426,6 +428,35 @@ std::vector<torch::Tensor> dpo_fwd(torch::Tensor logits, torch::Tensor ref_logit
     TORCH_CHECK(acco_dpo_fwd(logits.data_ptr(), ref_logits.data_ptr(), (const long long*)labels.data_ptr<int64_t>(), lse.data_ptr<float>(),
                              d.data_ptr<float>(), rowbuf.data_ptr<float>(), w.data_ptr<float>(), loss.data_ptr<float>(), out.data_ptr<float>(),
                              (int)P, (int)S, (int)V, (int)Vp, ignore_index, (float)beta, stream()) == 0, "dpo_fwd: bad arguments");
+    return {loss, lse, w};
+}
+
+// SimPO (orpo false: coef = beta, gamma the margin) or ORPO (orpo true: coef = lambda, gamma unused and 0) over the same pair
+// layout as DPO, without reference logits.  Returns (loss, lse [T], w [2P]); `out` (three fp32 on the logits' device) receives SimPO's
+// mean chosen reward, mean rejected reward and accuracy, or ORPO's NLL, mean log odds ratio and accuracy.  The backward is
+// dpo_bwd_inplace with these w.
+std::vector<torch::Tensor> pref_fwd(torch::Tensor logits, torch::Tensor labels, int64_t P, int64_t V, int64_t ignore_index, bool orpo,
+                                    double coef, double gamma, torch::Tensor out) {
+    const int64_t S = check_dpo(logits, labels, P, V);
+    const char* name = orpo ? "lambda" : "beta";
+    TORCH_CHECK(std::isfinite(coef) && coef > 0.0 && std::isfinite((float)coef) && (float)coef > 0.f, name, " must be finite and > 0, got ",
+                coef);
+    TORCH_CHECK(std::isfinite(gamma) && gamma >= 0.0 && std::isfinite((float)gamma) && (!orpo || gamma == 0.0),
+                "gamma must be finite and >= 0 (and 0 for ORPO), got ", gamma);
+    TORCH_CHECK(out.is_cuda() && out.device() == logits.device() && out.scalar_type() == torch::kFloat32 && out.numel() == 3 && out.is_contiguous(),
+                "out must be a contiguous three-element fp32 tensor on the logits' device");
+    const c10::cuda::CUDAGuard guard(logits.device());
+    const int64_t T = logits.size(0), Vp = logits.size(1);
+    auto f32 = logits.options().dtype(torch::kFloat32);
+    auto lse = torch::empty({T}, f32);
+    auto row_loss = torch::empty({T}, f32);
+    auto rowbuf = torch::empty({4 * P}, f32);
+    auto w = torch::empty({2 * P}, f32);
+    auto loss = torch::empty({}, f32);
+    TORCH_CHECK(acco_pref_fwd(logits.data_ptr(), (const long long*)labels.data_ptr<int64_t>(), lse.data_ptr<float>(), row_loss.data_ptr<float>(),
+                              rowbuf.data_ptr<float>(), w.data_ptr<float>(), loss.data_ptr<float>(), out.data_ptr<float>(), (int)P, (int)S,
+                              (int)V, (int)Vp, ignore_index, orpo ? 1 : 0, (float)coef, (float)gamma, stream()) == 0,
+                "pref_fwd: bad arguments");
     return {loss, lse, w};
 }
 
@@ -901,6 +932,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("alpha"), py::arg("temperature"), py::arg("out"));
     m.def("dpo_fwd", &dpo_fwd, py::arg("logits"), py::arg("ref_logits"), py::arg("labels"), py::arg("P"), py::arg("V"), py::arg("ignore_index"),
           py::arg("beta"), py::arg("out"));
+    m.def("pref_fwd", &pref_fwd, py::arg("logits"), py::arg("labels"), py::arg("P"), py::arg("V"), py::arg("ignore_index"), py::arg("orpo"),
+          py::arg("coef"), py::arg("gamma"), py::arg("out"));
     m.def("dpo_bwd_inplace", &dpo_bwd_inplace, py::arg("logits"), py::arg("labels"), py::arg("lse"), py::arg("w"), py::arg("dloss"), py::arg("P"),
           py::arg("V"), py::arg("ignore_index"));
     m.def("kd_bwd_inplace", &kd_bwd_inplace, py::arg("logits"), py::arg("teacher_logits"), py::arg("labels"), py::arg("lse3"), py::arg("scale"),

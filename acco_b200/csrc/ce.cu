@@ -40,6 +40,15 @@
 //             Subtracting per token keeps the cancellation out of the long fp32 sums and makes d == 0 exact for s == r.
 //   dpo_reduce : one CTA, fixed order: row sums of d, z, the loss, the per-row weight w and three logged means.
 //   dpo_bwd : in place on s, like ce_bwd with the scale dloss * w[row].
+//
+// Reference-free preference objectives (pref_reduce<kSimPO | kORPO>; no reference logits).  Same [2P, S] pair layout;
+// l(row) = sum_{t in R(row)} (s_t[y_t] - lse(s_t)), a(row) = l(row) / |row|, valid pair = both rows non-empty, n = #valid.
+//   SimPO: z_i = beta (a(c_i) - a(r_i)) - gamma,  loss = mean_valid softplus(-z_i),
+//          w(c_i) = beta sigma(-z_i) / (n |c_i|),  w(r_i) = -beta sigma(-z_i) / (n |r_i|).
+//   ORPO:  nll = -sum_valid l(c_i) / N_c (N_c = sum_valid |c_i|),  lo_i = (a - log(1 - e^a'))(c_i) - (a - log(1 - e^a'))(r_i),
+//          a' = min(a, -2^-20) (the clamp also enters the gradient),  loss = nll + lambda mean_valid softplus(-lo_i),
+//          w(c_i) = 1 / N_c + lambda sigma(-lo_i) / (n |c_i| (1 - e^a'(c_i))),  w(r_i) = -lambda sigma(-lo_i) / (n |r_i| (1 - e^a'(r_i))).
+//   Forward: ce_fwd<false, false> (lse and -log p per token) and pref_reduce; backward: dpo_bwd with the weights w.
 #include "common.cuh"
 
 namespace acco {
@@ -526,6 +535,115 @@ __global__ void __launch_bounds__(kCEThreads) dpo_bwd_kernel(__nv_bfloat16* __re
     }
 }
 
+// ---------------------------------------------------------------- SimPO / ORPO
+constexpr int kSimPO = 0, kORPO = 1;
+constexpr float kORPOMaxA = -9.5367431640625e-07f;      // -2^-20: a is clamped below 0 so that log(1 - e^a) stays finite
+
+ACCO_DEVINL float softplus_neg(float z) { return fmaxf(-z, 0.f) + log1pf(__expf(-fabsf(z))); }     // softplus(-z), any |z|
+
+ACCO_DEVINL float sigmoid_neg(float z) {                // sigma(-z), any |z|
+    const float e = __expf(-fabsf(z));
+    return z >= 0.f ? e / (1.f + e) : 1.f / (1.f + e);
+}
+
+ACCO_DEVINL float log1m_exp(float a) {                  // log(1 - e^a) for a < 0, without cancellation on either side of -ln 2
+    return a > -0.693147182f ? __logf(-expm1f(a)) : log1pf(-__expf(a));
+}
+
+// One CTA of 1024 threads, fixed order (two launches are bitwise equal), over ce_fwd's per-token -log p (0 on ignored tokens).
+//   rowbuf [2, 2P]: per row l = -sum row_loss and the count of non-ignored tokens (warp w sums rows w, w + 32, ...).
+//   coef: SimPO's beta or ORPO's lambda; gamma: SimPO's margin (ORPO ignores it).
+//   out: SimPO (mean beta a(c), mean beta a(r), mean [a(c) > a(r)]), ORPO (nll, mean lo, mean [lo > 0]).  n = 0: loss, w, out 0.
+template <int kObj>
+__global__ void __launch_bounds__(1024) pref_reduce_kernel(const float* __restrict__ row_loss, const long long* __restrict__ labels,
+                                                           float* __restrict__ rowbuf, float* __restrict__ w, float* __restrict__ loss,
+                                                           float* __restrict__ out, int P, int S, long long ignore_index, float coef,
+                                                           float gamma) {
+    __shared__ float red[32];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    const int R = 2 * P;
+    for (int r = wid; r < R; r += nw) {
+        float sl = 0.f, cnt = 0.f;
+        for (int t = lane; t < S; t += 32) {
+            const long long i = (long long)r * S + t;
+            if (labels[i] != ignore_index) {
+                sl -= row_loss[i];
+                cnt += 1.f;
+            }
+        }
+        sl = warp_sum(sl);
+        cnt = warp_sum(cnt);
+        if (lane == 0) {
+            rowbuf[r] = sl;
+            rowbuf[R + r] = cnt;
+        }
+    }
+    __syncthreads();
+    // SimPO: s1, s2 = sums of beta a(c), beta a(r).  ORPO: s1 = sum l(c), s2 = sum lo, sn = N_c.
+    float n = 0.f, sl = 0.f, s1 = 0.f, s2 = 0.f, sa = 0.f, sn = 0.f;
+    for (int i = threadIdx.x; i < P; i += blockDim.x) {
+        const float nc = rowbuf[R + i], nr = rowbuf[R + P + i];
+        if (nc > 0.f && nr > 0.f) {
+            const float ac = rowbuf[i] / nc, ar = rowbuf[P + i] / nr;
+            n += 1.f;
+            if constexpr (kObj == kSimPO) {
+                const float rc = __fmul_rn(coef, ac), rr = __fmul_rn(coef, ar);
+                sl += softplus_neg(__fsub_rn(__fsub_rn(rc, rr), gamma));
+                s1 += rc;
+                s2 += rr;
+                sa += ac > ar ? 1.f : 0.f;
+            } else {
+                const float lo = (ac - log1m_exp(fminf(ac, kORPOMaxA))) - (ar - log1m_exp(fminf(ar, kORPOMaxA)));
+                sl += softplus_neg(lo);
+                s1 += rowbuf[i];
+                s2 += lo;
+                sa += lo > 0.f ? 1.f : 0.f;
+                sn += nc;
+            }
+        }
+    }
+    n = block_sum(n, red);
+    sl = block_sum(sl, red);
+    s1 = block_sum(s1, red);
+    s2 = block_sum(s2, red);
+    sa = block_sum(sa, red);
+    if constexpr (kObj == kORPO) sn = block_sum(sn, red);
+    const float inv = n > 0.f ? 1.f / n : 0.f;
+    const float inv_nc = sn > 0.f ? 1.f / sn : 0.f;
+    for (int i = threadIdx.x; i < P; i += blockDim.x) {
+        const float nc = rowbuf[R + i], nr = rowbuf[R + P + i];
+        float wc = 0.f, wr = 0.f;
+        if (nc > 0.f && nr > 0.f) {
+            const float ac = rowbuf[i] / nc, ar = rowbuf[P + i] / nr;                                   // as above
+            if constexpr (kObj == kSimPO) {
+                const float z = __fsub_rn(__fsub_rn(__fmul_rn(coef, ac), __fmul_rn(coef, ar)), gamma);
+                const float g = coef * sigmoid_neg(z) * inv;
+                wc = g / nc;
+                wr = -g / nr;
+            } else {
+                const float cc = fminf(ac, kORPOMaxA), cr = fminf(ar, kORPOMaxA);
+                const float g = coef * sigmoid_neg((ac - log1m_exp(cc)) - (ar - log1m_exp(cr))) * inv;
+                wc = inv_nc + g / (nc * -expm1f(cc));
+                wr = -g / (nr * -expm1f(cr));
+            }
+        }
+        w[i] = wc;
+        w[P + i] = wr;
+    }
+    if (threadIdx.x == 0) {
+        if constexpr (kObj == kSimPO) {
+            *loss = sl * inv;
+            out[0] = s1 * inv;
+        } else {
+            const float nll = (0.f - s1) * inv_nc;
+            *loss = nll + coef * (sl * inv);
+            out[0] = nll;
+        }
+        out[1] = s2 * inv;
+        out[2] = sa * inv;
+    }
+}
+
 }  // namespace acco
 
 // `label_smoothing` in [0, 1] and `z_loss` >= 0 (checked by the binding); 0 runs the instantiation without the term.  With
@@ -592,5 +710,22 @@ extern "C" int acco_dpo_bwd(void* policy, const long long* labels, const float* 
     if (Vp % 8 != 0 || V <= 0 || V > Vp || P <= 0 || S <= 0) return -1;
     acco::dpo_bwd_kernel<<<(unsigned)(2LL * P * S), acco::kCEThreads, 0, st>>>((__nv_bfloat16*)policy, labels, lse, w, dloss, S, V, Vp,
                                                                                ignore_index);
+    return 0;
+}
+
+// SimPO (orpo == 0: coef = beta, gamma >= 0) or ORPO (orpo != 0: coef = lambda) over T = 2 P S token rows: finite coef > 0, finite
+// gamma >= 0, P, S > 0, Vp % 8 == 0 and V <= Vp, else -1 (nothing launched).  Writes lse, row_loss [T], rowbuf [4P], w [2P], the
+// loss and `out` (three fp32).  The backward is acco_dpo_bwd with these w.
+extern "C" int acco_pref_fwd(const void* logits, const long long* labels, float* lse, float* row_loss, float* rowbuf, float* w, float* loss,
+                             float* out, int P, int S, int V, int Vp, long long ignore_index, int orpo, float coef, float gamma,
+                             cudaStream_t st) {
+    if (Vp % 8 != 0 || V <= 0 || V > Vp || P <= 0 || S <= 0 || !(coef > 0.f && coef < INFINITY) || !(gamma >= 0.f && gamma < INFINITY) ||
+        out == nullptr)
+        return -1;
+    const long long T = 2LL * P * S;
+    acco::ce_fwd_kernel<false, false><<<(unsigned)T, acco::kCEThreads, 0, st>>>((const __nv_bfloat16*)logits, labels, lse, row_loss, V, Vp,
+                                                                                ignore_index, 1.f, 0.f, 0.f);
+    auto k = orpo ? acco::pref_reduce_kernel<acco::kORPO> : acco::pref_reduce_kernel<acco::kSimPO>;
+    k<<<1, 1024, 0, st>>>(row_loss, labels, rowbuf, w, loss, out, P, S, ignore_index, coef, gamma);
     return 0;
 }

@@ -63,6 +63,12 @@ class NativeCausalLM(nn.Module):
         # loss's mean chosen reward, mean rejected reward and accuracy (ops.dpo_loss)
         self.dpo_beta = 0.1
         self.dpo_out: Optional[torch.Tensor] = None
+        # reference-free preference objectives (train keys `simpo_beta` / `simpo_gamma`, `orpo_lambda`): the one set (not None) is the
+        # loss of a forward given preference_pairs=True; three fp32 on the device receive its logged means (ops.simpo_loss / orpo_loss)
+        self.simpo_beta: Optional[float] = None
+        self.simpo_gamma = 0.5
+        self.orpo_lambda: Optional[float] = None
+        self.pref_out: Optional[torch.Tensor] = None
 
     @property
     def embed_weight(self) -> torch.Tensor:
@@ -94,18 +100,24 @@ class NativeCausalLM(nn.Module):
 
     # ------------------------------------------------------------------ loss
     def _lm_output(self, logits: torch.Tensor, labels: Optional[torch.Tensor], B: int, S: int,
-                   teacher_logits: Optional[torch.Tensor] = None, reference_logits: Optional[torch.Tensor] = None) -> CausalLMOutput:
+                   teacher_logits: Optional[torch.Tensor] = None, reference_logits: Optional[torch.Tensor] = None,
+                   preference_pairs: bool = False) -> CausalLMOutput:
         """Logits ``[B*S, Vp]`` -> the logits cut to ``vocab_size`` without labels, else the mean cross-entropy loss, or with
         ``teacher_logits`` (a teacher's :meth:`padded_logits` on the same tokens) the distillation objective, over the same rows.
         With ``reference_logits`` (a frozen reference's :meth:`padded_logits`) the ``B = 2P`` rows are ``P`` preference pairs, chosen
-        rows first, and the loss is the DPO objective over the response tokens the labels keep (``ops.dpo_loss``)."""
+        rows first, and the loss is the DPO objective over the response tokens the labels keep (``ops.dpo_loss``).  With
+        ``preference_pairs=True`` the rows are laid out the same way and the loss is the reference-free objective set on the model:
+        SimPO (``simpo_beta``, ``simpo_gamma``; ``ops.simpo_loss``) or ORPO (``orpo_lambda``; ``ops.orpo_loss``)."""
         V = self.config.vocab_size
         if labels is None:
-            if teacher_logits is not None or reference_logits is not None:
-                raise ValueError("teacher_logits / reference_logits need labels: the loss is taken over the rows the labels keep")
+            if teacher_logits is not None or reference_logits is not None or preference_pairs:
+                raise ValueError("teacher_logits / reference_logits / preference_pairs need labels: the loss is taken over the rows the "
+                                 "labels keep")
             return CausalLMOutput(loss=None, logits=logits.view(B, S, -1)[..., :V])
         if teacher_logits is not None and reference_logits is not None:
             raise ValueError("give teacher_logits (distillation) or reference_logits (DPO), not both")
+        if preference_pairs and (teacher_logits is not None or reference_logits is not None):
+            raise ValueError("preference_pairs (SimPO / ORPO) needs no frozen model: give it without teacher_logits / reference_logits")
         # HF shift: position t predicts token t+1; the last position has no target
         shifted = torch.full_like(labels, -100)
         shifted[:, :-1] = labels[:, 1:]
@@ -121,6 +133,19 @@ class NativeCausalLM(nn.Module):
             if B % 2:
                 raise ValueError(f"DPO needs an even number of rows (P chosen, then P rejected), got {B}")
             loss = ops.dpo_loss(logits, reference_logits, shifted.reshape(B * S), B // 2, V, self.dpo_beta, out=self.dpo_out)
+            return CausalLMOutput(loss=loss, logits=None)
+        if preference_pairs:
+            if self.label_smoothing or self.z_loss_weight:
+                raise ValueError("SimPO / ORPO cannot be combined with label smoothing or the z-loss")
+            if (self.simpo_beta is None) == (self.orpo_lambda is None):
+                raise ValueError(f"preference_pairs needs exactly one objective set on the model: simpo_beta={self.simpo_beta!r}, "
+                                 f"orpo_lambda={self.orpo_lambda!r}")
+            if B % 2:
+                raise ValueError(f"preference pairs need an even number of rows (P chosen, then P rejected), got {B}")
+            if self.simpo_beta is not None:
+                loss = ops.simpo_loss(logits, shifted.reshape(B * S), B // 2, V, self.simpo_beta, self.simpo_gamma, out=self.pref_out)
+            else:
+                loss = ops.orpo_loss(logits, shifted.reshape(B * S), B // 2, V, self.orpo_lambda, out=self.pref_out)
             return CausalLMOutput(loss=loss, logits=None)
         loss = ops.softmax_cross_entropy(logits, shifted.reshape(B * S), V, -100, label_smoothing=self.label_smoothing,
                                          z_loss=self.z_loss_weight, z_loss_out=self.z_loss_out)

@@ -160,16 +160,19 @@ class LlamaForCausalLM(NativeCausalLM):
     # ------------------------------------------------------------------ forward
     def forward(self, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor] = None,
                 labels: Optional[torch.Tensor] = None, position_ids: Optional[torch.Tensor] = None,
-                teacher_logits: Optional[torch.Tensor] = None, reference_logits: Optional[torch.Tensor] = None, **unused) -> CausalLMOutput:
+                teacher_logits: Optional[torch.Tensor] = None, reference_logits: Optional[torch.Tensor] = None,
+                preference_pairs: bool = False, **unused) -> CausalLMOutput:
         """HF-style call.  ``attention_mask`` is accepted for API compatibility; with right
         padding and causal attention the logits at non-pad positions do not depend on it, and pad
         positions carry ``labels == -100`` (the collator's job), so it is not applied.
         ``position_ids [B, S]`` marks packed rows (``PackedCollator``): positions restart at 0 for every sample, RoPE uses them
         and no token attends to another sample.
         ``teacher_logits [B*S, Vp]`` (with labels): the loss is the distillation objective; ``reference_logits [B*S, Vp]`` (with
-        labels, ``B = 2P`` rows of preference pairs): the DPO objective (:meth:`_lm_output`)."""
+        labels, ``B = 2P`` rows of preference pairs): the DPO objective; ``preference_pairs=True`` (with labels, the same rows): the
+        model's SimPO or ORPO objective (:meth:`_lm_output`)."""
         B, S = input_ids.shape
-        return self._lm_output(self.padded_logits(input_ids, position_ids), labels, B, S, teacher_logits, reference_logits)
+        return self._lm_output(self.padded_logits(input_ids, position_ids), labels, B, S, teacher_logits, reference_logits,
+                               preference_pairs)
 
     def padded_logits(self, input_ids: torch.Tensor, position_ids: Optional[torch.Tensor] = None) -> torch.Tensor:
         """The LM head's output ``[B*S, Vp]``, vocabulary padding included (a distillation teacher's logits)."""

@@ -135,8 +135,8 @@ from .norm import rmsnorm, add_rmsnorm, rmsnorm_ref, add_rmsnorm_ref, layernorm,
 from .rope import rope_qkv, rope_qkv_ref, apply_rope_ref, rope_tables  # noqa: E402
 from .embedding import embedding  # noqa: E402
 from .activation import swiglu, swiglu_ref, gelu_new, gelu_new_ref  # noqa: E402
-from .cross_entropy import (distill_cross_entropy, distill_cross_entropy_ref, dpo_loss, dpo_loss_ref, softmax_cross_entropy,  # noqa: E402
-                            softmax_cross_entropy_ref)
+from .cross_entropy import (distill_cross_entropy, distill_cross_entropy_ref, dpo_loss, dpo_loss_ref, orpo_loss, orpo_loss_ref,  # noqa: E402
+                            simpo_loss, simpo_loss_ref, softmax_cross_entropy, softmax_cross_entropy_ref)
 from .linear import linear, LinearFn  # noqa: E402
 from .attention import causal_attention, causal_attention_ref, rope_causal_attention, packed_causal_attention, segment_starts  # noqa: E402
 from .adam import fused_adamw_shard, grad_sumsq  # noqa: E402
@@ -149,6 +149,7 @@ __all__ = [
     "rope_qkv", "rope_qkv_ref", "apply_rope_ref", "rope_tables", "embedding",
     "swiglu", "swiglu_ref",
     "softmax_cross_entropy", "softmax_cross_entropy_ref", "distill_cross_entropy", "distill_cross_entropy_ref", "dpo_loss", "dpo_loss_ref",
+    "simpo_loss", "simpo_loss_ref", "orpo_loss", "orpo_loss_ref",
     "linear", "LinearFn",
     "causal_attention", "causal_attention_ref", "rope_causal_attention", "packed_causal_attention", "segment_starts",
     "fused_adamw_shard", "grad_sumsq",

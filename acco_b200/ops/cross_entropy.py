@@ -42,7 +42,26 @@ its positions whose (shifted) label is not -100::
 The forward makes one streaming pass over both rows and takes the per-token difference of the two log-probabilities before any
 sum, so equal policy and reference logits give ``z = 0`` exactly; a one-CTA reduction forms the loss and the per-row weights, and
 the backward writes the gradient in place over ``s``.  ``out`` (three fp32) receives the mean chosen reward ``beta (l - l_ref)(c)``,
-the mean rejected reward and the accuracy (fraction of valid pairs with ``z > 0``) on the device."""
+the mean rejected reward and the accuracy (fraction of valid pairs with ``z > 0``) on the device.
+
+:func:`simpo_loss` (SimPO, Meng et al. 2024; TRL ``CPOTrainer(loss_type="simpo")`` without the NLL term) and :func:`orpo_loss` (ORPO,
+Hong et al. 2024; TRL ``ORPOTrainer``) take the same pair layout and need no reference.  With ``a(row) = l(row) / |row|`` the mean
+log-probability of the row's response tokens and ``n`` the number of valid pairs::
+
+    SimPO:  z_i  = beta (a(c_i) - a(r_i)) - gamma,    loss = (1/n) sum_valid softplus(-z_i)
+            d s_tc = +-(beta sigma(-z_i) / (n |row|)) (softmax(s_t)_c - [c = y_t])
+    ORPO:   nll  = -(1/N_c) sum_valid l(c_i)    (N_c = sum_valid |c_i|)
+            lo_i = (a(c_i) - log(1 - e^a'(c_i))) - (a(r_i) - log(1 - e^a'(r_i))),   a' = min(a, -2^-20)
+            loss = nll + lambda (1/n) sum_valid softplus(-lo_i)
+            d s_tc = (1/N_c + lambda sigma(-lo_i) / (n |c_i| (1 - e^a'(c_i)))) (softmax - onehot)          (chosen)
+                     -(lambda sigma(-lo_i) / (n |r_i| (1 - e^a'(r_i)))) (softmax - onehot)                  (rejected)
+
+The clamp ``a'`` keeps ``log(1 - e^a)`` finite once the policy is certain of every response token (``a`` can reach 0, and in fp32
+even pass it); it is applied in the loss and, straight through, in the gradient.  No valid pair: loss 0 and gradient 0.  The forward
+is the cross-entropy's streaming pass (``lse`` and ``-log p`` per token) and one one-CTA reduction to the loss and a weight per row;
+the backward is DPO's, in place over ``s``.  ``out`` (three fp32) receives, on the device, SimPO's mean chosen reward ``beta a(c)``,
+mean rejected reward and accuracy (fraction of valid pairs with ``a(c) > a(r)``; gamma is not part of it), or ORPO's ``nll``, mean
+``lo`` and accuracy (fraction with ``lo > 0``)."""
 from __future__ import annotations
 
 import math
@@ -255,3 +274,130 @@ def dpo_loss(logits: torch.Tensor, ref_logits: torch.Tensor, labels: torch.Tenso
     if use_kernels(logits, ref_logits) and logits.dtype == torch.bfloat16:
         return _DPOFn.apply(logits, ref_logits.detach(), labels, P, int(V), beta, out)
     return dpo_loss_ref(logits, ref_logits, labels, P, V, beta, out)
+
+
+# ------------------------------------------------------------------------------------------------ SimPO / ORPO
+ORPO_MAX_MEAN_LOGP = -(2.0 ** -20)       # ORPO's clamp a' = min(a, -2^-20): log(1 - e^a') stays finite
+
+
+def _row_mean_logps(logits: torch.Tensor, labels: torch.Tensor, P: int, valid_vocab: int, ignore_index: int):
+    """Per row of the ``[2P, S]`` layout: ``l`` (sum of the response tokens' log-probabilities), the token count, ``a = l / count``
+    (0 on an empty row), and per pair whether both rows have a response token."""
+    V = int(valid_vocab)
+    x = logits[..., :V].float().reshape(-1, V)
+    lb = labels.reshape(-1)
+    mask = lb != ignore_index
+    idx = torch.where(mask, lb, torch.zeros_like(lb))[:, None]
+    lp = torch.log_softmax(x, -1).gather(1, idx)[:, 0]
+    l = torch.where(mask, lp, torch.zeros_like(lp)).view(2 * P, -1).sum(1)
+    cnt = mask.view(2 * P, -1).sum(1)
+    valid = (cnt[:P] > 0) & (cnt[P:] > 0)
+    return l, cnt, l / cnt.clamp(min=1), valid
+
+
+def log1m_exp(a: torch.Tensor) -> torch.Tensor:
+    """``log(1 - e^a)`` for ``a < 0``: ``log(-expm1(a))`` above ``-ln 2``, ``log1p(-exp(a))`` below (no cancellation on either side)."""
+    return torch.where(a > -math.log(2.0), torch.log(-torch.expm1(a)), torch.log1p(-torch.exp(a)))
+
+
+def orpo_log_odds(a: torch.Tensor) -> torch.Tensor:
+    """``a - log(1 - e^a')`` with ``a' = min(a, -2^-20)`` taken straight through: the value uses ``a'``, the gradient is
+    ``1 / (1 - e^a')`` whether or not the clamp is active."""
+    ac = a + (a.clamp(max=ORPO_MAX_MEAN_LOGP) - a).detach()
+    return a - log1m_exp(ac)
+
+
+def simpo_loss_ref(logits: torch.Tensor, labels: torch.Tensor, P: int, valid_vocab: int, beta: float, gamma: float,
+                   out: Optional[torch.Tensor] = None, ignore_index: int = -100) -> torch.Tensor:
+    """fp32 reference of :func:`simpo_loss` (the CPU and non-bf16 path)."""
+    P = int(P)
+    _, _, a, valid = _row_mean_logps(logits, labels, P, valid_vocab, ignore_index)
+    n = valid.sum().clamp(min=1)
+    rc, rr = beta * a[:P], beta * a[P:]
+    z = rc - rr - gamma
+    zero = torch.zeros_like(z)
+    loss = torch.where(valid, F.softplus(-z), zero).sum() / n
+    if out is not None:
+        vals = [torch.where(valid, v, zero).sum() / n for v in (rc.detach(), rr.detach(), (a[:P] > a[P:]).float())]
+        out.copy_(torch.stack(vals).reshape(out.shape))
+    return loss
+
+
+def orpo_loss_ref(logits: torch.Tensor, labels: torch.Tensor, P: int, valid_vocab: int, lam: float, out: Optional[torch.Tensor] = None,
+                  ignore_index: int = -100) -> torch.Tensor:
+    """fp32 reference of :func:`orpo_loss` (the CPU and non-bf16 path)."""
+    P = int(P)
+    l, cnt, a, valid = _row_mean_logps(logits, labels, P, valid_vocab, ignore_index)
+    n = valid.sum().clamp(min=1)
+    lo = orpo_log_odds(a[:P]) - orpo_log_odds(a[P:])
+    zero = torch.zeros_like(lo)
+    n_c = torch.where(valid, cnt[:P], torch.zeros_like(cnt[:P])).sum().clamp(min=1)
+    nll = -torch.where(valid, l[:P], zero).sum() / n_c
+    loss = nll + lam * torch.where(valid, F.softplus(-lo), zero).sum() / n
+    if out is not None:
+        vals = [nll.detach(), torch.where(valid, lo.detach(), zero).sum() / n, torch.where(valid, (lo.detach() > 0).float(), zero).sum() / n]
+        out.copy_(torch.stack(vals).reshape(out.shape))
+    return loss
+
+
+def _check_pref(logits: torch.Tensor, labels: torch.Tensor, P: int, coefs, out: Optional[torch.Tensor]) -> None:
+    """``coefs``: (name, value, strictly positive) of each hyper-parameter."""
+    for name, v, positive in coefs:
+        if isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v) or v < 0.0 or (positive and v == 0.0):
+            raise ValueError(f"{name} must be finite and {'>' if positive else '>='} 0, got {v!r}")
+    if out is not None and (out.numel() != 3 or out.dtype != torch.float32):
+        raise ValueError("out must be a three-element fp32 tensor")
+    rows = logits.reshape(-1, logits.shape[-1]).shape[0]
+    if P <= 0 or rows % (2 * P) != 0 or labels.numel() != rows:
+        raise ValueError(f"the preference loss needs 2 P S rows and one label per row, got {rows} rows, {labels.numel()} labels and P={P}")
+
+
+class _PrefFn(torch.autograd.Function):
+    """SimPO (``orpo`` false) or ORPO through ``pref_fwd``; the backward is DPO's in-place kernel with the per-row weights."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, P, valid_vocab, orpo, coef, gamma, out):
+        C = load_ext(required=True)
+        lg = logits.reshape(-1, logits.shape[-1])
+        assert lg.is_contiguous()
+        lb = labels.reshape(-1).contiguous()
+        if out is None:
+            out = torch.empty(3, device=lg.device, dtype=torch.float32)
+        loss, lse, w = C.pref_fwd(lg, lb, int(P), int(valid_vocab), -100, bool(orpo), float(coef), float(gamma), out)
+        count_launch("ce_fwd")
+        count_launch("pref_reduce")
+        ctx.save_for_backward(lg, lb, lse, w)
+        ctx.P, ctx.valid_vocab, ctx.shape = int(P), int(valid_vocab), logits.shape
+        return loss
+
+    @staticmethod
+    def backward(ctx, dloss):
+        C = load_ext(required=True)
+        lg, lb, lse, w = ctx.saved_tensors
+        C.dpo_bwd_inplace(lg, lb, lse, w, dloss.float().reshape(1).contiguous(), ctx.P, ctx.valid_vocab, -100)
+        count_launch("dpo_bwd")
+        return lg.view(ctx.shape), None, None, None, None, None, None, None
+
+
+def simpo_loss(logits: torch.Tensor, labels: torch.Tensor, P: int, V: int, beta: float, gamma: float,
+               out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The SimPO objective of ``P`` preference pairs laid out as ``2P`` rows of ``S`` tokens (chosen rows first); ``labels`` are the
+    shifted labels of the ``2P S`` rows, -100 off the responses.  ``out`` (three fp32), when given, receives the mean chosen reward,
+    the mean rejected reward and the accuracy.
+    NOTE (kernel path): ``logits`` is consumed - its storage is reused for the gradient during backward."""
+    P = int(P)
+    _check_pref(logits, labels, P, (("beta", beta, True), ("gamma", gamma, False)), out)
+    if use_kernels(logits) and logits.dtype == torch.bfloat16:
+        return _PrefFn.apply(logits, labels, P, int(V), False, float(beta), float(gamma), out)
+    return simpo_loss_ref(logits, labels, P, V, float(beta), float(gamma), out)
+
+
+def orpo_loss(logits: torch.Tensor, labels: torch.Tensor, P: int, V: int, lam: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The ORPO objective (the chosen responses' NLL plus ``lam`` times the mean odds-ratio loss) of ``P`` preference pairs in the
+    layout of :func:`simpo_loss`.  ``out`` (three fp32), when given, receives the NLL, the mean log odds ratio and the accuracy.
+    NOTE (kernel path): ``logits`` is consumed - its storage is reused for the gradient during backward."""
+    P = int(P)
+    _check_pref(logits, labels, P, (("lambda", lam, True),), out)
+    if use_kernels(logits) and logits.dtype == torch.bfloat16:
+        return _PrefFn.apply(logits, labels, P, int(V), True, float(lam), 0.0, out)
+    return orpo_loss_ref(logits, labels, P, V, float(lam), out)

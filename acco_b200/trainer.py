@@ -78,7 +78,14 @@ TRAIN_DEFAULTS: Dict[str, Any] = dict(
     distill_temperature=1.0,        # T > 0: temperature of both softmaxes in the KL
     dpo_beta=None,                  # beta > 0 (TRL's usual 0.1): DPO on preference pairs against a frozen reference; None: off
     dpo_reference=None,             # HF checkpoint dir of the frozen native reference (main.py: model.pretrained when unset)
+    simpo_beta=None,                # beta > 0 (e.g. 2.0): SimPO on preference pairs, no reference; None: off
+    simpo_gamma=0.5,                # gamma >= 0: SimPO's target reward margin
+    orpo_lambda=None,               # lambda > 0 (TRL's usual 0.1): ORPO (SFT + odds-ratio term) on preference pairs, no reference; None: off
 )
+
+# the three device scalars each reference-free preference objective logs (ops.simpo_loss / ops.orpo_loss `out`)
+PREF_SCALARS = {"simpo": ("simpo_reward_chosen", "simpo_reward_rejected", "simpo_accuracy"),
+                "orpo": ("orpo_nll", "orpo_log_odds", "orpo_accuracy")}
 
 
 class _Args:
@@ -171,6 +178,7 @@ class DecoupledTrainer:
         self._fused_smoothing = self._check_label_smoothing()
         self.z_loss_weight = self._check_z_loss()
         teacher_src = self._check_distill(teacher)
+        self.pref_objective = self._check_simpo_orpo(reference, teacher_src is not None)
         reference_src = self._check_dpo(reference, teacher_src is not None)
         if not isinstance(self.args.no_decay_1d, bool):
             raise ValueError(f"no_decay_1d must be true or false, got {self.args.no_decay_1d!r}")
@@ -185,6 +193,11 @@ class DecoupledTrainer:
         if self.reference is not None and self.rank == 0:
             self.log.info(f">>> DPO: beta={self.model.dpo_beta} on preference pairs, {self.batch_size} pairs = {2 * self.batch_size} rows "
                           f"per micro-batch (eval reports the same objective)")
+        if self.pref_objective is not None and self.rank == 0:
+            hp = f"beta={self.model.simpo_beta}, gamma={self.model.simpo_gamma}" if self.pref_objective == "simpo" else \
+                f"lambda={self.model.orpo_lambda}"
+            self.log.info(f">>> {self.pref_objective.upper()}: {hp} on preference pairs, no reference model, {self.batch_size} pairs = "
+                          f"{2 * self.batch_size} rows per micro-batch (eval reports the same objective)")
         if self._fused_smoothing and self.rank == 0:
             self.log.info(f">>> label_smoothing_factor={self._fused_smoothing}: smoothed inside the fused cross-entropy kernel "
                           f"of {type(self.model).__name__} (CUDA graphs stay available)")
@@ -224,6 +237,14 @@ class DecoupledTrainer:
         if self.reference is not None:
             self.model.dpo_out = self.dpo_static
         self.eval_dpo_accuracy: Optional[float] = None
+        # SimPO / ORPO: each micro-batch's three logged means (PREF_SCALARS), written on the device like the z-term
+        self.pref_static = torch.zeros(3, device=self.device, dtype=torch.float32)
+        self.pref_host = torch.zeros(3, dtype=torch.float32)
+        if self.is_cuda:
+            self.pref_host = self.pref_host.pin_memory()
+        if self.pref_objective is not None:
+            self.model.pref_out = self.pref_static
+        self.eval_pref_accuracy: Optional[float] = None
         self.n_grad_acc_ddp = 1
         self._hook_extra_microbatches: Optional[Callable[[int, int], int]] = None   # tests: (rank, round) -> extra
         self._nvtx = os.environ.get("ACCO_NVTX") == "1"
@@ -496,6 +517,48 @@ class DecoupledTrainer:
         self.model.dpo_beta = float(beta)
         return src
 
+    def _check_simpo_orpo(self, reference: Optional[nn.Module], distilling: bool) -> Optional[str]:
+        """Validates ``simpo_beta`` / ``simpo_gamma`` / ``orpo_lambda`` and returns the objective that is on ("simpo", "orpo") or None.
+        Like DPO it needs a native policy and preference pairs (checked in :meth:`_tokenize_if_needed`) and no other loss option; it
+        needs no reference, so a reference given with it is rejected."""
+        a = self.args
+        on = {k: getattr(a, k) for k in ("simpo_beta", "orpo_lambda") if getattr(a, k) is not None}
+        if not on:
+            return None
+        for key, v in on.items():
+            if isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v) or not v > 0.0:
+                raise ValueError(f"{key} must be a finite number > 0, got {v!r}")
+        gamma = a.simpo_gamma
+        if "simpo_beta" in on and (isinstance(gamma, bool) or not isinstance(gamma, (int, float)) or not math.isfinite(gamma) or gamma < 0.0):
+            raise ValueError(f"simpo_gamma must be a finite number >= 0, got {gamma!r}")
+        others = [k for k, v in (("dpo_beta", a.dpo_beta), ("distill_teacher", distilling)) if v is not None and v is not False]
+        if len(on) + len(others) > 1:
+            raise ValueError(f"at most one of dpo_beta, simpo_beta, orpo_lambda and distill_teacher may be set, got {sorted(on) + others}")
+        key = next(iter(on))
+        if reference is not None or a.dpo_reference is not None:
+            raise ValueError(f"{key} is reference-free: a reference= model or dpo_reference is meaningless with it")
+        from .models import NativeCausalLM
+        if not isinstance(self.model, NativeCausalLM):
+            raise ValueError(f"{key} needs a native policy (LlamaForCausalLM / GPTForCausalLM): the loss is computed inside their fused "
+                             f"kernels, and {type(self.model).__name__} has no such loss")
+        for what, v in (("label_smoothing_factor > 0", self.label_smoothing_factor), ("z_loss_weight > 0", self.z_loss_weight),
+                        ("packing", a.packing), ("document_mask", a.document_mask), ("const_len_batch", a.const_len_batch)):
+            if v:
+                raise ValueError(f"{key} cannot be combined with {what}: it trains on padded preference pairs, one sample per row, "
+                                 f"with its own loss")
+        if key == "simpo_beta":
+            self.model.simpo_beta, self.model.simpo_gamma, self.model.orpo_lambda = float(on[key]), float(gamma), None
+            return "simpo"
+        self.model.simpo_beta, self.model.orpo_lambda = None, float(on[key])
+        return "orpo"
+
+    @property
+    def _preference_key(self) -> Optional[str]:
+        """The key of the preference objective that is on (its data are preference pairs), or None."""
+        if self.args.dpo_beta is not None:
+            return "dpo_beta"
+        return {"simpo": "simpo_beta", "orpo": "orpo_lambda"}.get(self.pref_objective)
+
     def _setup_frozen(self, src, role: str, trained: str) -> Optional[nn.Module]:
         """The frozen ``role`` model (distillation teacher or DPO reference) on this rank's device in the trained model's weight dtype (a
         full copy per rank).  It is held by the trainer only, never by the trained model, so its parameters stay out of the arena,
@@ -537,7 +600,7 @@ class DecoupledTrainer:
                 self.eval_dataset = self.eval_dataset.map(self.preprocess_dataset_fn, batched=True)
         if self.train_dataset is None:
             return
-        if self.args.dpo_beta is not None:
+        if self._preference_key is not None:
             self.train_dataset = self._preference_pairs(self.train_dataset)
             if self.eval_dataset is not None:
                 self.eval_dataset = self._preference_pairs(self.eval_dataset)
@@ -562,13 +625,13 @@ class DecoupledTrainer:
             self._log_packing()
 
     def _preference_pairs(self, ds):
-        """DPO data: token columns ``prompt_ids`` / ``chosen_ids`` / ``rejected_ids`` as they are, or TRL's ``prompt`` / ``chosen`` /
-        ``rejected`` text columns tokenised; anything else is not preference data."""
+        """Preference data (DPO, SimPO, ORPO): token columns ``prompt_ids`` / ``chosen_ids`` / ``rejected_ids`` as they are, or TRL's
+        ``prompt`` / ``chosen`` / ``rejected`` text columns tokenised; anything else is not preference data."""
         cols = set(ds.column_names)
         if set(PREFERENCE_COLUMNS) <= cols:
             return ds
         if not {"prompt", "chosen", "rejected"} <= cols:
-            raise ValueError(f"dpo_beta needs preference pairs: columns prompt / chosen / rejected (text) or {' / '.join(PREFERENCE_COLUMNS)} "
+            raise ValueError(f"{self._preference_key} needs preference pairs: columns prompt / chosen / rejected (text) or {' / '.join(PREFERENCE_COLUMNS)} "
                              f"(token ids), got {sorted(cols)}")
         if self.tokenizer is None:
             raise ValueError("the preference dataset has text columns and no tokenizer was given")
@@ -595,7 +658,7 @@ class DecoupledTrainer:
             mult = 64 if self.is_cuda else 1        # few distinct padded lengths -> one CUDA graph per length
             if self.is_cuda and os.environ.get("ACCO_ATTN", "").lower() == "own":
                 mult = 128                          # the own attention kernels tile the sequence in blocks of 128
-        if self.args.dpo_beta is not None:
+        if self._preference_key is not None:
             return PreferenceCollator(pad_token_id=pad, max_length=int(self.args.max_length), pad_to_multiple_of=int(mult))
         return PadCollator(pad_token_id=pad, max_length=int(self.args.max_length), pad_to_multiple_of=int(mult))
 
@@ -740,6 +803,9 @@ class DecoupledTrainer:
                 t_logits = teacher.padded_logits(inputs["input_ids"], inputs.get("position_ids"))
             labels = inputs["labels"] if "labels" in inputs else inputs["input_ids"]
             out = model(**{k: v for k, v in inputs.items() if k != "labels"}, labels=labels, teacher_logits=t_logits)
+        elif self.pref_objective is not None:
+            # SimPO / ORPO: the [2P, S] pair rows score themselves, no frozen model runs
+            out = model(**inputs, preference_pairs=True)
         elif "labels" in inputs:
             out = model(**inputs)
         elif self._fused_smoothing:
@@ -958,6 +1024,8 @@ class DecoupledTrainer:
             self.distill_host.copy_(self.distill_static, non_blocking=non_blocking)
         if self.reference is not None:
             self.dpo_host.copy_(self.dpo_static, non_blocking=non_blocking)
+        if self.pref_objective is not None:
+            self.pref_host.copy_(self.pref_static, non_blocking=non_blocking)
 
     def _poll_phase_end(self) -> None:
         """The flip decision must be taken when the *device* reaches the end of the phase ("if the com finished ... else accumulate
@@ -1180,6 +1248,11 @@ class DecoupledTrainer:
                     gn["dpo_reward_chosen"], gn["dpo_reward_rejected"], gn["dpo_accuracy"] = (float(v) for v in self.dpo_host.tolist())
                     if eval_loss is not None and self.eval_dpo_accuracy is not None:
                         gn["eval_dpo_accuracy"] = self.eval_dpo_accuracy
+                if self.pref_objective is not None:                   # loss = the SimPO / ORPO objective
+                    names = PREF_SCALARS[self.pref_objective]
+                    gn.update(zip(names, (float(v) for v in self.pref_host.tolist())))
+                    if eval_loss is not None and self.eval_pref_accuracy is not None:
+                        gn[f"eval_{names[2]}"] = self.eval_pref_accuracy
                 log_training_scalars(self.writer, nb_step, sched.count_grad_tot, self.rank, loss, eval_loss, self.t_beg,
                                      extra={"lr": getattr(self, "_last_lr", 0.0), **gn})
                 self._fire("on_log", {"step": nb_step, "count_grad_tot": sched.count_grad_tot, "loss": loss,
@@ -1198,6 +1271,9 @@ class DecoupledTrainer:
                     if self.reference is not None:
                         gn_txt += (f" | dpo_reward_chosen {gn['dpo_reward_chosen']:.4g} | dpo_reward_rejected {gn['dpo_reward_rejected']:.4g}"
                                    f" | dpo_accuracy {gn['dpo_accuracy']:.3f}")
+                    if self.pref_objective is not None:
+                        c, r, acc = PREF_SCALARS[self.pref_objective]
+                        gn_txt += f" | {c} {gn[c]:.4g} | {r} {gn[r]:.4g} | {acc} {gn[acc]:.3f}"
                     pr.emit(sched.count_grad_tot, sched.count_com, loss, extra=f" | {rate:,.0f} tok/s/rank | lr {getattr(self, '_last_lr', 0.0):.3e}{gn_txt}")
                 self.epoch = pr.epoch
         if committed and plan is not None and self.callbacks:
@@ -1249,13 +1325,16 @@ class DecoupledTrainer:
     @torch.no_grad()
     def eval_loop(self) -> torch.Tensor:
         """Mean loss over this rank's eval shard (`trainer_decoupled.py:399-415`).  With DPO the loss is the DPO objective (reference
-        forward included) and ``eval_dpo_accuracy`` the mean accuracy over the eval micro-batches."""
+        forward included) and ``eval_dpo_accuracy`` the mean accuracy over the eval micro-batches; with SimPO / ORPO the loss is that
+        objective and ``eval_simpo_accuracy`` / ``eval_orpo_accuracy`` (``eval_pref_accuracy``) its mean accuracy."""
         self._ensure_gathered()
         self.model.eval()
         losses: List[torch.Tensor] = []
         accs: List[torch.Tensor] = []
         if self.reference is not None:
             self.model.dpo_out = torch.zeros(3, device=self.device, dtype=torch.float32)   # the training scalars stay as logged
+        if self.pref_objective is not None:
+            self.model.pref_out = torch.zeros(3, device=self.device, dtype=torch.float32)  # likewise
         ctx = torch.autocast(device_type=self.device.type, dtype=self.dtype) if self.autocast else contextlib.nullcontext()
         if self.z_loss_weight:
             self.model.z_loss_weight = 0.0          # eval loss stays pure cross-entropy, comparable with runs without the key
@@ -1270,16 +1349,23 @@ class DecoupledTrainer:
                     losses.append(loss.detach().float().reshape(1))
                 if self.reference is not None:
                     accs.append(self.model.dpo_out[2:].clone())
+                elif self.pref_objective is not None:
+                    accs.append(self.model.pref_out[2:].clone())
         finally:
             if self.z_loss_weight:
                 self.model.z_loss_weight = self.z_loss_weight
             if self.reference is not None:
                 self.model.dpo_out = self.dpo_static
+            if self.pref_objective is not None:
+                self.model.pref_out = self.pref_static
         self.model.train()
         if not losses:
             return torch.tensor(float("nan"))
         mean = torch.cat(losses).mean().cpu()
-        if accs:
+        if accs and self.pref_objective is not None:
+            self.eval_pref_accuracy = float(torch.cat(accs).mean())
+            self.log.info(f"eval loss {float(mean):.4f} | eval {PREF_SCALARS[self.pref_objective][2]} {self.eval_pref_accuracy:.3f}")
+        elif accs:
             self.eval_dpo_accuracy = float(torch.cat(accs).mean())
             self.log.info(f"eval loss {float(mean):.4f} | eval dpo_accuracy {self.eval_dpo_accuracy:.3f}")
         else:

@@ -66,6 +66,9 @@ KERNELS = {
     "dpo_fwd.sass": "_ZN4acco14dpo_fwd_kernelEPK13__nv_bfloat16S2_PKxPfS5_iix",
     "dpo_reduce.sass": "_ZN4acco17dpo_reduce_kernelEPKfPKxPfS4_S4_S4_iixf",
     "dpo_bwd.sass": "_ZN4acco14dpo_bwd_kernelEP13__nv_bfloat16PKxPKfS5_S5_iiix",
+    # SimPO / ORPO (train.simpo_beta / train.orpo_lambda): ce_fwd's pass, then this one-CTA reduction; the backward is dpo_bwd
+    "simpo_reduce.sass": "_ZN4acco18pref_reduce_kernelILi0EEEvPKfPKxPfS5_S5_S5_iixff",
+    "orpo_reduce.sass": "_ZN4acco18pref_reduce_kernelILi1EEEvPKfPKxPfS5_S5_S5_iixff",
 }
 MNEMONICS = ["HGMMA", "UTMALDG", "UTMALDG.2D.MULTICAST", "UTMASTG", "UTMACMDFLUSH", "SYNCS", "USETMAXREG", "REDG", "LDGMC", "HMMA", "MUFU.SQRT",
              "MUFU.EX2", "CCTL"]
