@@ -133,7 +133,9 @@ def _bf16_model(family):
 @pytest.mark.parametrize("family", ["llama", "gptneo"])
 def test_per_document_oracle_on_the_kernels(family):
     """Tolerances of the whole-model test of ``test_packing_gpu.py``: mean token loss within 3e-2, attention-weight gradients with
-    cosine similarity > 0.99.  The documents alone run the unsegmented path (SDPA), so the two sides share no attention code."""
+    cosine similarity > 0.99.  The documents alone run the unsegmented path (SDPA), so the two sides share no attention code.
+    The fp64 check of document-masked steps at training widths, tensor by tensor under the whole-step criterion, is
+    ``test_step_matrix_gpu.py``."""
     model, watched = _bf16_model(family)
     rows = doc_rows(ORACLE_LENS, np.random.default_rng(2), eos=999)
     batch = DocumentCollator(999)([{"input_ids": r} for r in rows])
